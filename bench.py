@@ -210,12 +210,35 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
+H100_HBM_GBS = 3350.0   # NVIDIA H100 SXM data sheet, HBM3
+
+
 def measured_peak_gbs():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return H100_HBM_GBS, "fallback (H100 SXM data sheet, 3.35 TB/s)"
+
+
+# --dump-outputs: the dense matrix (replicas x nodes, ~0.3 GB on cfg3) is sampled by rows, a fixed seed picks them;
+# the sample is written twice (scores, feasibility mask), so each copy gets half of the output budget
+DUMP_SCORE_BYTES = 24 << 20
+
+
+def timed_outputs(eng, handle, fetched, total_r, width):
+    """What a caller of the resident-plan path receives after a pass: the placement arrays and a seeded
+    sample of the dense score rows (this rank's column slab), for output-by-output comparison of two builds.
+    An infeasible node scores -inf in the matrix; the dump keeps every value finite by writing such entries as 0
+    in `scores` and 0 in `score_feasible` (1 elsewhere)."""
+    assign, status, domain = fetched
+    n = max(1, min(total_r, DUMP_SCORE_BYTES // (4 * max(1, width))))
+    rows = np.sort(np.random.default_rng(0).choice(total_r, size=n, replace=False))
+    scores = np.stack([eng.read_scores(handle, int(r)) for r in rows]).astype(np.float32)
+    feasible = scores != -np.inf
+    return {"assign": assign.astype(np.float64), "status": status.astype(np.float64),
+            "domain": domain.astype(np.float64), "score_rows": rows.astype(np.float64),
+            "scores": np.where(feasible, scores, np.float32(0)), "score_feasible": feasible.astype(np.float32)}
 
 
 class _DevPtr:
@@ -389,9 +412,10 @@ def make_device_step(D, eng, handles, n_waves, mode):
     return step
 
 
-def run_config(D, args, cfg_name, with_clocks):
+def run_config(D, args, cfg_name, with_clocks, dump=None):
     """Stages one configuration, checks it against the oracle, times the resident-plan leg
-    (`value`) and the host-buffer leg (`e2e`).  Returns the pieces of the JSON line."""
+    (`value`) and the host-buffer leg (`e2e`).  Returns the pieces of the JSON line; `dump` (a dict)
+    receives the outputs of the last timed step of each leg."""
     torch = D.torch
     from rbg_b200 import synth
     from rbg_b200.engine import TopoPlacer
@@ -490,6 +514,8 @@ def run_config(D, args, cfg_name, with_clocks):
         dev_ms = ev0.elapsed_time(ev1)
         launches = eng.stats()["kernel_launches"] - launches0
         post = [eng.fetch(h) for h in handles]
+        if dump is not None:   # every slot holds the same fleet (re-checked below when slots > 1)
+            dump.update(timed_outputs(eng, handles[0], post[0], total_r, hi - lo))
         if slots > 1:   # every slot holds the same fleet: the chained passes must leave what the checked pass left
             rows = sorted(set(int(i) for i in np.linspace(0, total_r - 1, 16)))
             ref_rows = [eng.read_scores(handles[0], r).copy() for r in rows]
@@ -631,6 +657,8 @@ def run_config(D, args, cfg_name, with_clocks):
         torch.cuda.synchronize()
         rounds.append((time.perf_counter() - t0) * 1e3)
     e2e_ms = D.max_over_ranks(sorted(rounds)[len(rounds) // 2])
+    if dump is not None:
+        dump.update({"e2e_" + k: np.asarray(v, dtype=np.float64) for k, v in zip(("assign", "status", "domain"), res)})
     if not churn:
         # the host-buffer entry point (direct path) against the staged plan the oracle checked above: assignment, status, domain
         assert all(np.array_equal(x, y) for x, y in zip(fetched, res)), "e2e placement differs from the staged path"
@@ -655,17 +683,8 @@ def run_config(D, args, cfg_name, with_clocks):
 def roofline_of(r, peak, peak_src):
     achieved = (r["algo_bytes"] / 1e9) / (r["score_ms"] * 1e-3) if r.get("score_ms") else 0.0
     step_frac = (r["algo_bytes"] / 1e9) / (r["ms_per_step"] * 1e-3) / peak if r.get("ms_per_step") else None
-    traffic = None
-    traffic_src = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "score_select_dram_bytes.json")) as f:
-            j = json.load(f)
-            traffic = j.get("dram_bytes_per_step")
-            traffic_src = "static_from_profile: " + str(j.get("source", "ncu --set full capture kept under profiles/"))
-    except Exception:
-        pass
     return {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-            "frac": achieved / peak if peak else None, "traffic": traffic, "traffic_source": traffic_src,
+            "frac": achieved / peak if peak else None,
             "kernel": "k_emit_rows (one launch per step and rank emits the dense rows of every wave)",
             "kernel_timing": "CUDA events recorded inside the library around every launch of the kernel, on the launching stream, "
                              "over a second leg of the same K steps (an event between the two kernels of a step serialises them: "
@@ -673,12 +692,9 @@ def roofline_of(r, peak, peak_src):
             "ms_per_step_kernel_timing": r.get("ms_per_step_kernel_timing"),
             "peak_source": peak_src, "algo_bytes_per_step": r["algo_bytes"], "kernel_ms_per_step": r["score_ms"],
             "kernel_launch_us": r.get("emit_launch_us"), "select_launch_us": r.get("select_launch_us"),
-            "frac_of_nominal_8000": achieved / 8000.0,
-            "frac_note": "the peak is the measured COPY bandwidth (reads + writes); a write-only stream can exceed it, and at the "
-                         "end of a launch part of the stream is still dirty in the 126 MB L2 (see traffic): "
-                         "dram_frac_in_kernel = traffic / kernel time / peak is the HBM rate inside the launch itself",
-            "dram_frac_in_kernel": (traffic / 1e9) / (r["score_ms"] * 1e-3) / peak if (traffic and r.get("score_ms") and peak
-                                                                                     and r.get("config_name") == "cfg3") else None,
+            "frac_of_datasheet": achieved / H100_HBM_GBS,
+            "frac_note": "algorithmic bytes, not DRAM traffic: at the end of a launch part of the write stream is still dirty "
+                         "in the 50 MB L2",
             "whole_step_frac": step_frac,
             "whole_step_note": "the same algorithmic bytes over ms_per_step (dense-matrix kernel + selection/greedy kernel)"}
 
@@ -686,7 +702,12 @@ def roofline_of(r, peak, peak_src):
 def run_ours(args):
     D = Dist(args)
     rank, world = D.rank, D.world
-    main = run_config(D, args, args.config, with_clocks=True)
+    dump = {} if (args.dump_outputs and rank == 0) else None
+    main = run_config(D, args, args.config, with_clocks=True, dump=dump)
+    if dump is not None:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, a in dump.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), a)
     alts = {}
     if args.alt:
         for name in ("cfg4", "cfg5"):
@@ -758,7 +779,7 @@ def run_ours(args):
                 "groups": main["groups"], "nodes": n_nodes, "edges": main["edges"], "replicas_per_step": main["total_r"],
                 "emit_matrix": True,
                 "l2": "dense-matrix write stream per step "
-                      f"({main['total_r'] * (hi - lo) * 4 / 1e6:.0f} MB) exceeds the 126 MB L2; inputs are L2-resident by design",
+                      f"({main['total_r'] * (hi - lo) * 4 / 1e6:.0f} MB) exceeds the 50 MB L2; inputs are L2-resident by design",
                 "slots": main.get("slots", 1),
                 "value_leg": ("" if main.get("slots", 1) == 1 else
                               f"{main.get('slots')} staged copies of the fleet (independent batches: own matrix, plan, outputs) re-placed round "
@@ -858,6 +879,9 @@ def main():
                     help="staged copies of the fleet re-placed round robin in the resident leg (independent batches, one per "
                          "step); > 1 chains the dense-matrix kernel of a step behind the selection kernel of the step before it")
     ap.add_argument("--soak", type=float, default=0.6, help="seconds of untimed identical steps before the timed region")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the main config's last timed step as DIR/<name>.npy (float32/float64, "
+                         "placements in full, a seeded sample of the dense score rows with its feasibility mask)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -7,7 +7,7 @@ Licensed under the Apache License, Version 2.0 (the "License").
 // Package b200topo is a third implementation of scheduler.PodGroupManager
 // (pkg/scheduler/podgroup_manager.go:64-78): it keeps the PodGroup CR bookkeeping of the wrapped
 // kube / volcano implementation and additionally computes topology-aware placement hints for the
-// group's pending replicas on a B200 through librbgtopo.so (include/rbgtopo.h).
+// group's pending replicas on an H100 through librbgtopo.so (include/rbgtopo.h).
 //
 // Wiring (the only edits to reference code, INTEGRATION.md §1):
 //
@@ -54,7 +54,7 @@ type Manager struct {
 	gids   gidTable   // dense group ids (domain_owner[] compares against them)
 }
 
-// New never fails: without a B200 (RBGTOPO_ENODEVICE) or without the library the manager degrades
+// New never fails: without an H100 (RBGTOPO_ENODEVICE) or without the library the manager degrades
 // to the wrapped implementation — the controller's behaviour today.
 func New(c client.Client, in inner) *Manager {
 	m := &Manager{client: c, inner: in, nodes: newNodeCache()}

@@ -1,5 +1,5 @@
 /*
- * rbgtopo.h — C ABI of the B200-native topology-aware placement engine for
+ * rbgtopo.h — C ABI of the H100-native topology-aware placement engine for
  * sgl-project/rbg RoleBasedGroups.
  *
  * This is the drop-in boundary (DESIGN.md §2). The reference has NO FFI for
@@ -44,7 +44,7 @@ extern "C" {
 /* ---- status codes ------------------------------------------------------ */
 #define RBGTOPO_OK          0
 #define RBGTOPO_EINVAL     -1  /* malformed argument / blob                     */
-#define RBGTOPO_ENODEVICE  -2  /* no CUDA device / wrong arch (needs sm_100)     */
+#define RBGTOPO_ENODEVICE  -2  /* no CUDA device / wrong arch (needs sm_90)      */
 #define RBGTOPO_ECUDA      -3  /* CUDA runtime error (text in last_error)       */
 #define RBGTOPO_EINEXACT   -4  /* input violates the fp32 exactness contract     */
 #define RBGTOPO_ENOTOPO    -5  /* score/assign called before set_topology        */
@@ -348,8 +348,8 @@ int32_t rbgtopo_set_stream(rbgtopo_ctx* ctx, void* cuda_stream);
  * resident while the last dense-matrix CTAs drain).  On: an event is recorded between the two kernels —
  * rbgtopo_last_timing / rbgtopo_last_pass_times then report each kernel, and the two kernels serialise
  * (what bench.py's roofline leg measures).  With timing off the passes of the resident entry points
- * (rbgtopo_run_staged) record no events at all (an event record between two kernels costs ~3 us of stream
- * time): rbgtopo_last_timing then reports the staging and the D2H only.  Initial value: environment
+ * (rbgtopo_run_staged) record no events at all (an event record between two kernels costs microseconds of
+ * stream time): rbgtopo_last_timing then reports the staging and the D2H only.  Initial value: environment
  * RBGTOPO_KERNEL_TIMING. */
 int32_t rbgtopo_set_kernel_timing(rbgtopo_ctx* ctx, int32_t on);
 

@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE ONLY: imported by tests/ (and nothing under rbg_b200/).
 Each function restates one Go function of sgl-project/rbg and cites it
-(paths relative to /root/reference).  These are O(#roles) scalar functions, so
+(paths relative to the reference checkout).  These are O(#roles) scalar functions, so
 plain Python is the right tool; Python ``float`` is IEEE-754 binary64 == Go
 ``float64`` and ``math.ceil/floor`` == ``math.Ceil/Floor``.  They are pinned by
 tests/test_refpinned_golden.py against every table the reference's own tests

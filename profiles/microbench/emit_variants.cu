@@ -1,7 +1,7 @@
 // Which feature of k_score_emit costs bandwidth?  Progressive variants on the
 // bench's output shape: 3072 steps (R = 1,5,1 per group-wave, wave-major) x 10000
-// nodes, row stride 10016 floats, 5 chunks of 2048 per step, 888 persistent CTAs
-// with byte-balanced contiguous ranges.
+// nodes, row stride 10016 floats, 5 chunks of 2048 per step, 6 / 12 / 16 persistent CTAs
+// per SM with byte-balanced contiguous ranges.
 //   V0 stores only            V1 + base/free loads + compare/select
 //   V2 + per-step header/role loads (dependent chain)   V3 = V2 with 128-thread CTAs
 #include <cstdio>
@@ -51,7 +51,9 @@ int main() {
   cudaMalloc(&steps, NS * sizeof(Step)); cudaMalloc(&roles, NS * 16);
   cudaMemcpy(steps, hs.data(), NS * sizeof(Step), cudaMemcpyHostToDevice); cudaMemcpy(roles, hr.data(), NS * 16, cudaMemcpyHostToDevice);
   cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
-  for (int grid : {888, 1776, 148 * 16}) {
+  int sm = 132;
+  cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, 0);
+  for (int grid : {sm * 6, sm * 12, sm * 16}) {
     std::vector<int> ci(grid + 1, ITEMS);
     long long total = (long long)TR * 5; int s = 0;
     for (int g = 0; g < grid; ++g) {

@@ -1,5 +1,5 @@
 // Write-stream microbenchmark: what does a pure float4 store stream reach on this
-// B200, for the two output sizes of the bench waves (41 MB: L2-resident, 205 MB)?
+// GPU, for the two output sizes of the bench waves (41 MB, 205 MB)?
 // Variants: store flavour (default / .cs / .wt), grid size, bytes per thread-iteration.
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -30,10 +30,12 @@ int main() {
   const size_t maxb = 256u << 20;
   cudaMalloc(&out, maxb); cudaMalloc(&base, 1 << 20); cudaMemset(base, 0, 1 << 20);
   cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
+  int sm = 132;
+  cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, 0);
   for (size_t mb : {41, 205}) {
     const int tiles = (int)(mb * 1000000 / 8192);
     for (int mode = 0; mode < 3; ++mode)
-      for (int grid : {148 * 4, 148 * 6, 148 * 8, 148 * 16, tiles}) {
+      for (int grid : {sm * 4, sm * 6, sm * 8, sm * 16, tiles}) {
         float best = 1e9;
         for (int it = 0; it < 6; ++it) {
           cudaEventRecord(a);

@@ -1,9 +1,9 @@
-// TMA bulk-store write-stream ceiling (round 2): can ONE small CTA per SM, staging 8 KB tiles in
+// TMA bulk-store write-stream ceiling: can ONE small CTA per SM, staging 8 KB tiles in
 // shared memory and issuing cp.async.bulk.global.shared::cta stores from one elected thread, keep
 // the HBM write stream of the dense-matrix kernel at its ceiling?  (k_score_emit's per-thread
-// st.global.cs.v4 stream needs 6 CTAs x 256 threads per SM and 62 % of the issue slots; a bulk-store
+// st.global.cs.v4 stream needs 6 CTAs x 256 threads per SM and most of the issue slots; a bulk-store
 // version leaves the SM to the selection kernel running beside it.)
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tma_fill tma_fill.cu && ./tma_fill
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tma_fill tma_fill.cu && ./tma_fill
 // Work = `tiles` tiles of TILE floats, each stored `reps` times to consecutive rows (the role row
 // broadcast to its replicas); segments are taken from a global atomic counter (dynamic balance).
 #include <cuda_runtime.h>
@@ -173,7 +173,7 @@ float run_tma(float* out, const float* base, int tiles, int reps, int* ctr, int 
 
 int main(int argc, char** argv) {
   const size_t bytes = argc > 1 ? (size_t)atoll(argv[1]) << 20 : (size_t)287 << 20;
-  int sm = 148;
+  int sm = 132;
   cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, 0);
   float *out, *base;
   int* ctr;

@@ -1,7 +1,7 @@
-"""rbg_b200 — B200-native topology-aware placement hot path for sgl-project/rbg.
+"""rbg_b200 — H100-native topology-aware placement hot path for sgl-project/rbg.
 
 Only what the path needs lives here (DESIGN.md §1):
-  csrc/      sm_100a CUDA kernels + the C-ABI runtime (librbgtopo.so, include/rbgtopo.h)
+  csrc/      sm_90a CUDA kernels + the C-ABI runtime (librbgtopo.so, include/rbgtopo.h)
   _lib.py    ctypes binding of the C ABI (fails loudly when the .so is missing)
   engine.py  thin object wrapper over a rbgtopo_ctx
   blob.py    builder of the batch wire format

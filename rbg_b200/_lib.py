@@ -1,5 +1,5 @@
 """ctypes binding of include/rbgtopo.h.  The shared library is built in-tree by
-``__graft_entry__.build()`` (nvcc, sm_100a).  A missing library is a hard error:
+``__graft_entry__.build()`` (nvcc, sm_90a).  A missing library is a hard error:
 this package has no CPU or PyTorch fallback."""
 from __future__ import annotations
 
@@ -98,7 +98,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc -gencode arch=compute_100a,code=sm_100a). rbg_b200 has no CPU fallback.")
+            "(nvcc -gencode arch=compute_90a,code=sm_90a). rbg_b200 has no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported

@@ -2,9 +2,9 @@
 // (DESIGN.md §4.2).  Default dense-matrix kernel of rbgtopo_place_groups / plan batches.
 //
 // k_score_emit<false, ETAB> (score.cuh) walks steps -> roles -> replicas; on fleets whose waves hold one
-// or two replicas per role (cfg3: 1 / 5 / 1 rows per step) that loop nest costs ~60 warp instructions
-// per 512-byte warp store (ncu: 34.0 M instructions for 561 K stores, 62 % issue-active) and the kernel is
-// issue-bound at 0.81 of the HBM peak, while the same kernel reaches 0.99 on cfg4 (8 replicas per role).
+// or two replicas per role (cfg3: 1 / 5 / 1 rows per step) that loop nest costs tens of warp instructions
+// per 512-byte warp store and the kernel is issue-bound below the HBM peak, while the same kernel comes
+// close to it on cfg4 (8 replicas per role).
 // Here the unit is the dense row: the plan's row table (kernels.cuh: rtab, written by k_plan_etab on the
 // device) says per row what the row needs — need, demand and, for exclusive rows only, the group — and the
 // inner loop is  LDS.64 record -> 2 x (4 FMUL + 4 ISETP + 4 FSEL + STG.128)  with nothing per step.

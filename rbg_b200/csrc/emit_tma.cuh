@@ -2,19 +2,19 @@
 // TMA bulk stores from shared memory (cp.async.bulk.global.shared::cta), DESIGN.md §4.2.
 //
 // Why a second emit kernel.  k_score_emit (score.cuh) streams the matrix with per-thread
-// st.global.cs.v4: it needs 6 CTAs x 256 threads per SM (61 K registers) and 62 % of the issue slots
+// st.global.cs.v4: it needs 6 CTAs x 256 threads per SM (61 K registers) and most of the issue slots
 // to keep HBM busy, so nothing else fits on the SM beside it — running the selection kernel
-// concurrently made the step SLOWER (99 us vs 91 us serial, profiles/README.md round 2).  Here one
-// elected lane issues a 2 KB bulk store per replica row and the TMA engine moves the bytes: 8 warps
-// per SM (one 256-thread CTA, 34 KB of shared memory) reach the same write bandwidth
-// (profiles/microbench/tma_fill.cu: 6.3 TB/s at 8 warps/SM vs 6.7 TB/s for the plain-store fill),
+// concurrently made the step slower than running the two in series.  Here one elected lane
+// issues a 2 KB bulk store per replica row and the TMA engine moves the bytes: 8 warps per SM
+// (one 256-thread CTA, 34 KB of shared memory) come close to the plain-store write bandwidth
+// (profiles/microbench/tma_fill.cu measures both),
 // and 3/4 of the SM's registers and shared memory are left for k_plan_group, which runs BESIDE this
 // kernel on a second stream.
 //
 // Structure: persistent grid (one CTA per SM), every WARP is an independent worker.
 //   item  = a sub-chunk of EMIT_SUB = 512 nodes of this rank's slab x a block of `bsteps` consecutive
-//           steps; items are taken from a global atomic counter (dynamic balance: a static split was
-//           18 % slower in round 1, the slowest SM sets the time), the index of the next item is
+//           steps; items are taken from a global atomic counter (dynamic balance: with a static split
+//           the slowest SM sets the time), the index of the next item is
 //           fetched while the current one is processed;
 //   setup = the sub-chunk's node operands (base, free: 16 floats / ints per lane) into registers and
 //           the steps' emit records (emit table: 12 words per step, written once when the batch is
@@ -84,7 +84,7 @@ __device__ __noinline__ void emit_tile_excl(const int* __restrict__ free_, const
 // ctr[0] = item queue, ctr[1] = warps that left the loop (the last one resets both for the next launch)
 // STAGES = ring depth per warp; MINB = __launch_bounds__ min blocks (4 caps the kernel at 64 registers so
 // that 6 CTAs of k_plan_group fit beside it); CLK = per-warp phase clocks into `clk` (profiling builds of
-// the launch: RBGTOPO_EMIT_CLOCKS, profiles/README.md), [warp][4] = setup, wait, compute, issue cycles.
+// the launch: RBGTOPO_EMIT_CLOCKS), [warp][4] = setup, wait, compute, issue cycles.
 template <int STAGES, int MINB, bool CLK>
 __global__ void __launch_bounds__(32 * EMIT_WARPS, MINB)
 k_emit_tma(TopoDev t, BatchDev b, const int* __restrict__ etab, int subs, int items, int* __restrict__ ctr,
@@ -159,8 +159,8 @@ k_emit_tma(TopoDev t, BatchDev b, const int* __restrict__ etab, int subs, int it
         if (CLK) { const long long c1 = clock64(); c_wait += c1 - c0; c0 = c1; }
         if (rexcl && excl_step) {
           // rare: exclusive role of an exclusive step — domains owned by another group are infeasible.
-          // Kept out of line so that the common path below stays ~60 instructions per tile (inlined and
-          // predicated off it cost ~200 issue slots per tile: ncu, profiles/README.md round 2).
+          // Kept out of line so that the common path below stays short (inlined and predicated off, it
+          // costs issue slots on every tile).
           emit_tile_excl<V>(t.free_, t.base, t.node_owner, st, n0, n1, gid, demand, need);
         } else {
 #pragma unroll

@@ -135,7 +135,7 @@ __device__ __forceinline__ void st_stream_f4(float* p, float4 v) {
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// ---- mbarrier + TMA 1-D bulk copy (cp.async.bulk), sm_90+/sm_100a ----------
+// ---- mbarrier + TMA 1-D bulk copy (cp.async.bulk), sm_90+ -----------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
 }
@@ -247,8 +247,8 @@ k_base(TopoDev t, const int2* __restrict__ tiles, int fmin_staged, int fmin_byte
 // ======================================================= background order, small snapshots
 // order[0 .. hi-lo) = the nodes [lo, hi) sorted by key(base[n], n) descending, for slabs of at most
 // ORDER_SMALL_MAX nodes: ONE CTA, bitonic network in shared memory (keys are unique, so the order is the
-// same total order a radix sort gives).  10 000 nodes: ~8 us instead of the ~40 us a 4-pass library radix
-// sort plus its key build / expansion kernels take at this size; larger slabs keep the library sort.
+// same total order a radix sort gives), instead of a 4-pass library radix sort plus its key build /
+// expansion kernels; larger slabs keep the library sort.
 constexpr int ORDER_SMALL_MAX = 16384;
 constexpr int ORDER_SMALL_THREADS = 1024;
 __global__ void __launch_bounds__(ORDER_SMALL_THREADS) k_order_sort_small(const float* __restrict__ base, int lo, int hi,

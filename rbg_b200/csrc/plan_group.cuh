@@ -75,7 +75,7 @@ __device__ __forceinline__ float gtab_delta(const GroupTab& T, const float* pair
   return d;
 }
 
-#ifdef RBGTOPO_PHASE_CLOCKS  // one-off instrumentation (profiles/README.md): per-CTA phase timestamps
+#ifdef RBGTOPO_PHASE_CLOCKS  // one-off instrumentation: per-CTA phase timestamps
 __device__ long long g_phase_clk[2048 * 32];
 __device__ int g_dbg_skip;  // timing experiments only: bit 0 = no corrections, bit 1 = no patched-slot pass
 __device__ long long g_cta_ns[2048 * 4];  // globaltimer at CTA start / end, table entries, SM id

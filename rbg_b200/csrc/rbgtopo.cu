@@ -3,7 +3,7 @@
 // multi-wave plan geometry (the plan itself is expanded on the device: plan.cuh),
 // slot pool, launches, timing.  Kernels: kernels.cuh (snapshot), score.cuh (dense
 // matrix), plan_group.cuh / select_fast.cuh / select.cuh (selection + greedy).
-// No CPU fallback exists: every entry point needs a CUDA device (sm_100).
+// No CPU fallback exists: every entry point needs a CUDA device (sm_90).
 #include <cuda_runtime.h>
 #include <cub/device/device_radix_sort.cuh>
 #include <nvtx3/nvToolsExt.h>
@@ -216,7 +216,7 @@ struct Batch {
 
 struct rbgtopo_ctx {
   rbgtopo_config cfg{};
-  int sm_count = 148;
+  int sm_count = 132;
   int slab_lo = 0, slab_hi = 0, slab_stride = 0, lc = 1, chunk = 2048;
   std::shared_mutex topo_mu;  // update = exclusive, score calls = shared
   uint64_t topo_epoch = 0;    // bumped by set_topology: handles staged against an older topology are stale
@@ -267,9 +267,8 @@ constexpr int kMaxExactTerm = 1 << 24;  // pair weights and anchor counts above 
 const bool kPerWavePlan = getenv("RBGTOPO_PER_WAVE_PLAN") != nullptr;  // one launch per wave instead of k_plan_group
 // Multi-wave plans, default: the dense-matrix kernel, then k_plan_group applying the corrections itself.
 // RBGTOPO_CONCURRENT_PLAN=1: k_plan_group (record mode: it never touches the matrix) on a second stream
-// beside the dense-matrix kernel, corrections applied afterwards by k_plan_correct.  Measured SLOWER on
-// B200 in every configuration tried (profiles/README.md round 2: the write stream inflates the latency of
-// the selection's dependent loads 3-4x and the two kernels fight for registers), so it is opt-in.
+// beside the dense-matrix kernel, corrections applied afterwards by k_plan_correct.  Opt-in: the write
+// stream inflates the latency of the selection's dependent loads and the two kernels fight for registers.
 const bool kSerialPlan = getenv("RBGTOPO_CONCURRENT_PLAN") == nullptr;
 const bool kNoPdl = getenv("RBGTOPO_NO_PDL") != nullptr;                // plain stream order between the two plan kernels
 const bool kKernelTimingEnv = getenv("RBGTOPO_KERNEL_TIMING") != nullptr;  // initial value of rbgtopo_set_kernel_timing
@@ -282,7 +281,7 @@ const bool kSelectFirst = getenv("RBGTOPO_SELECT_FIRST") != nullptr;  // launch 
 const int kSelectSmemKB = getenv("RBGTOPO_SELECT_SMEM_KB") ? std::max(0, atoi(getenv("RBGTOPO_SELECT_SMEM_KB"))) : 0;
 // Dense rows of a plan: k_score_emit<false> (per-thread streaming stores) by default; RBGTOPO_EMIT_TMA=1
 // selects k_emit_tma (TMA bulk stores from shared memory, 8 warps per SM): bit-identical, a quarter of the
-// footprint, but 58-64 us against 54 us on cfg3 (per-warp latency bound), see profiles/README.md round 2.
+// footprint, but slower on cfg3 (per-warp latency bound).
 const bool kEmitSt = getenv("RBGTOPO_EMIT_TMA") == nullptr;
 // Default among the streaming-store kernels: k_emit_rows (emit_rows.cuh, row-major walk of the plan's row
 // table, ~1/3 of the instructions per store); RBGTOPO_EMIT_STEPS=1 selects the step-major k_score_emit<false, ETAB>.
@@ -306,18 +305,18 @@ const int kEmitBlockSteps =
     getenv("RBGTOPO_EMIT_BLOCK") ? std::min(EMIT_MAX_BLOCK, std::max(1, atoi(getenv("RBGTOPO_EMIT_BLOCK")))) : 4;
 // place_groups can pipeline a fleet as two halves (host geometry of half 2 under the device work of
 // half 1).  Opt-in: at 1 024 groups it does not pay — the step is device-bound and the latency-bound
-// k_plan_group takes as long for half the groups as for all of them (profiles/README.md).
+// k_plan_group takes as long for half the groups as for all of them.
 const int kSplitMinGroups =
     getenv("RBGTOPO_SPLIT_MIN_GROUPS") ? std::max(2, atoi(getenv("RBGTOPO_SPLIT_MIN_GROUPS"))) : (1 << 30);
 const bool kCompactSortKey = getenv("RBGTOPO_WIDE_SORT_KEY") == nullptr;
 const bool kRefreshGraph = getenv("RBGTOPO_NO_REFRESH_GRAPH") == nullptr;
 // RBGTOPO_SMALL_SORT=1: single-CTA bitonic sort of the order for slabs <= 16 384 nodes instead of the library
-// radix sort.  Measured SLOWER (105 barrier rounds: ~150 us vs ~40 us at 10 000 nodes), kept opt-in.
+// radix sort.  Opt-in: 105 barrier rounds at 10 000 nodes make it slower than the radix sort.
 const bool kSmallSort = getenv("RBGTOPO_SMALL_SORT") != nullptr;
 const bool kVerifyPlan = getenv("RBGTOPO_VERIFY_PLAN") != nullptr;  // self-check: device-expanded plan == host-built plan
 const int kHostThreads = getenv("RBGTOPO_HOST_THREADS") ? std::max(1, atoi(getenv("RBGTOPO_HOST_THREADS"))) : 4;
-// With the per-shape caches a group costs ~50 ns of host time: below a few thousand groups an OpenMP region costs more
-// than it saves (94 us on one thread against 114 / 143 us on 2 / 4 for the 1 024-group bench fleet).
+// With the per-shape caches a group costs little host time: below a few thousand groups an OpenMP region costs more
+// than it saves (the 1 024-group bench fleet is faster on one thread than on 2 or 4).
 const int kHostParallelMinGroups = getenv("RBGTOPO_HOST_PARALLEL_MIN") ? std::max(1, atoi(getenv("RBGTOPO_HOST_PARALLEL_MIN"))) : 4096;
 
 // Events that only measure (staging, early emit, D2H, refresh) are recorded with kernel timing on or under
@@ -956,7 +955,7 @@ int run_batch(rbgtopo_ctx* c, Batch* b, int iters) {
     const bool early = b->early_emit;  // the staging enqueued this pass's dense-matrix kernel and its events already
     b->early_emit = false;
     // per-pass events only with kernel timing on (or for the pass the staging started): an event record between two
-    // kernels costs ~3 us of stream time on this stack, as much as it measures
+    // kernels costs microseconds of stream time, as much as it measures
     const bool timed = early ? b->tev : (b->passes < kMaxTimedPasses && c->kernel_timing.load(std::memory_order_relaxed));
     const int e0 = 3 * b->passes;
     if (timed && !early) {
@@ -1026,7 +1025,7 @@ int run_batch(rbgtopo_ctx* c, Batch* b, int iters) {
 // Pipeline of staged PLAN batches on one stream, ENQUEUE ONLY: `passes` passes, pass k over batch k % n.  Batches are
 // independent (own matrix, plan, outputs), so every dense-matrix kernel but the first is chained behind the selection
 // kernel of the batch before it as a programmatic dependent: its CTAs fill the SMs while the slowest groups of that
-// selection are still being placed (their CTA lifetimes spread over 20-30 us on cfg3), instead of after the launch gap.
+// selection are still being placed (their CTA lifetimes spread widely on cfg3), instead of after the launch gap.
 // Falls back to plain passes when the chain does not apply (kernel timing on, other dense-matrix kernels, world > 1's
 // per-wave paths, batches on different streams).
 int run_chain(rbgtopo_ctx* c, Batch** bs, int n, int passes) {
@@ -1307,8 +1306,8 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
   if (cfg->device < 0 || cfg->device >= ndev) return fail(RBGTOPO_ENODEVICE, "device %d of %d", cfg->device, ndev);
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10)
-    return fail(RBGTOPO_ENODEVICE, "device %d is sm_%d%d; kernels are built for sm_100a only", cfg->device,
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(RBGTOPO_ENODEVICE, "device %d is sm_%d%d; kernels are built for sm_90a only", cfg->device,
                 prop.major, prop.minor);
   CK(cudaSetDevice(cfg->device));
   auto c = std::make_unique<rbgtopo_ctx>();
@@ -2488,8 +2487,8 @@ int plan_geometry(const TopoHost& T, int lc, Batch* b, const int32_t* gb, int64_
   }
   // Launch order of k_plan_group: its CTAs all start at once and CTA i runs on SM (i mod #SMs) for the whole kernel,
   // so a fleet whose heavy groups recur with a period that divides the SM count (the bench fleet: every 4th group has
-  // 3 scheduled pods, 148 = 4 * 37) piles the heavy groups onto the same SMs and the slowest SM sets the kernel time
-  // (per-SM end times 20-30 us, profiles/README.md).  Groups are dealt in descending order of their expected table size
+  // 3 scheduled pods, 132 = 4 * 33) piles the heavy groups onto the same SMs and the slowest SM sets the kernel
+  // time.  Groups are dealt in descending order of their expected table size
   // (neighbourhoods of the scheduled pods + of the replicas to place): every SM gets one group of every weight stratum.
   {
     int32_t* const perm = poff + ns + 1;
@@ -2598,7 +2597,7 @@ int plan_stage(rbgtopo_ctx* c, Batch* b, const int32_t* gb, int64_t words, bool 
     return RBGTOPO_OK;
   };
   b->early_emit = false;
-  // The upload of the GROUPS blob does not wait for its validation: ~15 us of PCIe time under the host's check + numbering
+  // The upload of the GROUPS blob does not wait for its validation: its PCIe time hides under the host's check + numbering
   b->prestaged_h = nullptr;
   b->prestaged_d = nullptr;
   if (early_emit && !dev_groups && g_lo == 0 && words >= RBGTOPO_HDR_WORDS && !b->h_in.pageable && (size_t)words <= b->h_in.cap &&
@@ -2780,7 +2779,7 @@ namespace {
 // it is validated: bytes only), the host validates every group, checks the exactness bound and collects a handful of
 // maxima (per-shape caches: a fleet repeats a few templates), k_group_rtab derives the row table, k_emit_rows writes the
 // dense matrix and k_plan_group<true> — a programmatic dependent of it — replays each group's waves from its role
-// table.  8 CUDA calls and ~50 us of host time per call instead of ~20 calls and ~115 us (DESIGN.md §4.4).
+// table.  8 CUDA calls per call instead of ~20, and less than half the host time (DESIGN.md §4.4).
 // Used with the default kernels (any world: selection is replicated); *handled = false -> the caller takes the staged
 // path (plan_stage).
 const bool kNoDirect = getenv("RBGTOPO_NO_DIRECT") != nullptr;
@@ -3174,7 +3173,7 @@ int32_t rbgtopo_place_groups(rbgtopo_ctx* c, const int32_t* gb, int64_t words, i
     Batch* b = nullptr;
     int rc = handled ? RBGTOPO_OK : acquire_batch(c, &b);
     if (rc) return rc;
-    static const bool no_early = getenv("RBGTOPO_NO_EARLY_EMIT") != nullptr;  // A/B switch (profiles/README.md)
+    static const bool no_early = getenv("RBGTOPO_NO_EARLY_EMIT") != nullptr;  // A/B switch
     if (handled) {
       // results and dirty groups are in place: the host loop for the latter follows below, outside the lock
     } else if (!split) {

@@ -160,7 +160,7 @@ def test_node_axis_sharding_matches_oracle(tmp_path):
     if ngpu < 2:
         # One GPU: NCCL needs one device per rank, so the same protocol runs with both ranks as contexts of this
         # device and a device copy as the all-gather (tests/test_gpu_shard_single.py) — same library entry points,
-        # same oracle checks; the NCCL transport itself is exercised on the >= 2-GPU boxes (profiles/README.md).
+        # same oracle checks; the NCCL transport itself is exercised on machines with >= 2 GPUs.
         import test_gpu_shard_single as single
         single.test_step_batches_sharded_on_one_device(2)
         single.test_group_plans_sharded_on_one_device(2)
