@@ -11,7 +11,9 @@ It restates, independently of rbg_b200/plugin.py and rbg_b200/blob.py:
   * the wave rule of DESIGN.md §3.2 (a wave = the next <= 32 replicas of <= 8 roles of one level);
   * the pair matrix (same role, dependency edge, shared CoordinatedPolicy rule) and
     need_rho = min(16, still-unplaced replicas of the paired roles);
-  * the BLOB wire format of include/rbgtopo.h (one contiguous int32 array);
+  * the BLOB wire format of include/rbgtopo.h (one contiguous int32 array), and the GROUPS wire
+    format it reads back (groups_from_blob: a raw GROUPS blob with explicit levels, pair weights and
+    anchor counts runs through the same loop);
   * the feedback of a wave's placements into the next (anchors, consumed capacity, the fixed
     exclusive domain, gang all-or-nothing over the group: k8s-scheduler-plugin/manager.go:131).
 Parity of the placements themselves is UNPINNED upstream (oracle/placer_oracle.c header).
@@ -48,9 +50,11 @@ class OGroup:
     rules: List[Sequence[str]] = field(default_factory=list)   # CoordinatedPolicy role sets
     exclusive: bool = False
     gang: bool = False
-    placed: List[Tuple[str, int]] = field(default_factory=list)   # (role, node) of scheduled pods
+    placed: List[Tuple] = field(default_factory=list)   # (role, node) or (role, node, count) of scheduled pods
     fixed_domain: int = -1
     current: Dict[str, int] = field(default_factory=dict)         # replicas that already exist
+    pair: Optional[Sequence[Sequence[int]]] = None   # explicit [Q][Q] weights instead of the host rule
+    levels: Optional[Sequence[int]] = None           # explicit level per role: roles taken in the given order
 
 
 def build_blob(steps: List[dict]) -> np.ndarray:
@@ -100,24 +104,34 @@ class GroupState:
         roles = g.roles
         self.Q = len(roles)
         index = {r.name: i for i, r in enumerate(roles)}
-        pair = np.eye(self.Q, dtype=np.int64)
-        for i, r in enumerate(roles):
-            for d in r.deps:
-                pair[i, index[d]] = pair[index[d], i] = 1
-        for rule in g.rules:
-            ids = [index[x] for x in rule if x in index]
-            for a in ids:
-                for b in ids:
-                    pair[a, b] = 1
+        if g.pair is not None:
+            pair = np.asarray(g.pair, dtype=np.int64).reshape(self.Q, self.Q)
+        else:
+            pair = np.eye(self.Q, dtype=np.int64)
+            for i, r in enumerate(roles):
+                for d in r.deps:
+                    pair[i, index[d]] = pair[index[d], i] = 1
+            for rule in g.rules:
+                ids = [index[x] for x in rule if x in index]
+                for a in ids:
+                    for b in ids:
+                        pair[a, b] = 1
         self.pair = pair
-        levels = refpinned.dependency_order({r.name: list(r.deps) for r in roles})
+        if g.levels is not None:               # consecutive roles of equal level form a level
+            levels: List[List[str]] = []
+            for i, r in enumerate(roles):
+                if i == 0 or g.levels[i] != g.levels[i - 1]:
+                    levels.append([])
+                levels[-1].append(r.name)
+        else:
+            levels = refpinned.dependency_order({r.name: list(r.deps) for r in roles})
         self.first = [g.current.get(r.name, 0) for r in roles]
         self.pending = [max(r.replicas - g.current.get(r.name, 0), 0) for r in roles]
         self.unplaced = list(self.pending)
         self.anchors: Dict[Tuple[int, int], int] = {}
-        for role_name, node in g.placed:
-            k = (int(node), index[role_name])
-            self.anchors[k] = self.anchors.get(k, 0) + 1
+        for pod in g.placed:
+            k = (int(pod[1]), index[pod[0]])
+            self.anchors[k] = self.anchors.get(k, 0) + (int(pod[2]) if len(pod) > 2 else 1)
         self.consumed: Dict[int, int] = {}
         self.fixed_domain = g.fixed_domain
         self.failed = False
@@ -197,7 +211,7 @@ class GroupState:
 
 
 def run_fleet(topo, groups: Sequence[OGroup], nthreads: int = 1, want_matrix: bool = False,
-              on_wave: Optional[Callable] = None, reuse_matrix: bool = False):
+              on_wave: Optional[Callable] = None, reuse_matrix: bool = False, want_topk: bool = False):
     """Level-synchronous wave loop over the CPU oracle.  Returns (states, blobs).
     on_wave(w, active_states, blob, oracle_result) is called after every wave (before absorb)."""
     states = [GroupState(g) for g in groups]
@@ -209,7 +223,7 @@ def run_fleet(topo, groups: Sequence[OGroup], nthreads: int = 1, want_matrix: bo
             break
         blob = build_blob([s.step(w) for s in active])
         blobs.append(blob)
-        r = oracle_placer.place(topo, blob, want_matrix=want_matrix, want_topk=False, nthreads=nthreads,
+        r = oracle_placer.place(topo, blob, want_matrix=want_matrix, want_topk=want_topk, nthreads=nthreads,
                                 reuse_matrix=reuse_matrix)
         if r["rc"] != 0:
             raise RuntimeError(f"oracle rc={r['rc']} in wave {w}")
@@ -222,3 +236,28 @@ def run_fleet(topo, groups: Sequence[OGroup], nthreads: int = 1, want_matrix: bo
             off += cnt
         w += 1
     return states, blobs
+
+
+GROUPS_MAGIC, GROUP_WORDS = 0x47474252, 12
+
+
+def groups_from_blob(gblob) -> List[OGroup]:
+    """The groups of a GROUPS blob (include/rbgtopo.h, GROUPS section) as OGroups: roles in the blob's order with
+    their levels, pending counts, demands and exclusive flags, the pair matrix as given, the anchors with their
+    counts (repeated (node, role) records add up), the fixed domain and the gang / exclusive flags.  Role r of
+    group i is named "r<r>" and its pending replicas get ordinals 0.., the group is named "g<i>"."""
+    b = np.asarray(gblob, dtype=np.int64)
+    if len(b) < HDR_WORDS or b[0] != GROUPS_MAGIC or b[1] != VERSION or b[3] != len(b):
+        raise ValueError("not a GROUPS blob")
+    out: List[OGroup] = []
+    for i in range(int(b[2])):
+        gid, flags, fixed, q, role_off, pair_off, na, anchor_off = (int(x) for x in b[HDR_WORDS + i * GROUP_WORDS:][:8])
+        rt = b[role_off:role_off + 4 * q].reshape(q, 4)
+        roles = [ORole(f"r{r}", int(rt[r, 1]), demand=int(rt[r, 2]), exclusive=bool(rt[r, 3] & ROLE_EXCLUSIVE))
+                 for r in range(q)]
+        pair = b[pair_off:pair_off + q * q].reshape(q, q).tolist()
+        at = b[anchor_off:anchor_off + 3 * na].reshape(na, 3)
+        placed = [(f"r{int(a[1])}", int(a[0]), int(a[2])) for a in at]
+        out.append(OGroup(f"g{i}", gid, roles, exclusive=bool(flags & STEP_EXCLUSIVE), gang=bool(flags & STEP_GANG),
+                          placed=placed, fixed_domain=fixed, pair=pair, levels=[int(x) for x in rt[:, 0]]))
+    return out

@@ -322,7 +322,8 @@ def test_plan_variants_in_a_subprocess(var):
     RBGTOPO_EMIT_STEPS: the step-major dense-matrix kernel (k_score_emit<false, ETAB>) instead of k_emit_rows.
     RBGTOPO_KERNEL_TIMING / RBGTOPO_NO_PDL: an event between the two plan kernels / plain stream order instead of the
     programmatic dependent launch.  RBGTOPO_EMIT_ROWS=1: one row per segment of k_emit_rows (the smallest segment).
-    RBGTOPO_NO_DIRECT: rbgtopo_place_groups through the staged path (expanded plan, early emit) that world > 1 takes."""
+    RBGTOPO_NO_DIRECT: rbgtopo_place_groups through the staged path (expanded plan, early emit) that world > 1 takes.
+    Each variant runs this file and tests/test_gpu_groups_limits.py (8-role waves, 16-role groups, ragged node counts)."""
     import os
     import subprocess
     import sys
@@ -332,7 +333,8 @@ def test_plan_variants_in_a_subprocess(var):
     for v in var.split("+"):
         env[v] = "1"
     r = subprocess.run(
-        [sys.executable, "-m", "pytest", "tests/test_gpu_groups.py", "-q", "-m", "gpu", "-x", "-k", "not subprocess"],
+        [sys.executable, "-m", "pytest", "tests/test_gpu_groups.py", "tests/test_gpu_groups_limits.py", "-q", "-m", "gpu", "-x",
+         "-k", "not subprocess"],
         cwd=root, env=env, capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]
     assert "passed" in r.stdout

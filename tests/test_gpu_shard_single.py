@@ -166,6 +166,42 @@ def test_group_plans_sharded_on_one_device(world):
             e.release(h)
         for e in engs:
             e.close()
+    # a generated fleet at the limits of the GROUPS ABI (8-role waves, 16-role groups, weighted pairs, N % 4 != 0)
+    import groups_gen as gg
+    from test_gpu_groups_limits import group_slices, oracle_plan
+    case = gg.make_case(14, 2049)
+    states, _ = oracle_plan(case.topo, case.blob)
+    engs = _engines(case.topo, world)
+    hs = [e.stage_groups(case.blob) for e in engs]
+    for w in range(engs[0].shard_waves(hs[0])):
+        allk = _gather([e.shard_wave_score(h, w) for e, h in zip(engs, hs)])
+        m = [e.shard_wave_merge(h, w, allk.data_ptr()) for e, h in zip(engs, hs)]
+        all2 = _gather([(x[1], x[2]) for x in m]) if m[0][0] else None
+        for e, h in zip(engs, hs):
+            e.shard_wave_assign(h, w, all2.data_ptr() if all2 is not None else None)
+    res = [e.fetch(h) for e, h in zip(engs, hs)]
+    for r, (assign, status, domain) in enumerate(res):
+        for i, (st, sl) in enumerate(zip(states, group_slices(states))):
+            want = st.result()
+            if want["status"] == 1:   # left to the host loop by the plan: status only
+                assert status[i] == 1, (world, r, i)
+                continue
+            assert assign[sl].tolist() == st.assign_in_group_order(), (world, r, i)
+            assert (status[i], domain[i]) == (want["status"], want["domain"]), (world, r, i)
+    for e, h in zip(engs, hs):
+        e.release(h)
+    for r, e in enumerate(engs):
+        h = e.stage_groups(case.blob)
+        e.run_staged(h, 1)
+        a2, s2, d2 = e.fetch(h)
+        assert np.array_equal(a2, res[0][0]) and np.array_equal(s2, res[0][1]) and np.array_equal(d2, res[0][2]), (world, r)
+        e.release(h)
+        a4, s4, d4 = e.place_groups(case.blob)
+        for i, (st, sl) in enumerate(zip(states, group_slices(states))):
+            want = st.result()
+            assert a4[sl].tolist() == st.assign_in_group_order() and (s4[i], d4[i]) == (want["status"], want["domain"]), (world, r, i)
+    for e in engs:
+        e.close()
 
 
 def _connect_p2p(engs):

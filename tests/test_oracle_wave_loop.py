@@ -25,6 +25,13 @@ def test_wave_blobs_and_results_match_the_plugin_mirror(shape, n_groups, n):
     for st, r in zip(states, ref):
         res = st.result()
         assert res["nodes"] == r.nodes and res["status"] == r.status and res["domain"] == r.domain
+    # the plugin's own GROUPS blob, decoded by the oracle alone (explicit levels, pair matrix, anchor counts)
+    gblob, _ = B200TopoPodGroupManager(pl).groups_blob(bench.to_plugin(specs))
+    decoded, _ = wave_loop.run_fleet(topo, wave_loop.groups_from_blob(gblob))
+    for st, d in zip(states, decoded):
+        assert d.assign_in_group_order() == st.assign_in_group_order()
+        assert (d.result()["status"], d.result()["domain"]) == (st.result()["status"], st.result()["domain"])
+        assert [[c for _, _, c in w] for w in d.waves] == [[c for _, _, c in w] for w in st.waves]
 
 
 def test_big_gang_exclusive_groups():

@@ -103,3 +103,28 @@ def test_plan_describe_rejects_what_place_groups_rejects():
     assert rc == -1
     # exactness bound: heavy rows make the scores leave the exact fp32 range
     assert describe(blob, wsum_max=10 ** 7)[0] == -4
+
+
+@pytest.mark.parametrize("seed,n", [(s, n) for s, n, _, _ in __import__("groups_gen").CASES] + [(20 + s, 512) for s in range(6)])
+def test_oracle_wave_split_matches_plan_describe_at_the_abi_limits(seed, n):
+    """Generated GROUPS blobs (16-role groups, levels of 9+ pending roles, waves of exactly 8 role rows / 32 replicas,
+    zero-pending roles and levels): the oracle's wave decomposition of the raw blob equals the host plan geometry step by
+    step — (group, wave) in wave-major order, first dense row, first role row, replicas of the earlier waves."""
+    import groups_gen as gg
+    from oracle import wave_loop
+    case = gg.make_case(seed, n, scarce=seed % 2 == 0)
+    states = [wave_loop.GroupState(g) for g in wave_loop.groups_from_blob(case.blob)]
+    rc, steps, n_waves, _ = describe(case.blob, n_nodes=case.topo.n, n_domains=len(case.topo.domain_owner))
+    assert rc == 0
+    assert n_waves == max(len(st.waves) for st in states)
+    exp, role_row = [], 0
+    group_off = np.cumsum([0] + [sum(st.pending) for st in states])
+    for w in range(n_waves):
+        for gi, st in enumerate(states):
+            if w < len(st.waves):
+                i0 = sum(c for wave in st.waves[:w] for _, _, c in wave)
+                exp.append((gi, w, int(group_off[gi]) + i0, role_row, i0))
+                role_row += len(st.waves[w])
+    got = [(int(s[0]), int(s[1]), int(s[4]), int(s[5]), int(s[7])) for s in steps]
+    assert got == exp
+    assert any(len(wave) == 8 for st in states for wave in st.waves)
