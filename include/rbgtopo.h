@@ -282,6 +282,19 @@ int32_t rbgtopo_read_scores(rbgtopo_ctx* ctx, int32_t handle, int32_t row,
 int32_t rbgtopo_read_topk(rbgtopo_ctx* ctx, int32_t handle, int32_t rolerow,
                           uint64_t* out_keys, int32_t k);
 
+/* Diagnostics / tests: copy one per-snapshot vector of the current snapshot to the host once the refresh
+ * that produced it has completed, exactly as the device holds it.  what = RBGTOPO_SNAP_BASE (float[n]),
+ * RBGTOPO_SNAP_ORDER (uint64[slab], key(base, node) form), RBGTOPO_SNAP_ORDER_ALL (uint64[n]; the same
+ * buffer as ORDER when world == 1), RBGTOPO_SNAP_POS (int32[n], world == 1 only),
+ * RBGTOPO_SNAP_DELTA_REPAIRS (int64[1]: incremental repairs since the last set_topology).  *n_out (may be
+ * NULL) receives the element count, also when out_bytes is too small; then RBGTOPO_EINVAL is returned. */
+#define RBGTOPO_SNAP_BASE          0
+#define RBGTOPO_SNAP_ORDER         1
+#define RBGTOPO_SNAP_ORDER_ALL     2
+#define RBGTOPO_SNAP_POS           3
+#define RBGTOPO_SNAP_DELTA_REPAIRS 4
+int32_t rbgtopo_read_snapshot(rbgtopo_ctx* ctx, int32_t what, void* out, int64_t out_bytes, int64_t* n_out);
+
 /* ---- node-axis sharding over `world` GPUs (SURVEY.md §8e) --------------- *
  * rank g scores columns [slab_lo, slab_hi) and selects a local top-K; the
  * caller all-gathers the key lists (NCCL, one collective per pass) and every

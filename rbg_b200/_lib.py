@@ -47,6 +47,7 @@ SIGNATURES = {
     "rbgtopo_release": (C.c_int32, [C.c_void_p, C.c_int32]),
     "rbgtopo_read_scores": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, f32p, C.c_int32]),
     "rbgtopo_read_topk": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, u64p, C.c_int32]),
+    "rbgtopo_read_snapshot": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]),
     "rbgtopo_shard_waves": (C.c_int32, [C.c_void_p, C.c_int32, i32p]),
     "rbgtopo_shard_wave_score": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]),
     "rbgtopo_shard_wave_merge": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, i32p, C.POINTER(C.c_void_p),

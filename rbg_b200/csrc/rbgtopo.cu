@@ -256,6 +256,7 @@ struct rbgtopo_ctx {
   rbgtopo_timing last{};
   std::vector<float> last_score_ms, last_select_ms;  // per pass, harvested by the last fetch (rbgtopo_last_pass_times)
   long long calls = 0, scores_total = 0, launches = 0;
+  long long delta_repairs = 0;  // incremental repairs of update_nodes_delta since the last set_topology
   // occupancy of k_plan_group: per instantiation (DIRECT) the launch shape last asked about and its CTAs per SM;
   // the last launch's grid and CTAs per SM (rbgtopo_plan_occupancy)
   struct PlanOcc { int nth = 0; size_t smem = 0; int per_sm = 0; } plan_occ[2];
@@ -410,7 +411,10 @@ int prepare_refresh(rbgtopo_ctx* c) {
   {  // compact sort key: node bits + bits of the largest possible base = (wsum_max + self) * F
     auto bits = [](unsigned long long v) { int b = 0; while (v) { ++b; v >>= 1; } return std::max(1, b); };
     const int nb = bits((unsigned long long)std::max(1, T.n - 1));
-    const int bb = bits((unsigned long long)(T.wsum_max + RBGTOPO_SELF_W) * RBGTOPO_F_CAP);
+    // From 2^24 on, base is an fp32 sum that is no longer exact (such a snapshot only admits need = 0 steps): a
+    // rounded sum can reach the power of two above the bound (bound 2^28 - 8 sums to 2^28), so reserve one more bit.
+    const unsigned long long bound = (unsigned long long)(T.wsum_max + RBGTOPO_SELF_W) * RBGTOPO_F_CAP;
+    const int bb = bits(bound) + (bound >= (1ull << 24) ? 1 : 0);
     if (kCompactSortKey && nb + bb <= 62 && nb <= 31) {
       T.key_nb = nb;
       T.key_bits = nb + bb;
@@ -1512,6 +1516,7 @@ int32_t rbgtopo_set_topology(rbgtopo_ctx* c, int32_t n, int64_t e, const int32_t
     T.max_degp1 = std::max(T.max_degp1, T.h_degp1[i]);
   }
   T.refresh_ready = false;  // new sizes / pointers: re-capture the refresh chain
+  c->delta_repairs = 0;
   int rc = run_base(c, c->topo_stream, true);
   if (rc) return rc;
   T.valid = true;
@@ -1630,6 +1635,7 @@ int32_t rbgtopo_update_nodes_delta(rbgtopo_ctx* c, int32_t n_changed, const int3
   if (tev) CK(cudaEventRecord(c->ev_base_b, s));
   CK(cudaEventRecord(c->topo_ready, s));
   c->base_timing_pending = tev;
+  c->delta_repairs += 1;
   CK(cudaGetLastError());
   std::lock_guard<std::mutex> g(c->stat_mu);
   c->launches += 3;
@@ -3477,6 +3483,40 @@ int32_t rbgtopo_read_topk(rbgtopo_ctx* c, int32_t handle, int32_t rolerow, uint6
   CK(cudaSetDevice(c->cfg.device));
   CK(cudaStreamSynchronize(stream_of(c, b)));
   CK(cudaMemcpy(out, b->merged.p + (size_t)rolerow * KS, (size_t)k * 8, cudaMemcpyDeviceToHost));
+  return RBGTOPO_OK;
+}
+
+// The device buffer as it is: nothing is recomputed or re-sorted, so a stale or wrong vector shows.
+int32_t rbgtopo_read_snapshot(rbgtopo_ctx* c, int32_t what, void* out, int64_t out_bytes, int64_t* n_out) {
+  if (!c) return fail(RBGTOPO_EINVAL, "null ctx");
+  std::shared_lock<std::shared_mutex> lk(c->topo_mu);
+  const Topology& T = c->topo;
+  if (!T.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
+  const void* src = nullptr;
+  long long n = 0;
+  size_t elem = 8;
+  switch (what) {
+    case RBGTOPO_SNAP_BASE: src = T.base.p; n = T.n; elem = 4; break;
+    case RBGTOPO_SNAP_ORDER: src = T.order.p; n = c->slab_hi - c->slab_lo; break;
+    case RBGTOPO_SNAP_ORDER_ALL: src = c->cfg.world > 1 ? T.order_all.p : T.order.p; n = T.n; break;
+    case RBGTOPO_SNAP_POS:
+      if (c->cfg.world != 1) return fail(RBGTOPO_EINVAL, "pos exists with world == 1 only");
+      src = T.pos.p; n = T.n; elem = 4;
+      break;
+    case RBGTOPO_SNAP_DELTA_REPAIRS: n = 1; break;
+    default: return fail(RBGTOPO_EINVAL, "what = %d", what);
+  }
+  if (n_out) *n_out = n;
+  if (n == 0) return RBGTOPO_OK;
+  if (!out || out_bytes < n * (long long)elem) return fail(RBGTOPO_EINVAL, "out_bytes %lld < %lld", (long long)out_bytes, n * (long long)elem);
+  if (what == RBGTOPO_SNAP_DELTA_REPAIRS) {
+    const int64_t v = c->delta_repairs;
+    memcpy(out, &v, sizeof v);
+    return RBGTOPO_OK;
+  }
+  CK(cudaSetDevice(c->cfg.device));
+  CK(cudaEventSynchronize(c->topo_ready));
+  if (n) CK(cudaMemcpy(out, src, (size_t)n * elem, cudaMemcpyDeviceToHost));
   return RBGTOPO_OK;
 }
 

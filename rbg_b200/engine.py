@@ -167,6 +167,21 @@ class TopoPlacer:
         self._check(self.lib.rbgtopo_read_topk(self._h, handle, rolerow, _p(out, _lib.u64p), k))
         return out
 
+    SNAPSHOT = {"base": (0, np.float32), "order": (1, np.uint64), "order_all": (2, np.uint64), "pos": (3, np.int32),
+                "delta_repairs": (4, np.int64)}
+
+    def read_snapshot(self, what: str) -> np.ndarray:
+        """One per-snapshot vector exactly as the device holds it (rbgtopo_read_snapshot): "base", "order" (this
+        rank's slab), "order_all", "pos" (world == 1) or "delta_repairs" (one int64)."""
+        code, dt = self.SNAPSHOT[what]
+        n = C.c_int64()
+        rc = self.lib.rbgtopo_read_snapshot(self._h, code, None, 0, C.byref(n))   # sizes only: EINVAL unless empty
+        if rc not in (0, -1):
+            self._check(rc)
+        out = np.empty(n.value, dtype=dt)
+        self._check(self.lib.rbgtopo_read_snapshot(self._h, code, out.ctypes.data_as(C.c_void_p), out.nbytes, C.byref(n)))
+        return out
+
     # -- node-axis sharding
     def slab(self) -> Tuple[int, int]:
         lo, hi = C.c_int32(), C.c_int32()
