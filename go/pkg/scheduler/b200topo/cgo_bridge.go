@@ -61,6 +61,13 @@ static int32_t rbgtopo_go_place_groups(rbgtopo_ctx* ctx, const int32_t* groups, 
   rbgtopo_go_err(ctx, rc, err);
   return rc;
 }
+static int32_t rbgtopo_go_place_groups_committed(rbgtopo_ctx* ctx, const int32_t* groups, int64_t words,
+                                                 int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds,
+                                                 char* err) {
+  int32_t rc = rbgtopo_place_groups_committed(ctx, groups, words, assign, status, domain, rounds);
+  rbgtopo_go_err(ctx, rc, err);
+  return rc;
+}
 */
 import "C"
 
@@ -164,4 +171,21 @@ func (p *placer) placeGroups(blob []int32) (assign, status, domain []int32, err 
 		return nil, nil, nil, err
 	}
 	return assign[:nPending], status[:nGroups], domain[:nGroups], nil
+}
+
+// placeGroupsCommitted: placeGroups as a committed batch (DESIGN.md §3.8): the groups in blob order, each seeing the
+// capacity and exclusive domains the groups before it took; rounds = selection rounds the library ran.
+func (p *placer) placeGroupsCommitted(blob []int32) (assign, status, domain []int32, rounds int32, err error) {
+	nGroups, nPending := int(blob[2]), int(blob[4])
+	assign = make([]int32, max(nPending, 1))
+	status = make([]int32, max(nGroups, 1))
+	domain = make([]int32, max(nGroups, 1))
+	var r C.int32_t
+	var buf [C.RBGTOPO_GO_ERRLEN]C.char
+	rc := C.rbgtopo_go_place_groups_committed(p.ctx, p32(blob), C.int64_t(len(blob)), p32(assign), p32(status), p32(domain),
+		&r, &buf[0])
+	if err = mkErr(rc, &buf); err != nil {
+		return nil, nil, nil, 0, err
+	}
+	return assign[:nPending], status[:nGroups], domain[:nGroups], int32(r), nil
 }

@@ -236,6 +236,25 @@ int32_t rbgtopo_place_groups(rbgtopo_ctx* ctx, const int32_t* groups,
                              int64_t groups_words, int32_t* assign,
                              int32_t* status, int32_t* domain);
 
+/* Committed batch (DESIGN.md §3.8).  Same GROUPS blob, same outputs, same validation and error codes
+ * as rbgtopo_place_groups, but the groups are placed IN BLOB ORDER, each seeing what the groups before
+ * it took: every replica an earlier group placed consumes (node, demand) — a failed gang consumes
+ * nothing — and every exclusive domain an earlier group reports (status != RBGTOPO_GANG_FAILED) counts
+ * as owned by that group's gid (the last such group's, when several report it).  Scores, base and the
+ * background order stay those of the snapshot.  So the hints of one call never ask a node for more
+ * than free[n], and two exclusive groups with different gids never get the same domain unless the
+ * caller fixed it (fixed_domain) for the later of the two.  Group 0 gets exactly what
+ * rbgtopo_place_groups gives it.  The call holds the snapshot shared for all its rounds (one host
+ * synchronisation each), so a long committed batch delays set_topology / update_nodes on the ctx.
+ * Use it for batches of concurrent reconciles whose hints must hold together; rbgtopo_place_groups
+ * keeps snapshot semantics (§3.7).  No dense matrix is computed; selection runs in rounds (at most
+ * n_groups, one when no group reads a node or domain an earlier group took), *rounds (may be NULL) =
+ * selection rounds run.  Valid for any world: every rank returns the identical result.  Gids need not
+ * be distinct.  A group whose table of patched nodes does not fit k_plan_group's shared memory makes
+ * the call return RBGTOPO_ELIMIT (there is no per-wave fallback for committed batches). */
+int32_t rbgtopo_place_groups_committed(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                       int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds);
+
 /* rbgtopo_place_groups pipeline, staged: the groups are compiled into a
  * device-resident multi-wave plan (one step blob, wave-major, expanded on the
  * device), so rbgtopo_run_staged runs ONE score launch for the dense rows of every

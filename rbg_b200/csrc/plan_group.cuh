@@ -122,15 +122,66 @@ __device__ __forceinline__ BgCand bg_load(const TopoDev& t, int need_i, int i, i
   return bg_attrs(t, need_i, i, n_sel, (i < n_sel && need_i > 0) ? t.order_all[i] : 0ull);
 }
 
+// ---- committed batch (rbgtopo_place_groups_committed, DESIGN.md §3.8) -----------------------------------------------
+// Group g of a committed batch sees what the groups before it took: capacity on the nodes their replicas were placed
+// on, and the exclusive domains they reported.  Both are kept as short linked lists that k_commit_claims rebuilds from
+// the results of every round; a node or domain nobody claimed costs one load.  The selection reads them exactly where
+// it reads the node's attributes (the table's dense view, the background candidates) and records that it did, so that
+// k_commit_diff can tell which later groups a changed claim can affect.
+struct CommitDev {
+  const int* head;     // [nodes] first claim on the node (the dense row of the replica), -1 = none
+  const int4* claim;   // [rows] {group index, demand, next claim on the same node, 0}
+  const int* dhead;    // [domains] first exclusive group that reported the domain, -1 = none
+  const int2* dclaim;  // [groups] {gid, next group that reported the same domain}
+  int* reader;         // [nodes] largest group index whose selection read the node this round
+  int* dreader;        // [domains] the same for the owner of the domain (exclusive groups)
+  int g;               // the group this CTA places (set by the kernel)
+  bool excl;           // ... and whether it is exclusive
+};
+// capacity the groups before cm.g took on `node`
+__device__ __forceinline__ int commit_ext(const CommitDev& cm, int node) {
+  int s = 0;
+  for (int i = cm.head[node]; i >= 0;) {
+    const int4 c = cm.claim[i];
+    if (c.x < cm.g) s += c.y;
+    i = c.z;
+  }
+  return s;
+}
+// owner of domain `dom` for group cm.g: the gid of the LAST earlier exclusive group that reported it, else `owner`
+__device__ __forceinline__ int commit_owner(const CommitDev& cm, int dom, int owner) {
+  int last = -1;
+  for (int i = cm.dhead[dom]; i >= 0;) {
+    const int2 c = cm.dclaim[i];
+    if (i < cm.g && i > last) { last = i; owner = c.x; }
+    i = c.y;
+  }
+  return owner;
+}
+// The marks only grow within a round, so a plain L2 load that already shows cm.g or more makes the atomic redundant; the
+// CTAs of a round all read the head of the background order, and this keeps them from queueing on the same addresses.
+__device__ __forceinline__ void commit_note_read(const CommitDev& cm, int node, int dom) {
+  if (__ldcg(&cm.reader[node]) < cm.g) atomicMax(&cm.reader[node], cm.g);
+  if (cm.excl && __ldcg(&cm.dreader[dom]) < cm.g) atomicMax(&cm.dreader[dom], cm.g);
+}
+// a background candidate as group cm.g sees it (the selection notes the read where the candidate's capacity or owner
+// can decide anything: not where its domain alone rules it out)
+__device__ __forceinline__ void commit_adjust(BgCand& c, const CommitDev& cm) {
+  if (c.node < 0) return;
+  c.free_ -= commit_ext(cm, c.node);
+  if (cm.excl) c.owner = commit_owner(cm, c.dom, c.owner);
+}
+
 // top-K of a role row into out[0..KS) (+ capacities): select_role_fast with the
 // delta evaluated from the per-group-role planes.  `first` = bg_load(..., lane, ...) when
-// have_first.  One warp.
+// have_first.  One warp.  COMMIT: the background candidates it loads are seen through `cm` (`first` already is).
+template <bool COMMIT = false>
 __device__ __forceinline__ void select_role_group(const TopoDev& t, int gid, bool excl_step, const GroupRole& role,
                                                   const float* pair_row, int Q, int K, int dom, const GroupTab& T,
                                                   int cnt, bool have_first, const BgCand& first, int dbg,
                                                   unsigned long long* sAcc, int* sAccAv,
                                                   unsigned long long* sPat, int* sPatAv, unsigned long long* out,
-                                                  int* outAvail) {
+                                                  int* outAvail, const CommitDev* cm = nullptr) {
   const int lane = threadIdx.x & 31;
   if (dom == DOM_NONE || K <= 0) {
     out[lane] = 0;
@@ -148,6 +199,8 @@ __device__ __forceinline__ void select_role_group(const TopoDev& t, int gid, boo
   constexpr int EREG = 8;
   auto entry_key = [&](int i) -> unsigned long long {
     const int av = gtab_avail(T, i), dd = T.dDom[i];
+    if constexpr (COMMIT)
+      if (dom == DOM_ANY || (dd & 0x7FFFFFFF) == dom) commit_note_read(*cm, T.node[T.dSlot[i]], dd & 0x7FFFFFFF);
     if (av >= demand && !(rexcl && dd < 0) && (dom == DOM_ANY || (dd & 0x7FFFFFFF) == dom)) {
       const int slot = T.dSlot[i];
       return make_key(fmaf(need, T.dBase[i], gtab_delta(T, pair_row, Q, slot)), T.node[slot]);
@@ -191,7 +244,11 @@ __device__ __forceinline__ void select_role_group(const TopoDev& t, int gid, boo
   // ---- (b) walk the background order; patched nodes are skipped by a table probe
   int acc = 0;
   for (int pos = 0; pos < t.n && acc < K; pos += 32) {
-    const BgCand c = (pos == 0 && have_first) ? first : bg_load(t, role.need, pos + lane, t.n);
+    BgCand c = (pos == 0 && have_first) ? first : bg_load(t, role.need, pos + lane, t.n);
+    if constexpr (COMMIT) {
+      if (!(pos == 0 && have_first)) commit_adjust(c, *cm);
+      if (c.node >= 0 && (dom == DOM_ANY || c.dom == dom)) commit_note_read(*cm, c.node, c.dom);
+    }
     bool ok = c.node >= 0 && c.free_ >= demand;
     if (ok && rexcl) ok = (c.owner == -1 || c.owner == gid);
     if (ok && dom != DOM_ANY) ok = c.dom == dom;
@@ -324,8 +381,14 @@ __global__ void __launch_bounds__(32 * RTAB_WARPS) k_group_rtab(const int* __res
 // group's role table, and reports per GROUP: b.status[g] = worst wave status, b.domain_out[g] = the exclusive
 // domain.  The host then computes nothing per step — no step numbering, section sizes or prefixes — and launches
 // this kernel right behind the dense-matrix kernel (DESIGN.md §4.4).
-template <bool DIRECT>
-__global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group(TopoDev t, BatchDev b, int QB, int HT, int CAP, int record) {
+//
+// COMMIT = true (k_plan_group_commit, rbgtopo_place_groups_committed; implies DIRECT): one round of a committed batch
+// (DESIGN.md §3.8).  The CTA's group sees the claims of the groups before it through `cm` where it reads node
+// attributes — free capacity minus what they took, the owner of a domain they reported — and records what it read.
+// No dense matrix exists: the kernel never touches one.  `need` counts the replicas actually placed by earlier
+// waves (not the planned ones), so every group is exact without the host-driven loop.
+template <bool DIRECT, bool COMMIT>
+__device__ __forceinline__ void plan_group_body(TopoDev t, BatchDev b, int QB, int HT, int CAP, int record, CommitDev cm) {
   extern __shared__ __align__(16) unsigned char pg_smem[];
   __shared__ int sTakenNode[KS], sTakenAmt[KS], sTakenRole[KS];
   __shared__ int sDstar, sCnt, sNew, sStatus, sAny, sCorrN;
@@ -407,6 +470,10 @@ __global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group(TopoDev t, BatchDev
   const bool excl_step = (h.flags & RBGTOPO_STEP_EXCLUSIVE) != 0;
   const bool gang = (h.flags & RBGTOPO_STEP_GANG) != 0;
   const int gid = h.gid, Q = h.Q;
+  if constexpr (COMMIT) {
+    cm.g = step;
+    cm.excl = excl_step;
+  }
   int fixed = excl_step ? h.fixed_domain : -1;
   g_dom = fixed;  // DIRECT: an exclusive group confirms the domain it already occupies
   const size_t stride = (size_t)t.slab_stride;
@@ -473,6 +540,8 @@ __global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group(TopoDev t, BatchDev
     BgCand first;
     const bool have_first = warp < h.P;
     if (have_first) first = bg_attrs(t, sRole[warp].need, lane, t.n, ob0);
+    if constexpr (COMMIT)
+      if (have_first) commit_adjust(first, cm);
     // closed neighbourhoods of the placements: one flat pass over all their CSR entries
     {
       int total = 0;
@@ -501,11 +570,13 @@ __global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group(TopoDev t, BatchDev
       const int node = T.node[T.dSlot[d]];
       int dd = t.domain[node];
       if (excl_step) {
-        const int o = t.node_owner[node];
+        int o = t.node_owner[node];
+        if constexpr (COMMIT) o = commit_owner(cm, dd, o);
         if (!(o == -1 || o == gid)) dd |= 0x80000000;
       }
       T.dBase[d] = t.base[node];
       T.dFree[d] = t.free_[node];
+      if constexpr (COMMIT) T.dFree[d] -= commit_ext(cm, node);  // the selection notes the read (select_role_group)
       T.dDom[d] = dd;
     }
     cnt_done = cnt;
@@ -522,8 +593,8 @@ __global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group(TopoDev t, BatchDev
       if (warp == 0) {
         int d = -1;
         if (pstar >= 0) {
-          select_role_group(t, gid, excl_step, sRole[pstar], sPair + pstar * QB, Q, 1, DOM_ANY, T,
-                            cnt, pstar == 0, first, 29, sAcc, sAccAv, sPat, sPatAv, sList, sListAv);
+          select_role_group<COMMIT>(t, gid, excl_step, sRole[pstar], sPair + pstar * QB, Q, 1, DOM_ANY, T,
+                                    cnt, pstar == 0, first, 29, sAcc, sAccAv, sPat, sPatAv, sList, sListAv, &cm);
           const unsigned long long top = sList[0];
           d = top ? t.domain[key_node(top)] : -1;
         }
@@ -539,9 +610,9 @@ __global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group(TopoDev t, BatchDev
       int K = 0;
       for (int q = 0; q <= p; ++q) K += sRole[q].count;
       K = min(K, t.n);
-      select_role_group(t, gid, excl_step, sRole[p], sPair + p * QB, Q, K, dom, T, cnt, true, first, warp == 0 ? wave_i * 8 + 6 : -1,
-                        sAcc + p * KS, sAccAv + p * KS, sPat + p * KS, sPatAv + p * KS, sList + p * KS,
-                        sListAv + p * KS);
+      select_role_group<COMMIT>(t, gid, excl_step, sRole[p], sPair + p * QB, Q, K, dom, T, cnt, true, first,
+                                warp == 0 ? wave_i * 8 + 6 : -1, sAcc + p * KS, sAccAv + p * KS, sPat + p * KS,
+                                sPatAv + p * KS, sList + p * KS, sListAv + p * KS, &cm);
       if (!DIRECT) b.merged[(size_t)(h.rolerow_off + p) * KS + lane] = sList[p * KS + lane];
     }
     __syncthreads();
@@ -552,7 +623,7 @@ __global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group(TopoDev t, BatchDev
 #ifdef RBGTOPO_PHASE_CLOCKS
     if (!(g_dbg_skip & 1))
 #endif
-    if (warp != 0 && record) {
+    if (warp != 0 && record && !COMMIT) {
       // one record per patched node of this rank's slab whose rows differ from the background:
       // [node, value of role row 0 .. P-1] (the summed delta, or -inf); region of step s =
       // b.corr + poff[s] * b.corr_w, never more than the step's patch capacity
@@ -582,7 +653,7 @@ __global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group(TopoDev t, BatchDev
             if (p < h.P) e[1 + p] = __float_as_int(v[p]);
         }
       }
-    } else if (warp != 0) {
+    } else if (warp != 0 && !COMMIT) {
       // first touch of the matrix: as a programmatic dependent of the dense-matrix kernel, everything up to
       // here (table, selection of wave 0) ran while that kernel was draining; warp 0 (greedy) never waits
       if (wave_i == 0) {
@@ -637,6 +708,8 @@ __global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group(TopoDev t, BatchDev
             ++unplaced;
           }
           if (lane == 0) b.assign[h.rep_off + r] = pick;
+          if constexpr (COMMIT)
+            if (lane == 0 && pick >= 0) sPlaced[grole] += 1;  // placed, not planned: `need` of the next wave is exact
         }
       }
       int status = unplaced ? RBGTOPO_PLACED_PART : RBGTOPO_PLACED_ALL;
@@ -661,14 +734,16 @@ __global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group(TopoDev t, BatchDev
         sAny = ntaken > 0;
       }
     }
-    if (DIRECT && tid < h.P) sPlaced[sWRole[tid]] += sWCount[tid];  // planned, as the host's wave rule counts them
+    if (DIRECT && !COMMIT && tid < h.P) sPlaced[sWRole[tid]] += sWCount[tid];  // planned, as the host's wave rule counts them
     __syncthreads();
     if (record && tid == 0) b.corr_cnt[step] = sCorrN;
     PCLK(wave_i * 8 + 5);
     ++wave_i;
     if (DIRECT) {  // per-group result (what plan_results derives from the per-step outputs of the expanded plan)
       g_stat = max(g_stat, sStatus);
-      if (dstar >= 0) g_dom = dstar;
+      // COMMIT: like the host-driven loop, a wave that placed nothing does not move the reported domain (the
+      // snapshot path re-runs such groups through that loop)
+      if (dstar >= 0 && (!COMMIT || sAny)) g_dom = dstar;
       g_i0 += h.R;
       n_new = sNew;
       if (excl_step && dstar >= 0 && sAny) fixed = dstar;
@@ -712,6 +787,78 @@ __global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group(TopoDev t, BatchDev
 #ifdef RBGTOPO_PHASE_CLOCKS
   if (tid == 0 && blockIdx.x < 2048) { g_cta_ns[blockIdx.x * 4 + 1] = pg_gtime(); g_cta_ns[blockIdx.x * 4 + 2] = sCnt; }
 #endif
+}
+
+template <bool DIRECT>
+__global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group(TopoDev t, BatchDev b, int QB, int HT, int CAP, int record) {
+  plan_group_body<DIRECT, false>(t, b, QB, HT, CAP, record, CommitDev{});
+}
+
+// One round of a committed batch (DESIGN.md §3.8): b.perm[0 .. gridDim.x) = the groups of the round (ascending).
+__global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group_commit(TopoDev t, BatchDev b, int QB, int HT, int CAP, CommitDev cm) {
+  plan_group_body<true, true>(t, b, QB, HT, CAP, 0, cm);
+}
+
+// Claims of a committed batch, one warp per group, from the results of the last round (assign / domain_out of the
+// plan kernel, the blob for groups with nothing pending): every placed replica links its dense row into the list of
+// its node, every exclusive group that reports a domain links itself into the list of the domain.  head / dhead are
+// -1 on entry.  A failed gang has no placements and reports no domain.
+__global__ void __launch_bounds__(32 * RTAB_WARPS) k_commit_claims(const int* __restrict__ grp, int n_groups,
+                                                                 const int* __restrict__ assign, const int* __restrict__ domain,
+                                                                 int* head, int4* claim, int* dhead, int2* dclaim) {
+  const int lane = threadIdx.x & 31;
+  const int g = blockIdx.x * RTAB_WARPS + (threadIdx.x >> 5);
+  if (g >= n_groups) return;
+  const int* rec = grp + RBGTOPO_HDR_WORDS + (size_t)g * RBGTOPO_GROUP_WORDS;
+  const int q = rec[3], roff = rec[4], row0 = rec[8], pend = rec[9];
+  if (lane == 0 && (rec[1] & RBGTOPO_STEP_EXCLUSIVE)) {
+    const int d = pend > 0 ? domain[g] : rec[2];  // nothing pending: the group confirms the domain it occupies
+    if (d >= 0) dclaim[g] = make_int2(rec[0], atomicExch(&dhead[d], g));
+  }
+  int pre = 0;  // a group's rows are its roles' pending replicas in role order
+  for (int r = 0; r < q; ++r) {
+    const int pr = grp[roff + 4 * r + 1], dem = grp[roff + 4 * r + 2];
+    for (int i = lane; i < pr; i += 32) {
+      const int row = row0 + pre + i, node = assign[row];
+      if (node >= 0) claim[row] = make_int4(g, dem, atomicExch(&head[node], row), 0);
+    }
+    pre += pr;
+  }
+}
+
+// After a round of a committed batch: which later groups can a changed claim affect?  One warp per group of the round
+// (b.perm order).  A group's claims changed when a placement or its reported domain differs from the previous round's
+// (`prev`, which is then updated).  A changed claim on node n matters only when a later group read n this round
+// (reader[n] > g), a changed domain only when a later exclusive group read a node of it.  *cmin = the lowest group with
+// a claim that matters: groups up to it saw exactly the claims they will see from now on, the next round re-runs the
+// groups above it.
+__global__ void __launch_bounds__(32 * RTAB_WARPS) k_commit_diff(const int* __restrict__ grp, const int* __restrict__ groups,
+                                                               int n_run, const int* __restrict__ assign,
+                                                               const int* __restrict__ domain, int* prev_assign,
+                                                               int* prev_domain, const int* __restrict__ reader,
+                                                               const int* __restrict__ dreader, int* cmin) {
+  const int lane = threadIdx.x & 31;
+  const int k = blockIdx.x * RTAB_WARPS + (threadIdx.x >> 5);
+  if (k >= n_run) return;
+  const int g = groups[k];
+  const int* rec = grp + RBGTOPO_HDR_WORDS + (size_t)g * RBGTOPO_GROUP_WORDS;
+  const int row0 = rec[8], pend = rec[9];
+  bool hit = false;
+  for (int i = lane; i < pend; i += 32) {
+    const int a = assign[row0 + i], o = prev_assign[row0 + i];
+    if (a != o) {
+      hit |= (a >= 0 && reader[a] > g) || (o >= 0 && reader[o] > g);
+      prev_assign[row0 + i] = a;
+    }
+  }
+  if (lane == 0) {
+    const int d = domain[g], od = prev_domain[g];
+    if (d != od) {
+      hit |= (d >= 0 && dreader[d] > g) || (od >= 0 && dreader[od] > g);
+      prev_domain[g] = d;
+    }
+  }
+  if (__any_sync(FULL, hit) && lane == 0) atomicMin(cmin, g);
 }
 
 // Applies the correction records k_plan_group(record = 1) left: one warp per step, one lane per

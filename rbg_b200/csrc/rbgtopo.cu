@@ -204,6 +204,11 @@ struct Batch {
   std::vector<int> grp_flags, grp_assign_off, grp_pending, grp_fixed;
   DevBuf<int> out;  // assign[total_r] | status[n] | domain[n] | dstar[n]
   PinBuf<int> h_in, h_out;
+  // committed batches (place_groups_committed): head[nodes] | dhead[domains] | reader[nodes] | dreader[domains] |
+  // previous round's assign[total_r] and domain[n] | lowest group whose changed claims matter; the claim lists
+  DevBuf<int> cm_int;
+  DevBuf<int4> cm_claim;
+  DevBuf<int2> cm_dclaim;
   ~Batch() {
     if (stream) cudaStreamDestroy(stream);
     if (stream2) cudaStreamDestroy(stream2);
@@ -1377,6 +1382,8 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
   CK(cudaFuncSetAttribute(k_plan_group<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_plan_group<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_plan_group<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  CK(cudaFuncSetAttribute(k_plan_group_commit, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
+  CK(cudaFuncSetAttribute(k_plan_group_commit, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CK(cudaFuncSetAttribute(emit_tma_fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)emit_tma_smem_bytes(kEmitStages)));
   // k_emit_tma and k_plan_group are meant to share an SM: both ask for the largest shared-memory carve-out,
   // otherwise the persistent emit CTA pins the SM at the small carve-out it needs alone and the CTAs of
@@ -3201,6 +3208,169 @@ int place_groups_direct(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_
   return done(RBGTOPO_OK);
 }
 
+// ---- rbgtopo_place_groups_committed -----------------------------------------------------------------------------------
+// A committed batch (DESIGN.md §3.8) is rounds of selection only, no dense matrix: k_plan_group_commit over a suffix of
+// the groups (each sees the claims of the previous round's results of the groups before it), k_commit_diff (the lowest
+// group with a changed claim some later group read), k_commit_claims (the lookups of the next round), and one 4-byte
+// read-back.  Groups up to that lowest group are final, the next round re-runs the groups above it: it only grows, so
+// there are at most n_groups rounds, and a batch whose groups read nothing an earlier group took needs one.  The host
+// validates the blob exactly as the direct path of rbgtopo_place_groups does (same codes).
+int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign, int32_t* status,
+                           int32_t* domain, int32_t* rounds_out) {
+  *rounds_out = 0;
+  if (words < RBGTOPO_HDR_WORDS || gb[0] != RBGTOPO_GROUPS_MAGIC || gb[1] != RBGTOPO_ABI_VERSION || gb[3] != words)
+    return fail(RBGTOPO_EINVAL, "bad groups blob header");
+  const int ng = gb[2];
+  if (ng < 0 || (int64_t)RBGTOPO_HDR_WORDS + (int64_t)ng * RBGTOPO_GROUP_WORDS > words)
+    return fail(RBGTOPO_EINVAL, "group table exceeds blob");
+  if (words > 0x3FFFFFFFLL) return fail(RBGTOPO_ELIMIT, "groups blob too large");
+  NvtxRange nv("rbgtopo:place_groups_committed");
+  const Topology& T = c->topo;
+  TopoHost th;
+  th.n = T.n;
+  th.n_domains = T.n_domains;
+  th.degp1 = T.h_degp1.data();
+  th.max_degp1 = T.max_degp1;
+  th.wsum_max = T.wsum_max;
+  const long long row_w = T.wsum_max + RBGTOPO_SELF_W;
+  const long long amax_limit = ((1LL << 24) + row_w - 1) / row_w;
+  static thread_local std::vector<GroupFacts> facts;
+  static thread_local std::vector<int32_t> order, run;
+  order.resize((size_t)std::max(ng, 1));
+  DirectGeom G;
+  int rc = direct_pass1(th, gb, words, ng, amax_limit, row_w, facts, order.data(), &G);
+  if (rc) return rc;
+  rc = direct_pass2(th, gb, words, ng, amax_limit, row_w, facts, &G);
+  if (rc) return rc;
+  if (G.max_cap > 0x3FFFFFFFLL || G.smem > kFastSmemMax)
+    return fail(RBGTOPO_ELIMIT, "a group's table of patched nodes (%lld entries, %zu B of shared memory) does not fit "
+                                "k_plan_group: a committed batch has no per-wave fallback", G.max_cap, G.smem);
+  run.clear();  // groups with pending replicas, ascending: a round runs a suffix of them
+  for (int g = 0; g < ng; ++g)
+    if (facts[g].nw > 0) run.push_back(g);
+  const int n0 = (int)run.size();
+  const long long total_r = G.total_r;
+  const size_t out_n = (size_t)total_r + 2 * (size_t)ng;
+  Batch* b = nullptr;
+  rc = acquire_batch(c, &b);
+  if (rc) return rc;
+  cudaStream_t s = stream_of(c, b);
+  const bool timed = c->kernel_timing.load(std::memory_order_relaxed);
+  std::vector<float> round_ms;
+  int rounds = 0;
+  rc = [&]() -> int {
+    if (n0 == 0) return RBGTOPO_OK;
+    const size_t run_off = ((size_t)words + 3) & ~(size_t)3;  // staging: GROUPS blob | pad | run[n0]
+    const size_t src_words = run_off + (size_t)n0;
+    CK(b->h_in.reserve(src_words));
+    CK(b->gsrc.reserve(src_words));
+    CK(b->out.reserve(out_n + 4));
+    CK(b->h_out.reserve(out_n + 4));
+    const int N = T.n, ND = T.n_domains;
+    const size_t o_dhead = (size_t)N, o_reader = o_dhead + ND, o_dreader = o_reader + N, o_prev = o_dreader + ND,
+                 o_cmin = o_prev + out_n, n_int = o_cmin + 1;
+    CK(b->cm_int.reserve(n_int));
+    CK(b->cm_claim.reserve((size_t)std::max<long long>(total_r, 1)));
+    CK(b->cm_dclaim.reserve((size_t)std::max(ng, 1)));
+    memcpy(b->h_in.p, gb, (size_t)words * 4);
+    memcpy(b->h_in.p + run_off, run.data(), (size_t)n0 * 4);
+    CK(cudaMemcpyAsync(b->gsrc.p, b->h_in.p, src_words * 4, cudaMemcpyHostToDevice, s));
+    int* const ci = b->cm_int.p;
+    int* const o_assign = b->out.p;
+    int* const o_domain = b->out.p + total_r + ng;
+    // nothing placed and no domain reported yet: the claims before round 0 are those of groups with nothing pending
+    CK(cudaMemsetAsync(b->out.p, 0xFF, out_n * 4, s));
+    CK(cudaMemsetAsync(ci + o_prev, 0xFF, out_n * 4, s));
+    CK(cudaMemsetAsync(ci, 0xFF, (size_t)(N + ND) * 4, s));
+    const int claim_grid = (ng + RTAB_WARPS - 1) / RTAB_WARPS;
+    k_commit_claims<<<claim_grid, 32 * RTAB_WARPS, 0, s>>>(b->gsrc.p, ng, o_assign, o_domain, ci, b->cm_claim.p, ci + o_dhead,
+                                                           b->cm_dclaim.p);
+    CK(cudaStreamWaitEvent(s, c->topo_ready, 0));  // a pending snapshot refresh: free, owners, base and the order
+    BatchDev d{};
+    d.blob = b->gsrc.p;
+    d.n_steps = ng;
+    d.lc = c->lc;
+    d.chunk = c->chunk;
+    d.parts = 1;
+    d.assign = o_assign;
+    d.status = b->out.p + total_r;
+    d.domain_out = o_domain;
+    d.dstar = o_domain;
+    CommitDev cm{};
+    cm.head = ci;
+    cm.claim = b->cm_claim.p;
+    cm.dhead = ci + o_dhead;
+    cm.dclaim = b->cm_dclaim.p;
+    cm.reader = ci + o_reader;
+    cm.dreader = ci + o_dreader;
+    int first = 0;  // run[first ..) = the groups of the next round
+    while (first < n0) {
+      if (rounds >= ng) return fail(RBGTOPO_ECUDA, "internal: committed batch did not converge in %d rounds", ng);
+      const int n_run = n0 - first;
+      d.perm = b->gsrc.p + run_off + first;
+      CK(cudaMemsetAsync(ci + o_reader, 0xFF, (size_t)(N + ND) * 4, s));  // reader and dreader: -1
+      CK(cudaMemsetAsync(ci + o_cmin, 0x7F, 4, s));                        // > any group index
+      if (timed) CK(cudaEventRecord(b->ev[0], s));
+      k_plan_group_commit<<<n_run, G.nth, G.smem, s>>>(topo_dev(c), d, G.max_q, G.HT, G.CAP, cm);
+      CK(cudaGetLastError());
+      if (timed) CK(cudaEventRecord(b->ev[1], s));
+      k_commit_diff<<<(n_run + RTAB_WARPS - 1) / RTAB_WARPS, 32 * RTAB_WARPS, 0, s>>>(
+          b->gsrc.p, d.perm, n_run, o_assign, o_domain, ci + o_prev, ci + o_prev + total_r + ng, ci + o_reader,
+          ci + o_dreader, ci + o_cmin);
+      CK(cudaMemsetAsync(ci, 0xFF, (size_t)(N + ND) * 4, s));  // head and dhead
+      k_commit_claims<<<claim_grid, 32 * RTAB_WARPS, 0, s>>>(b->gsrc.p, ng, o_assign, o_domain, ci, b->cm_claim.p,
+                                                             ci + o_dhead, b->cm_dclaim.p);
+      CK(cudaMemcpyAsync(b->h_out.p + out_n, ci + o_cmin, 4, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      CK(cudaGetLastError());
+      ++rounds;
+      if (timed) {
+        float ms = 0.0f;
+        CK(cudaEventElapsedTime(&ms, b->ev[0], b->ev[1]));
+        round_ms.push_back(ms);
+      }
+      const int cmin = b->h_out.p[out_n];
+      if (cmin >= ng) break;  // no changed claim was read by a later group: every group saw its final input
+      first = (int)(std::upper_bound(run.begin(), run.end(), cmin) - run.begin());
+    }
+    CK(cudaMemcpyAsync(b->h_out.p, b->out.p, out_n * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    return RBGTOPO_OK;
+  }();
+  if (rc) {
+    cudaStreamSynchronize(s);
+    release_batch(c, b);
+    return rc;
+  }
+  const int32_t* a = b->h_out.p;
+  if (total_r > 0) memcpy(assign, a, (size_t)total_r * 4);
+  for (int g = 0; g < ng; ++g) {
+    const int32_t* rec = gb + RBGTOPO_HDR_WORDS + (int64_t)g * RBGTOPO_GROUP_WORDS;
+    const bool excl = (rec[1] & RBGTOPO_STEP_EXCLUSIVE) != 0;
+    int st = RBGTOPO_PLACED_ALL, dm = excl ? rec[2] : -1;  // nothing pending: placed, the domain it occupies confirmed
+    if (facts[g].nw > 0) {
+      st = a[total_r + g];
+      dm = excl ? a[total_r + ng + g] : -1;
+    }
+    if (status) status[g] = st;
+    if (domain) domain[g] = dm;
+  }
+  release_batch(c, b);
+  *rounds_out = rounds;
+  {
+    rbgtopo_timing tm{};
+    tm.launches = 3 * rounds + (n0 > 0 ? 1 : 0);  // kernels: the first claims build, then plan + diff + claims per round
+    tm.h2d_words = (int32_t)std::min<long long>((long long)words + n0, INT32_MAX);
+    std::lock_guard<std::mutex> g(c->stat_mu);
+    c->last = tm;
+    c->last_score_ms.assign(round_ms.size(), 0.0f);  // no dense matrix; one selection time per round
+    c->last_select_ms = round_ms;
+    c->calls += 1;
+    c->launches += tm.launches;
+  }
+  return RBGTOPO_OK;
+}
+
 }  // namespace
 
 int32_t rbgtopo_place_groups(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign,
@@ -3297,6 +3467,19 @@ int32_t rbgtopo_place_groups(rbgtopo_ctx* c, const int32_t* gb, int64_t words, i
   for (char d : dirty) any |= d != 0;
   if (!any) return RBGTOPO_OK;
   return place_groups_slow(c, gb, words, assign, status, domain, &dirty);
+}
+
+int32_t rbgtopo_place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign,
+                                       int32_t* status, int32_t* domain, int32_t* rounds) {
+  if (rounds) *rounds = 0;
+  if (!c || !gb || !assign) return fail(RBGTOPO_EINVAL, "null argument");
+  std::shared_lock<std::shared_mutex> lk(c->topo_mu);
+  if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
+  CK(cudaSetDevice(c->cfg.device));
+  int32_t r = 0;
+  const int rc = place_groups_committed(c, gb, words, assign, status, domain, &r);
+  if (rounds) *rounds = r;
+  return rc;
 }
 
 int32_t rbgtopo_plan_describe(const int32_t* gb, int64_t words, int32_t n_nodes, int32_t n_domains,

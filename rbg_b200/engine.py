@@ -117,6 +117,19 @@ class TopoPlacer:
         self._check(self.lib.rbgtopo_place_groups(self._h, _p(gb), len(gb), _p(assign), _p(status), _p(domain)))
         return assign[:tp], status[:ng], domain[:ng]
 
+    def place_groups_committed(self, groups_blob: np.ndarray) -> Tuple[np.ndarray, np.ndarray, np.ndarray, int]:
+        """Whole groups as a committed batch (DESIGN.md §3.8): in blob order, each group sees the capacity and the
+        exclusive domains the groups before it took.  Returns (assign, status, domain, selection rounds run)."""
+        gb = _i32(groups_blob)
+        ng, tp = int(gb[2]), int(gb[4])
+        assign = np.empty(max(tp, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        rounds = C.c_int32()
+        self._check(self.lib.rbgtopo_place_groups_committed(self._h, _p(gb), len(gb), _p(assign), _p(status),
+                                                            _p(domain), C.byref(rounds)))
+        return assign[:tp], status[:ng], domain[:ng], rounds.value
+
     # -- staged (device-resident) batches
     def stage(self, blob: np.ndarray) -> int:
         blob = _i32(blob)

@@ -318,9 +318,16 @@ class B200TopoPodGroupManager:
                          fixed_domain=g.fixed_domain if g.exclusive else -1))
         return gb.build(), runs
 
-    def reconcile_pod_groups(self, rbgs: Sequence[RoleBasedGroup]) -> List[Placement]:
+    def reconcile_pod_groups(self, rbgs: Sequence[RoleBasedGroup], committed: bool = False) -> List[Placement]:
+        """committed=False: every group against the same snapshot (DESIGN.md §3.7), like concurrent reconciles.
+        committed=True: a committed batch (§3.8) in the order given — each group sees the capacity and exclusive
+        domains the groups before it took, so the hints of one call never contradict each other (the controller
+        passes the groups ordered by namespaced name)."""
         blob, runs = self.groups_blob(rbgs)
-        assign, status, domain = self.placer.place_groups(blob)
+        if committed:
+            assign, status, domain, _ = self.placer.place_groups_committed(blob)
+        else:
+            assign, status, domain = self.placer.place_groups(blob)
         out, off = [], 0
         n_nodes = self.placer.n_nodes
         for i, g in enumerate(runs):
