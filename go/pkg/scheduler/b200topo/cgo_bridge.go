@@ -55,6 +55,13 @@ static int32_t rbgtopo_go_update_nodes_delta(rbgtopo_ctx* ctx, int32_t n_changed
   rbgtopo_go_err(ctx, rc, err);
   return rc;
 }
+static int32_t rbgtopo_go_set_exclusive_levels(rbgtopo_ctx* ctx, int32_t n_levels, const int32_t* level_domain,
+                                              const int32_t* level_n_domains, int32_t n_occ, const int32_t* occ,
+                                              uint64_t gen, char* err) {
+  int32_t rc = rbgtopo_set_exclusive_levels(ctx, n_levels, level_domain, level_n_domains, n_occ, occ, gen);
+  rbgtopo_go_err(ctx, rc, err);
+  return rc;
+}
 static int32_t rbgtopo_go_place_groups(rbgtopo_ctx* ctx, const int32_t* groups, int64_t words, int32_t* assign,
                                        int32_t* status, int32_t* domain, char* err) {
   int32_t rc = rbgtopo_place_groups(ctx, groups, words, assign, status, domain);
@@ -156,6 +163,16 @@ func (p *placer) updateNodes(free, owner []int32, gen uint64) error {
 func (p *placer) updateNodesDelta(nodes, free []int32, gen uint64) error {
 	var buf [C.RBGTOPO_GO_ERRLEN]C.char
 	rc := C.rbgtopo_go_update_nodes_delta(p.ctx, C.int32_t(len(nodes)), p32(nodes), p32(free), C.uint64_t(gen), &buf[0])
+	return mkErr(rc, &buf)
+}
+
+// setExclusiveLevels: occupancy mode (DESIGN.md §3.9).  levelDomain holds nLevels rows of n node domains (nil keeps
+// the installed partitions and refreshes the records only); occ holds (node, gid, level) per pod carrying the
+// group-unique-hash label.
+func (p *placer) setExclusiveLevels(nLevels int, levelDomain, levelNDomains, occ []int32, gen uint64) error {
+	var buf [C.RBGTOPO_GO_ERRLEN]C.char
+	rc := C.rbgtopo_go_set_exclusive_levels(p.ctx, C.int32_t(nLevels), p32(levelDomain), p32(levelNDomains),
+		C.int32_t(len(occ)/3), p32(occ), C.uint64_t(gen), &buf[0])
 	return mkErr(rc, &buf)
 }
 

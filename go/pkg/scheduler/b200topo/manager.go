@@ -52,6 +52,32 @@ type Manager struct {
 	nodes  *nodeCache // Node informer -> CSR + free / domain arrays (nodecache.go)
 	hints  sync.Map   // "ns/name" -> map[RoleID]string (node name)
 	gids   gidTable   // dense group ids (domain_owner[] compares against them)
+	// exclusiveKeys: the topology keys exclusive groups may name (DESIGN.md §3.9), keys[0] = the level-0 label.
+	// nil: every key is treated as the level-0 label (the behaviour before levels existed).
+	exclusiveKeys []string
+}
+
+// SetExclusiveKeys configures the topology keys exclusive groups may name; keys[0] must be the level-0 label (the
+// first tier label of the node cache).  nil restores the behaviour without levels.
+func (m *Manager) SetExclusiveKeys(keys []string) { m.exclusiveKeys = append([]string(nil), keys...) }
+
+// exclusiveLevel: the level of an exclusive group's key, or a reason for giving it no hint.  The library places
+// level-0 groups only, and a hint into a domain of the wrong key is worse than none (kube-scheduler enforces the
+// group's required terms on its own key).
+func (m *Manager) exclusiveLevel(rbg *workloadsv1alpha2.RoleBasedGroup) (int32, string) {
+	key, ok := rbg.GetExclusiveKey()
+	if !ok || m.exclusiveKeys == nil {
+		return 0, ""
+	}
+	for i, k := range m.exclusiveKeys {
+		if k == key {
+			if i == 0 {
+				return 0, ""
+			}
+			return int32(i), "exclusive key " + key + " is not the level-0 label: no placement at that level yet"
+		}
+	}
+	return -1, "exclusive key " + key + " is not configured"
 }
 
 // New never fails: without an H100 (RBGTOPO_ENODEVICE) or without the library the manager degrades
@@ -85,6 +111,11 @@ func (m *Manager) ReconcilePodGroup(ctx context.Context, rbg *workloadsv1alpha2.
 	pods, err := m.scheduledPods(ctx, rbg)
 	if err != nil {
 		return err // an API error: requeue like every other LIST failure of the controller
+	}
+	if _, reason := m.exclusiveLevel(rbg); reason != "" {
+		m.hints.Delete(key)
+		logger.Info("no placement hint", "rbg", key, "reason", reason)
+		return nil
 	}
 	g, err := marshalGroup(rbg, pods, snap, m.gids.id(rbg))
 	if err != nil {

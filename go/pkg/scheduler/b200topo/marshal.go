@@ -192,7 +192,7 @@ func marshalGroup(rbg *workloadsv1alpha2.RoleBasedGroup, pods []corev1.Pod, snap
 	blob := make([]int32, 0, words)
 	blob = append(blob, groupsMagic, abiVersion, 1, int32(words), int32(m.pending), 0, 0, 0)
 	blob = append(blob, gid, flags, fixed, int32(q), int32(roleOff), int32(pairOff), int32(len(anchors)/3), int32(anchorOff),
-		0, int32(m.pending), 0, 0)
+		0, int32(m.pending), 0, 0) // +10 exclusive level 0: Manager.exclusiveLevel keeps other keys out
 	blob = append(blob, roleRecs...)
 	blob = append(blob, pair...)
 	blob = append(blob, anchors...)

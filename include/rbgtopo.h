@@ -107,7 +107,8 @@ extern "C" {
  *     +12 replica_off   prefix sum of R over earlier steps (row of the dense
  *                       matrix and index into assign[])
  *     +13 rolerow_off   prefix sum of P over earlier steps
- *     +14,15 reserved (0)
+ *     +14 exclusive level (0; see rbgtopo_set_exclusive_levels)
+ *     +15 reserved (0)
  *   then the variable sections the offsets point at.
  * Replica order inside a step: role records in the given order (the host
  * passes them lexicographically, dependency.go:133-137), ordinal ascending
@@ -179,6 +180,40 @@ int32_t rbgtopo_update_nodes(rbgtopo_ctx* ctx, const int32_t* free_slots,
 int32_t rbgtopo_update_nodes_delta(rbgtopo_ctx* ctx, int32_t n_changed, const int32_t* nodes,
                                    const int32_t* free_slots, uint64_t generation);
 
+/* Exclusive topology at the key each group names (DESIGN.md §3.9).  The annotation
+ * rbg.workloads.x-k8s.io/group-exclusive-topology names a topology key
+ * (api/workloads/constants/annotation.go:23-25) and pod_reconciler.go:126-137,172-231 turns it into two
+ * required terms on that key: pod affinity group-unique-hash In {own key} and pod anti-affinity
+ * group-unique-hash Exists, NotIn {own key}.  The snapshot holds up to RBGTOPO_MAX_EXCL_LEVELS node
+ * partitions ("levels"): level 0 is set_topology's domain[], levels 1..n_levels come from here, each with
+ * its own domain count.  Ownership is then derived from the pods that carry the exclusive label:
+ * occ[n_occ][3] = (node, gid, level) says "a pod of exclusive group gid, whose key is `level`, is bound on
+ * node".  With a = b -> a, -1 (+) x = x and anything else -> -2 (blocked for every group):
+ *   present_L[d] = (+) of the gids of ALL records on nodes of domain d of level L,
+ *   keyed_L[d]   = (+) of the gids of the records OF LEVEL L on nodes of domain d of level L,
+ *   owner_L[n]   = present_L[dom_L(n)] (+) keyed_0[dom_0(n)] (+) ... (+) keyed_K[dom_K(n)],
+ * which restates both terms, including the symmetric enforcement of an existing pod's anti-affinity.
+ * A participating role of an exclusive group g at level L may not use node n when owner_L[n] is not -1 or g.
+ *
+ * The first call after set_topology enters OCCUPANCY MODE: from then on every level's owner vector, level 0
+ * included, is derived from the records (domain_owner of set_topology no longer counts, and
+ * rbgtopo_update_nodes with domain_owner != NULL returns RBGTOPO_EINVAL); set_topology leaves the mode and
+ * drops the levels.  With level-0 records only, owner_0 equals owner[domain[n]] of the domain-owner map the
+ * records imply, and every result equals that of a ctx given that map.
+ *   level_domain [n_levels][n_nodes] (level-major; domain of every node at levels 1..n_levels) and
+ *   level_n_domains[n_levels]: installs the partitions (the call then waits for in-flight batches, like
+ *   set_topology); level_domain == NULL keeps the installed ones (n_levels must match them; 0 before any
+ *   were installed) and refreshes the occupancy only, ordered behind in-flight batches like update_nodes.
+ *   Neither form recomputes base or the background order: ownership does not enter them.
+ * Limits: n_levels <= RBGTOPO_MAX_EXCL_LEVELS - 1; record node in [0, n), gid >= 0, level in [0, n_levels].
+ * Placement: groups and steps at level 0 (word +10 of a GROUPS record, word +14 of a step record = 0) are
+ * placed against owner_0 on every entry point.  A non-zero level returns RBGTOPO_EINVAL without installed
+ * levels or above n_levels, and RBGTOPO_ELIMIT otherwise: this build places at level 0 only. */
+#define RBGTOPO_MAX_EXCL_LEVELS 8
+int32_t rbgtopo_set_exclusive_levels(rbgtopo_ctx* ctx, int32_t n_levels, const int32_t* level_domain,
+                                     const int32_t* level_n_domains, int32_t n_occ, const int32_t* occ,
+                                     uint64_t generation);
+
 /* ---- the hot path ------------------------------------------------------- */
 /* Score + select + greedy-assign one batch of steps (host buffers in, host
  * buffers out; H2D/D2H inside).  Plugs in between step 5 and step 7 of
@@ -227,7 +262,8 @@ int32_t rbgtopo_score_assign(rbgtopo_ctx* ctx, const int32_t* blob,
  *        level, pending replicas, demand, role_flags)
  *     +5 pair_off (pair[q][q])  +6 n_anchors  +7 anchor_off (node, role, count)
  *     +8 assign_off (prefix sum of pending over earlier groups)
- *     +9 n_pending (sum of the roles' pending)  +10,11 reserved
+ *     +9 n_pending (sum of the roles' pending)  +10 exclusive level (0; see
+ *        rbgtopo_set_exclusive_levels)  +11 reserved
  * Output: assign[total pending] in (group, role order, ordinal) order,
  * status[n_groups] (RBGTOPO_PLACED_*), domain[n_groups]. */
 #define RBGTOPO_GROUPS_MAGIC 0x47474252
@@ -306,12 +342,15 @@ int32_t rbgtopo_read_topk(rbgtopo_ctx* ctx, int32_t handle, int32_t rolerow,
  * RBGTOPO_SNAP_ORDER (uint64[slab], key(base, node) form), RBGTOPO_SNAP_ORDER_ALL (uint64[n]; the same
  * buffer as ORDER when world == 1), RBGTOPO_SNAP_POS (int32[n], world == 1 only),
  * RBGTOPO_SNAP_DELTA_REPAIRS (int64[1]: incremental repairs since the last set_topology).  *n_out (may be
- * NULL) receives the element count, also when out_bytes is too small; then RBGTOPO_EINVAL is returned. */
+ * NULL) receives the element count, also when out_bytes is too small; then RBGTOPO_EINVAL is returned.
+ * RBGTOPO_SNAP_LEVEL_OWNER (int32[(n_levels + 1) * n], level-major): the owner vectors of occupancy mode
+ * (rbgtopo_set_exclusive_levels), 0 elements outside it. */
 #define RBGTOPO_SNAP_BASE          0
 #define RBGTOPO_SNAP_ORDER         1
 #define RBGTOPO_SNAP_ORDER_ALL     2
 #define RBGTOPO_SNAP_POS           3
 #define RBGTOPO_SNAP_DELTA_REPAIRS 4
+#define RBGTOPO_SNAP_LEVEL_OWNER   5
 int32_t rbgtopo_read_snapshot(rbgtopo_ctx* ctx, int32_t what, void* out, int64_t out_bytes, int64_t* n_out);
 
 /* ---- node-axis sharding over `world` GPUs (SURVEY.md §8e) --------------- *

@@ -38,6 +38,7 @@ SIGNATURES = {
                                          i32p, C.c_int32, i32p, C.c_uint64]),
     "rbgtopo_update_nodes": (C.c_int32, [C.c_void_p, i32p, i32p, C.c_uint64]),
     "rbgtopo_update_nodes_delta": (C.c_int32, [C.c_void_p, C.c_int32, i32p, i32p, C.c_uint64]),
+    "rbgtopo_set_exclusive_levels": (C.c_int32, [C.c_void_p, C.c_int32, i32p, i32p, C.c_int32, i32p, C.c_uint64]),
     "rbgtopo_score_assign": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, i32p, i32p]),
     "rbgtopo_place_groups": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, i32p, i32p]),
     "rbgtopo_place_groups_committed": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, i32p, i32p, i32p]),

@@ -29,6 +29,7 @@ class Step:
     consumed: List[Tuple[int, int]] = field(default_factory=list)       # (node, amount)
     flags: int = 0
     fixed_domain: int = -1
+    level: int = 0      # exclusive level (word +14; DESIGN.md §3.9)
 
     @property
     def n_replicas(self) -> int:
@@ -70,7 +71,7 @@ class BlobBuilder:
                 body.extend(int(x) for x in c)
             R = s.n_replicas
             table[i] = [s.gid, s.flags, s.fixed_domain, P, role_off, Q, pair_off, len(s.anchors),
-                        anchor_off, len(s.consumed), cons_off, R, racc, pacc, 0, 0]
+                        anchor_off, len(s.consumed), cons_off, R, racc, pacc, s.level, 0]
             racc += R
             pacc += P
         words = base + len(body)
@@ -99,6 +100,7 @@ class Group:
     anchors: List[Tuple[int, int, int]] = field(default_factory=list)
     flags: int = 0
     fixed_domain: int = -1
+    level: int = 0      # exclusive level (word +10; DESIGN.md §3.9)
 
 
 class GroupsBuilder:
@@ -129,7 +131,7 @@ class GroupsBuilder:
                 body.extend(int(x) for x in a)
             pend = sum(r[1] for r in g.roles)
             table[i] = [g.gid, g.flags, g.fixed_domain, q, role_off, pair_off, len(g.anchors), anchor_off,
-                        pacc, pend, 0, 0]
+                        pacc, pend, g.level, 0]
             pacc += pend
         words = base + len(body)
         out = np.zeros(words, dtype=np.int32)

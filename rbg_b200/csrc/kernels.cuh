@@ -182,6 +182,44 @@ __global__ void k_prep(int n, const int* __restrict__ free_, const int* __restri
   }
 }
 
+// ============================================================= k_level_owner
+// Owner vectors of occupancy mode (DESIGN.md §3.9, rbgtopo_set_exclusive_levels).  Level L's vectors live at
+// [L * ls, L * ls + n) of `dom` / `owner` (ls = level_stride(n): the dense-matrix kernels load owners as int4);
+// the per-level domain tables are tab[doff[L] + d] (present) and tab[total_d + doff[L] + d] (keyed).  Owner
+// values merge with  -1 (+) x = x,  x (+) x = x,  anything else -2  (blocked for every group).
+// phase 0: clear the tables; 1: scatter the records (node, gid, level); 2: one gather per node.
+__host__ __device__ __forceinline__ int level_stride(int n) { return (n + 31) & ~31; }
+__device__ __forceinline__ int owner_merge(int a, int b) { return a == -1 ? b : (b == -1 || a == b) ? a : -2; }
+__device__ __forceinline__ void owner_merge_at(int* p, int g) {
+  const int old = atomicCAS(p, -1, g);
+  if (old != -1 && old != g && old != -2) atomicExch(p, -2);  // -2 absorbs: nothing can leave it afterwards
+}
+__global__ void k_level_owner(int phase, int n, int n_lv, const int* __restrict__ dom, const int* __restrict__ doff,
+                              int total_d, int* __restrict__ tab, const int* __restrict__ occ, int n_occ,
+                              int* __restrict__ owner) {
+  const int ls = level_stride(n);
+  const int stride = gridDim.x * blockDim.x;
+  const int i0 = blockIdx.x * blockDim.x + threadIdx.x;
+  if (phase == 0) {
+    for (int i = i0; i < 2 * total_d; i += stride) tab[i] = -1;
+  } else if (phase == 1) {
+    for (int r = i0; r < n_occ; r += stride) {
+      const int node = occ[3 * r], gid = occ[3 * r + 1], lv = occ[3 * r + 2];
+      for (int L = 0; L < n_lv; ++L) {
+        const int d = doff[L] + dom[(size_t)L * ls + node];
+        owner_merge_at(tab + d, gid);                       // present: records count at every level
+        if (L == lv) owner_merge_at(tab + total_d + d, gid);  // keyed: only at the record's own level
+      }
+    }
+  } else {
+    for (int v = i0; v < n; v += stride) {
+      int k = -1;
+      for (int L = 0; L < n_lv; ++L) k = owner_merge(k, tab[total_d + doff[L] + dom[(size_t)L * ls + v]]);
+      for (int L = 0; L < n_lv; ++L) owner[(size_t)L * ls + v] = owner_merge(tab[doff[L] + dom[(size_t)L * ls + v]], k);
+    }
+  }
+}
+
 // base[n] = sum_j w_j * fmin[col_j] + SELF_W * fmin[n]   for the rows of one tile.
 // The tile's contiguous col_idx / edge_w segment and (when it fits) the whole u8
 // fmin vector are staged into shared memory with TMA bulk copies completing on

@@ -147,6 +147,13 @@ struct Topology {
   int n_tiles = 0;
   std::vector<int> h_domain;  // kept for update_nodes validation
   float base_ms = 0.f;
+  // occupancy mode (rbgtopo_set_exclusive_levels, DESIGN.md §3.9): levels 0..n_levels, level L's domain / owner
+  // vector at [L * level_stride(n), + n) of lvl_domain / lvl_owner (row 0 of lvl_domain = domain); the selection
+  // kernels then read lvl_owner's row 0 instead of node_owner (topo_dev)
+  bool occ = false;
+  int n_levels = 0;
+  int lvl_total_d = 0;                      // sum of the levels' domain counts
+  DevBuf<int> lvl_domain, lvl_owner, lvl_doff, lvl_tab, occ_rec;
 };
 
 struct BatchMeta {
@@ -245,7 +252,7 @@ struct rbgtopo_ctx {
   bool base_timing_pending = false;
   // update_nodes staging, double buffered: the copy of update k leaves h_free[k & 1]; the host only
   // waits for update k - 2's H2D (long finished) before overwriting it, not for the refresh chain
-  PinBuf<int> h_free[2], h_owner[2];
+  PinBuf<int> h_free[2], h_owner[2], h_occ[2];
   cudaEvent_t stage_ev[2] = {nullptr, nullptr};
   unsigned stage_idx = 0;
   std::mutex stat_mu;
@@ -271,6 +278,16 @@ struct rbgtopo_ctx {
 namespace {
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
+
+// Exclusive level of a group (word +10) or caller-built step (word +14), DESIGN.md §3.9.  n_levels = the installed
+// levels (0 outside occupancy mode), -1 when unknown (the describe calls accept any level >= 0).  Level 0 is placed
+// everywhere; a higher installed level is a documented limit of this build.
+inline int level_code(int level, int n_levels) {
+  if (level == 0) return RBGTOPO_OK;
+  if (level < 0 || (n_levels >= 0 && level > n_levels)) return RBGTOPO_EINVAL;
+  return n_levels < 0 ? RBGTOPO_OK : RBGTOPO_ELIMIT;
+}
+inline int installed_levels(const rbgtopo_ctx* c) { return c->topo.occ ? c->topo.n_levels : 0; }
 constexpr size_t kFastSmemMax = 200 * 1024;
 constexpr int kMaxExactTerm = 1 << 24;  // pair weights and anchor counts above this can never satisfy spec §3.4
 // Switches, read once when the library loads (INTEGRATION.md §5).
@@ -364,7 +381,7 @@ TopoDev topo_dev(const rbgtopo_ctx* c) {
   t.w = T.w.p;
   t.free_ = T.free_.p;
   t.domain = T.domain.p;
-  t.node_owner = T.node_owner.p;
+  t.node_owner = T.occ ? T.lvl_owner.p : T.node_owner.p;  // occupancy mode: owner_0 derived from the pods
   t.fmin = T.fmin.p;
   t.base = T.base.p;
   t.dom_ptr = T.dom_ptr.p;
@@ -616,7 +633,9 @@ int validate_blob(const rbgtopo_ctx* c, const int32_t* blob, int64_t words, Batc
       if (st[1] & ~(RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG)) STEP_FAIL(RBGTOPO_EINVAL, "step %d: unknown step flags 0x%x", s, st[1]);
       for (int p = 0; p < P; ++p)
         if (roles[4 * p + 3] & ~RBGTOPO_ROLE_EXCLUSIVE) STEP_FAIL(RBGTOPO_EINVAL, "step %d role %d: unknown role flags", s, p);
-      if (st[14] != 0 || st[15] != 0) STEP_FAIL(RBGTOPO_EINVAL, "step %d: reserved words 14/15 must be 0", s);
+      if (st[15] != 0) STEP_FAIL(RBGTOPO_EINVAL, "step %d: reserved word 15 must be 0", s);
+      if (const int lc = level_code(st[14], installed_levels(c)))
+        STEP_FAIL(lc, "step %d: exclusive level %d (%d installed; placement at level 0 only)", s, st[14], installed_levels(c));
       for (int i = 0; i < P * Q; ++i)
         if (pair[i] < 0 || pair[i] > kMaxExactTerm) STEP_FAIL(RBGTOPO_EINVAL, "step %d: pair weight out of [0, 2^24]", s);
       for (int a = 0; a < na; ++a) {
@@ -1523,6 +1542,8 @@ int32_t rbgtopo_set_topology(rbgtopo_ctx* c, int32_t n, int64_t e, const int32_t
     T.max_degp1 = std::max(T.max_degp1, T.h_degp1[i]);
   }
   T.refresh_ready = false;  // new sizes / pointers: re-capture the refresh chain
+  T.occ = false;            // a new topology leaves occupancy mode and drops the levels
+  T.n_levels = 0;
   c->delta_repairs = 0;
   int rc = run_base(c, c->topo_stream, true);
   if (rc) return rc;
@@ -1536,6 +1557,8 @@ int32_t rbgtopo_update_nodes(rbgtopo_ctx* c, const int32_t* free_slots, const in
   std::unique_lock<std::shared_mutex> lk(c->topo_mu);  // no call enqueues while we hold it ...
   Topology& T = c->topo;
   if (!T.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
+  if (owner && T.occ)
+    return fail(RBGTOPO_EINVAL, "domain_owner in occupancy mode: ownership comes from rbgtopo_set_exclusive_levels");
   CK(cudaSetDevice(c->cfg.device));
   cudaStream_t s = c->topo_stream;
   {  // ... and what run_staged / shard_* already enqueued (asynchronously) reads the old snapshot first
@@ -1646,6 +1669,99 @@ int32_t rbgtopo_update_nodes_delta(rbgtopo_ctx* c, int32_t n_changed, const int3
   CK(cudaGetLastError());
   std::lock_guard<std::mutex> g(c->stat_mu);
   c->launches += 3;
+  return RBGTOPO_OK;
+}
+
+// Occupancy mode (DESIGN.md §3.9): the node partitions of the exclusive levels and the pods that carry the exclusive
+// label; k_level_owner derives every level's owner vector on the refresh stream.  Installing partitions waits for the
+// batches in flight (the buffers may move, as with set_topology); an occupancy-only refresh is ordered behind them like
+// update_nodes and reuses its staging double buffer.  Neither touches base or the background order.
+int32_t rbgtopo_set_exclusive_levels(rbgtopo_ctx* c, int32_t n_levels, const int32_t* level_domain,
+                                     const int32_t* level_n_domains, int32_t n_occ, const int32_t* occ,
+                                     uint64_t generation) {
+  if (!c || n_occ < 0 || (n_occ > 0 && !occ) || (level_domain && n_levels > 0 && !level_n_domains))
+    return fail(RBGTOPO_EINVAL, "null argument");
+  if (n_levels < 0 || n_levels > RBGTOPO_MAX_EXCL_LEVELS - 1)
+    return fail(RBGTOPO_EINVAL, "n_levels = %d (0 .. %d)", n_levels, RBGTOPO_MAX_EXCL_LEVELS - 1);
+  std::unique_lock<std::shared_mutex> lk(c->topo_mu);
+  Topology& T = c->topo;
+  if (!T.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
+  const int n = T.n;
+  const bool install = level_domain != nullptr || !T.occ;
+  if (!level_domain && n_levels != (T.occ ? T.n_levels : 0))
+    return fail(RBGTOPO_EINVAL, "level_domain is NULL: n_levels = %d must equal the installed %d", n_levels, T.occ ? T.n_levels : 0);
+  std::vector<int> doff((size_t)n_levels + 2, 0);
+  doff[1] = T.n_domains;
+  if (install) {
+    for (int L = 1; L <= n_levels; ++L) {
+      const int nd = level_n_domains[L - 1];
+      if (nd < 1) return fail(RBGTOPO_EINVAL, "level_n_domains[%d] = %d", L - 1, nd);
+      const int32_t* dl = level_domain + (size_t)(L - 1) * n;
+      for (int i = 0; i < n; ++i)
+        if (dl[i] < 0 || dl[i] >= nd) return fail(RBGTOPO_EINVAL, "level_domain[%d][%d] = %d outside [0, %d)", L - 1, i, dl[i], nd);
+      if ((long long)doff[L] + nd > 0x3FFFFFF0LL) return fail(RBGTOPO_ELIMIT, "domains of all levels exceed 2^30");
+      doff[L + 1] = doff[L] + nd;
+    }
+  }
+  for (int r = 0; r < n_occ; ++r) {
+    const int32_t* o = occ + 3 * (size_t)r;
+    if (o[0] < 0 || o[0] >= n || o[1] < 0 || o[2] < 0 || o[2] > n_levels)
+      return fail(RBGTOPO_EINVAL, "occ[%d] = (%d, %d, %d): node in [0, %d), gid >= 0, level in [0, %d]", r, o[0], o[1], o[2], n, n_levels);
+  }
+  CK(cudaSetDevice(c->cfg.device));
+  cudaStream_t s = c->topo_stream;
+  const int ls = level_stride(n);
+  const int n_lv = n_levels + 1;
+  if (install) {
+    int frc = fence_batches(c, true);
+    if (frc) return frc;
+    CK(cudaStreamSynchronize(s));
+    CK(T.lvl_domain.reserve((size_t)n_lv * ls));
+    CK(T.lvl_owner.reserve((size_t)n_lv * ls));
+    CK(T.lvl_doff.reserve((size_t)n_lv + 1));
+    CK(T.lvl_tab.reserve(2 * (size_t)doff[n_lv]));
+    // on the refresh stream, ahead of k_level_owner (the host arrays are pageable: synchronised below before they go)
+    CK(cudaMemsetAsync(T.lvl_domain.p, 0, T.lvl_domain.cap * 4, s));
+    CK(cudaMemsetAsync(T.lvl_owner.p, 0xFF, T.lvl_owner.cap * 4, s));  // -1, also in the padding the int4 loads reach
+    CK(cudaMemcpyAsync(T.lvl_domain.p, T.domain.p, (size_t)n * 4, cudaMemcpyDeviceToDevice, s));
+    for (int L = 1; L <= n_levels; ++L)
+      CK(cudaMemcpyAsync(T.lvl_domain.p + (size_t)L * ls, level_domain + (size_t)(L - 1) * n, (size_t)n * 4,
+                         cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(T.lvl_doff.p, doff.data(), (size_t)n_lv * 4 + 4, cudaMemcpyHostToDevice, s));
+    CK(cudaStreamSynchronize(s));  // the caller's level_domain and the local doff may go once the call returns
+    T.n_levels = n_levels;
+    T.lvl_total_d = doff[n_lv];
+    T.occ = true;
+  } else {
+    int frc = fence_batches(c, false);  // batches already enqueued read the old owners first
+    if (frc) return frc;
+  }
+  if (n_occ > 0) {
+    const unsigned sb = c->stage_idx++ & 1u;
+    CK(cudaEventSynchronize(c->stage_ev[sb]));
+    CK(c->h_occ[sb].reserve(3 * (size_t)n_occ));
+    memcpy(c->h_occ[sb].p, occ, 3 * (size_t)n_occ * 4);
+    if (T.occ_rec.cap < 3 * (size_t)n_occ) {
+      CK(cudaStreamSynchronize(s));  // an earlier derivation may still read the old records
+      CK(T.occ_rec.reserve(3 * (size_t)n_occ));
+    }
+    CK(cudaMemcpyAsync(T.occ_rec.p, c->h_occ[sb].p, 3 * (size_t)n_occ * 4, cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(c->stage_ev[sb], s));
+  }
+  const int td = T.lvl_total_d;
+  const int th = 256;
+  auto grid = [&](long long work) { return (unsigned)std::max(1LL, std::min((work + th - 1) / th, (long long)c->sm_count * 8)); };
+  k_level_owner<<<grid(2LL * td), th, 0, s>>>(0, n, n_lv, T.lvl_domain.p, T.lvl_doff.p, td, T.lvl_tab.p, T.occ_rec.p, n_occ, T.lvl_owner.p);
+  if (n_occ > 0)
+    k_level_owner<<<grid(n_occ), th, 0, s>>>(1, n, n_lv, T.lvl_domain.p, T.lvl_doff.p, td, T.lvl_tab.p, T.occ_rec.p, n_occ, T.lvl_owner.p);
+  k_level_owner<<<grid(n), th, 0, s>>>(2, n, n_lv, T.lvl_domain.p, T.lvl_doff.p, td, T.lvl_tab.p, T.occ_rec.p, n_occ, T.lvl_owner.p);
+  CK(cudaGetLastError());
+  // the owners are node attributes of both the dense-matrix kernels and selection
+  CK(cudaEventRecord(c->base_ready, s));
+  CK(cudaEventRecord(c->topo_ready, s));
+  T.generation = generation;
+  std::lock_guard<std::mutex> g(c->stat_mu);
+  c->launches += n_occ > 0 ? 3 : 2;
   return RBGTOPO_OK;
 }
 
@@ -1969,6 +2085,7 @@ int build_plan(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int64_t* plan_w
     }
     if (pend > 0x3FFFFFFFLL) GROUP_FAIL(RBGTOPO_ELIMIT, "group %d: pending replicas", g);
     if (rec[0] < 0 || rec[2] < -1 || rec[2] >= n_domains) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: gid / fixed_domain", g);
+    if (const int lc = level_code(rec[10], installed_levels(c))) GROUP_FAIL(lc, "group %d: exclusive level %d", g, rec[10]);
     if (rec[1] & ~(RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG)) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: unknown flags 0x%x", g, rec[1]);
     for (int i = 0; i < q; ++i)
       if (roles[4 * i + 3] & ~RBGTOPO_ROLE_EXCLUSIVE) GROUP_FAIL(RBGTOPO_EINVAL, "group %d role %d: unknown role flags", g, i);
@@ -2174,6 +2291,7 @@ int build_plan(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int64_t* plan_w
 // What the plan geometry needs to know about the snapshot (host side only).
 struct TopoHost {
   int n = 0, n_domains = 0;
+  int n_levels = -1;  // exclusive levels installed (occupancy mode, 0 outside it); -1: unknown (the describe calls)
   const int* degp1 = nullptr;  // [n] deg + 1, or nullptr = all 1
   int max_degp1 = 1;
   long long wsum_max = 0;
@@ -2302,7 +2420,9 @@ int plan_geometry(const TopoHost& T, int lc, Batch* b, const int32_t* gb, int64_
       v->pend = pend;
       v->nw = nw_g;
     }
-    if (rec[0] < 0 || rec[2] < -1 || rec[2] >= n_domains) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: gid / fixed_domain", g);
+    if (rec[0] < 0 || rec[2] < -1 || (rec[10] == 0 && rec[2] >= n_domains)) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: gid / fixed_domain", g);
+    if (const int lc = level_code(rec[10], T.n_levels))
+      GROUP_FAIL(lc, "group %d: exclusive level %d (%d installed; placement at level 0 only)", g, rec[10], std::max(0, T.n_levels));
     if (rec[1] & ~(RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG)) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: unknown flags 0x%x", g, rec[1]);
     long long pc = 0;  // closed neighbourhoods of the scheduled pods
     for (int a = 0; a < rec[6]; ++a) {
@@ -2606,6 +2726,7 @@ int plan_stage(rbgtopo_ctx* c, Batch* b, const int32_t* gb, int64_t words, bool 
   TopoHost th;
   th.n = T.n;
   th.n_domains = T.n_domains;
+  th.n_levels = installed_levels(c);
   th.degp1 = T.h_degp1.data();
   th.max_degp1 = T.max_degp1;
   th.wsum_max = T.wsum_max;
@@ -2932,7 +3053,9 @@ int group_facts(const TopoHost& T, const int32_t* gb, int64_t words, int g, bool
     sf = &w;
   }
   if (phase & 1) {
-    if (rec[0] < 0 || rec[2] < -1 || rec[2] >= T.n_domains) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: gid / fixed_domain", g);
+    if (rec[0] < 0 || rec[2] < -1 || (rec[10] == 0 && rec[2] >= T.n_domains)) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: gid / fixed_domain", g);
+    if (const int lc = level_code(rec[10], T.n_levels))
+      GROUP_FAIL(lc, "group %d: exclusive level %d (%d installed; placement at level 0 only)", g, rec[10], std::max(0, T.n_levels));
     if (rec[1] & ~(RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG)) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: unknown flags 0x%x", g, rec[1]);
     out->pend = (int)sf->pend;
     out->nw = sf->nw;
@@ -3086,6 +3209,7 @@ int place_groups_direct(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_
   TopoHost th;
   th.n = T.n;
   th.n_domains = T.n_domains;
+  th.n_levels = installed_levels(c);
   th.degp1 = T.h_degp1.data();
   th.max_degp1 = T.max_degp1;
   th.wsum_max = T.wsum_max;
@@ -3229,6 +3353,7 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
   TopoHost th;
   th.n = T.n;
   th.n_domains = T.n_domains;
+  th.n_levels = installed_levels(c);
   th.degp1 = T.h_degp1.data();
   th.max_degp1 = T.max_degp1;
   th.wsum_max = T.wsum_max;
@@ -3687,6 +3812,7 @@ int32_t rbgtopo_read_snapshot(rbgtopo_ctx* c, int32_t what, void* out, int64_t o
       src = T.pos.p; n = T.n; elem = 4;
       break;
     case RBGTOPO_SNAP_DELTA_REPAIRS: n = 1; break;
+    case RBGTOPO_SNAP_LEVEL_OWNER: n = T.occ ? (long long)(T.n_levels + 1) * T.n : 0; elem = 4; break;
     default: return fail(RBGTOPO_EINVAL, "what = %d", what);
   }
   if (n_out) *n_out = n;
@@ -3699,6 +3825,11 @@ int32_t rbgtopo_read_snapshot(rbgtopo_ctx* c, int32_t what, void* out, int64_t o
   }
   CK(cudaSetDevice(c->cfg.device));
   CK(cudaEventSynchronize(c->topo_ready));
+  if (what == RBGTOPO_SNAP_LEVEL_OWNER) {  // rows of level_stride(n) on the device, packed rows of n here
+    CK(cudaMemcpy2D(out, (size_t)T.n * 4, T.lvl_owner.p, (size_t)level_stride(T.n) * 4, (size_t)T.n * 4, T.n_levels + 1,
+                    cudaMemcpyDeviceToHost));
+    return RBGTOPO_OK;
+  }
   if (n) CK(cudaMemcpy(out, src, (size_t)n * elem, cudaMemcpyDeviceToHost));
   return RBGTOPO_OK;
 }

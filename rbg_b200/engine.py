@@ -85,6 +85,7 @@ class TopoPlacer:
         self._check(self.lib.rbgtopo_set_topology(self._h, n, len(col_idx), _p(row_ptr), _p(col_idx), _p(edge_w),
                                                   _p(free), _p(domain), len(owner), _p(owner), generation))
         self.n_nodes = n
+        self._n_levels = 0   # a new topology leaves occupancy mode
 
     def update_nodes(self, free=None, domain_owner=None, generation: int = 0) -> None:
         f = None if free is None else _i32(free)
@@ -96,6 +97,25 @@ class TopoPlacer:
         nd, fr = _i32(nodes), _i32(free)
         assert len(nd) == len(fr)
         self._check(self.lib.rbgtopo_update_nodes_delta(self._h, len(nd), _p(nd), _p(fr), generation))
+
+    def set_exclusive_levels(self, level_domain, occupancy, generation: int = 0, level_n_domains=None) -> None:
+        """Occupancy mode (DESIGN.md §3.9).  level_domain: [n_levels][n_nodes] domains of levels 1..n_levels (a list
+        of per-level vectors or a 2-D array; an empty list = level 0 only), or None to keep the installed partitions
+        and refresh the occupancy only.  occupancy: (node, gid, level) per pod carrying the exclusive label.
+        level_n_domains: domains per level (default: largest domain id + 1)."""
+        occ = _i32(np.asarray(occupancy, dtype=np.int64).reshape(-1, 3))
+        if level_domain is None:
+            n_levels = getattr(self, "_n_levels", 0)
+            lv = nd = None
+        else:
+            lv = _i32(np.asarray(level_domain, dtype=np.int64).reshape(-1, self.n_nodes))
+            n_levels = lv.shape[0]
+            nd = _i32(level_n_domains if level_n_domains is not None else [int(r.max()) + 1 for r in lv])
+            if not n_levels:   # install "no levels above 0": a non-NULL level_domain with n_levels = 0
+                lv, nd = np.zeros(1, dtype=np.int32), None
+        self._check(self.lib.rbgtopo_set_exclusive_levels(self._h, n_levels, _p(lv), _p(nd), len(occ), _p(occ),
+                                                          generation))
+        self._n_levels = n_levels
 
     # -- hot path, host buffers in/out
     def score_assign(self, blob: np.ndarray) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
@@ -181,11 +201,12 @@ class TopoPlacer:
         return out
 
     SNAPSHOT = {"base": (0, np.float32), "order": (1, np.uint64), "order_all": (2, np.uint64), "pos": (3, np.int32),
-                "delta_repairs": (4, np.int64)}
+                "delta_repairs": (4, np.int64), "level_owner": (5, np.int32)}
 
     def read_snapshot(self, what: str) -> np.ndarray:
         """One per-snapshot vector exactly as the device holds it (rbgtopo_read_snapshot): "base", "order" (this
-        rank's slab), "order_all", "pos" (world == 1) or "delta_repairs" (one int64)."""
+        rank's slab), "order_all", "pos" (world == 1), "delta_repairs" (one int64) or "level_owner" (occupancy mode:
+        [n_levels + 1][n_nodes], empty outside it)."""
         code, dt = self.SNAPSHOT[what]
         n = C.c_int64()
         rc = self.lib.rbgtopo_read_snapshot(self._h, code, None, 0, C.byref(n))   # sizes only: EINVAL unless empty
@@ -193,7 +214,7 @@ class TopoPlacer:
             self._check(rc)
         out = np.empty(n.value, dtype=dt)
         self._check(self.lib.rbgtopo_read_snapshot(self._h, code, out.ctypes.data_as(C.c_void_p), out.nbytes, C.byref(n)))
-        return out
+        return out.reshape(-1, self.n_nodes) if what == "level_owner" else out
 
     # -- node-axis sharding
     def slab(self) -> Tuple[int, int]:

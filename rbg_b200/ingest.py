@@ -146,3 +146,54 @@ def refresh(topo: Topology, index: NodeIndex, nodes: Sequence[NodeInfo], resourc
         if dname in index.domains:
             owner[index.domains.index(dname)] = gid
     return free, owner
+
+
+@dataclass
+class ExclusiveLevels:
+    """Node partitions of the exclusive-topology keys (DESIGN.md §3.9): keys[0] is the level-0 label (the domain of
+    build_topology), keys[L] for L >= 1 gives domain[L - 1][n] with n_domains[L - 1] domains named names[L - 1]."""
+    keys: Tuple[str, ...]
+    domain: np.ndarray                 # [len(keys) - 1][n] int32
+    n_domains: np.ndarray              # [len(keys) - 1] int32
+    names: List[List[str]]
+
+
+def build_exclusive_levels(nodes: Sequence[NodeInfo], index: NodeIndex, keys: Sequence[str]) -> ExclusiveLevels:
+    """Partitions for rbgtopo_set_exclusive_levels, node ids of `index` (build_topology).  As for level 0, a node
+    without the label gets a domain of its own, and domain ids follow node-name order, so the result does not depend
+    on the order the informer delivered the nodes in."""
+    if not keys:
+        raise ValueError("keys[0] must be the level-0 label")
+    by_name = {nd.name: nd for nd in nodes}
+    if set(by_name) != set(index.names):
+        raise ValueError("node set changed: rebuild the topology")
+    rows, counts, names = [], [], []
+    for key in keys[1:]:
+        ids: Dict[str, int] = {}
+        row = np.zeros(len(index.names), dtype=np.int32)
+        for n, nm in enumerate(index.names):        # index.names is name-sorted
+            v = by_name[nm].labels.get(key)
+            k = v if v is not None else f"node/{nm}"
+            row[n] = ids.setdefault(k, len(ids))
+        rows.append(row)
+        counts.append(max(1, len(ids)))
+        names.append(list(ids))
+    dom = np.stack(rows) if rows else np.zeros((0, len(index.names)), dtype=np.int32)
+    return ExclusiveLevels(tuple(keys), dom, np.asarray(counts, dtype=np.int32), names)
+
+
+def exclusive_occupancy(levels: ExclusiveLevels, index: NodeIndex,
+                        pods: Sequence[Tuple[str, int, str]]) -> np.ndarray:
+    """Records (node, gid, level) for rbgtopo_set_exclusive_levels from the pods that carry the group-unique-hash
+    label: (node name, gid of the pod's group, the topology key its group's annotation names).  Pods on nodes
+    outside the snapshot are skipped; a key outside `levels.keys` is an error (that group cannot be placed)."""
+    pos = {nm: i for i, nm in enumerate(index.names)}
+    out = []
+    for node, gid, key in pods:
+        if node not in pos:
+            continue
+        if key not in levels.keys:
+            raise ValueError(f"exclusive key {key!r} is not configured")
+        out.append((pos[node], int(gid), levels.keys.index(key)))
+    out.sort()
+    return np.asarray(out, dtype=np.int32).reshape(-1, 3)

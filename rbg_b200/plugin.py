@@ -25,6 +25,7 @@ from __future__ import annotations
 
 import ctypes as C
 import json
+import logging
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -97,9 +98,12 @@ class RoleBasedGroup:
     status: Dict[str, RoleStatus] = field(default_factory=dict)
 
 
+RBGTOPO_NO_HINT = -1   # Placement.status of a group the manager gives no hint (B200TopoPodGroupManager.no_hint)
+
+
 @dataclass
 class Placement:
-    status: int                      # 0 all placed, 1 partial, 2 gang failed
+    status: int                      # 0 all placed, 1 partial, 2 gang failed, RBGTOPO_NO_HINT
     nodes: Dict[str, int]            # "{rbg}-{role}-{ordinal}" -> node (-1 = unplaced)
     domain: int = -1
     scores: int = 0                  # (replica x node) scores computed for this group
@@ -287,13 +291,49 @@ class _GroupRun:
 class B200TopoPodGroupManager:
     """Third ``PodGroupManager`` implementation (plugin type "b200-topo")."""
 
-    def __init__(self, placer: TopoPlacer, inner: Optional[str] = "scheduler-plugins"):
+    def __init__(self, placer: TopoPlacer, inner: Optional[str] = "scheduler-plugins",
+                 exclusive_keys: Optional[Sequence[str]] = None):
         """inner: the gang plugin this manager wraps for the PodGroup CR and the pod-group label —
-        "scheduler-plugins" (kube), "volcano" or None (the Go manager takes the implementation object)."""
+        "scheduler-plugins" (kube), "volcano" or None (the Go manager takes the implementation object).
+        exclusive_keys: the topology keys exclusive groups may name (DESIGN.md §3.9), keys[0] = the level-0 label.
+        None: every key is treated as the level-0 label.  With a list, an exclusive group whose key is not keys[0]
+        gets no hint and a logged reason (no_hint[(ns, name)]): the library places level 0 only, and a hint into a
+        domain of the wrong key is worse than none."""
         self.placer = placer
         self.arith = HostArith()
         self.inner = inner
+        self.exclusive_keys = None if exclusive_keys is None else tuple(exclusive_keys)
+        self.no_hint: Dict[Tuple[str, str], str] = {}
         self._hints: Dict[Tuple[str, str], Placement] = {}
+
+    def exclusive_level(self, rbg: RoleBasedGroup) -> Tuple[int, str]:
+        """(level of the group's exclusive key, reason for no hint or "")."""
+        key = rbg.annotations.get(EXCLUSIVE_TOPOLOGY_KEY)
+        if key is None or self.exclusive_keys is None:
+            return 0, ""
+        if key not in self.exclusive_keys:
+            return -1, f"exclusive key {key!r} is not configured"
+        lv = self.exclusive_keys.index(key)
+        return lv, "" if lv == 0 else f"exclusive key {key!r} is not the level-0 label: no placement at that level yet"
+
+    def _split_no_hint(self, rbgs: Sequence[RoleBasedGroup]):
+        """The groups that get a hint, and a no-hint Placement per group that does not (logged, hint dropped)."""
+        keep, skipped = [], {}
+        for i, r in enumerate(rbgs):
+            _, reason = self.exclusive_level(r)
+            if not reason:
+                keep.append(r)
+                continue
+            self._hints.pop((r.namespace, r.name), None)
+            self.no_hint[(r.namespace, r.name)] = reason
+            logging.getLogger(__name__).info("no placement hint for %s/%s: %s", r.namespace, r.name, reason)
+            skipped[i] = Placement(RBGTOPO_NO_HINT, {}, -1, 0)
+        return keep, skipped
+
+    @staticmethod
+    def _merge(rbgs, placed, skipped):
+        it = iter(placed)
+        return [skipped[i] if i in skipped else next(it) for i in range(len(rbgs))]
 
     # -- ReconcilePodGroup(ctx, rbg, ...) for one group -------------------------
     def ReconcilePodGroup(self, rbg: RoleBasedGroup) -> Placement:  # noqa: N802 (reference name)
@@ -323,6 +363,10 @@ class B200TopoPodGroupManager:
         committed=True: a committed batch (§3.8) in the order given — each group sees the capacity and exclusive
         domains the groups before it took, so the hints of one call never contradict each other (the controller
         passes the groups ordered by namespaced name)."""
+        all_rbgs = rbgs
+        rbgs, skipped = self._split_no_hint(rbgs)
+        if not rbgs:
+            return self._merge(all_rbgs, [], skipped)
         blob, runs = self.groups_blob(rbgs)
         if committed:
             assign, status, domain, _ = self.placer.place_groups_committed(blob)
@@ -340,11 +384,13 @@ class B200TopoPodGroupManager:
             p = Placement(int(status[i]), nodes, int(domain[i]), len(nodes) * n_nodes)
             self._hints[(g.rbg.namespace, g.rbg.name)] = p
             out.append(p)
-        return out
+        return self._merge(all_rbgs, out, skipped)
 
     # -- the same loop in Python over single-level batches (rbgtopo_score_assign):
     #    kept as the readable mirror of the C++ loop and for cross-checks.
     def reconcile_pod_groups_by_waves(self, rbgs: Sequence[RoleBasedGroup]) -> List[Placement]:
+        all_rbgs = rbgs
+        rbgs, skipped = self._split_no_hint(rbgs)
         runs = [_GroupRun(r, self.arith) for r in rbgs]
         n_nodes = self.placer.n_nodes
         w = 0
@@ -378,7 +424,7 @@ class B200TopoPodGroupManager:
                 p = Placement(g.status, nodes, g.fixed_domain if g.exclusive else -1, g.scores)
             self._hints[(g.rbg.namespace, g.rbg.name)] = p
             out.append(p)
-        return out
+        return self._merge(all_rbgs, out, skipped)
 
     # -- coordination-aware batching (SURVEY.md §8f rank 4) ------------------------
     def coordination_batches(self, rbg: RoleBasedGroup, max_batches: int = 64) -> List[Dict[str, int]]:
