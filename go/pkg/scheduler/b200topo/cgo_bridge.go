@@ -75,6 +75,13 @@ static int32_t rbgtopo_go_place_groups_committed(rbgtopo_ctx* ctx, const int32_t
   rbgtopo_go_err(ctx, rc, err);
   return rc;
 }
+static int32_t rbgtopo_go_place_groups_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t words, int32_t n_alt,
+                                              int32_t* assign, int32_t* status, int32_t* domain, float* score,
+                                              int32_t* alt_node, float* alt_score, char* err) {
+  int32_t rc = rbgtopo_place_groups_ranked(ctx, groups, words, n_alt, assign, status, domain, score, alt_node, alt_score);
+  rbgtopo_go_err(ctx, rc, err);
+  return rc;
+}
 */
 import "C"
 
@@ -205,4 +212,24 @@ func (p *placer) placeGroupsCommitted(blob []int32) (assign, status, domain []in
 		return nil, nil, nil, 0, err
 	}
 	return assign[:nPending], status[:nGroups], domain[:nGroups], int32(r), nil
+}
+
+// placeGroupsRanked: placeGroups plus, per pending replica, up to nAlt next-best nodes that still have room once its
+// group is placed (DESIGN.md §3.10); altNode[r*nAlt+i] = -1 where there are fewer.  assign / status / domain are
+// placeGroups'.
+func (p *placer) placeGroupsRanked(blob []int32, nAlt int) (assign, status, domain, altNode []int32, err error) {
+	nGroups, nPending := int(blob[2]), int(blob[4])
+	assign = make([]int32, max(nPending, 1))
+	status = make([]int32, max(nGroups, 1))
+	domain = make([]int32, max(nGroups, 1))
+	score := make([]float32, max(nPending, 1))
+	altNode = make([]int32, max(nPending*nAlt, 1))
+	altScore := make([]float32, max(nPending*nAlt, 1))
+	var buf [C.RBGTOPO_GO_ERRLEN]C.char
+	rc := C.rbgtopo_go_place_groups_ranked(p.ctx, p32(blob), C.int64_t(len(blob)), C.int32_t(nAlt), p32(assign), p32(status),
+		p32(domain), (*C.float)(unsafe.Pointer(&score[0])), p32(altNode), (*C.float)(unsafe.Pointer(&altScore[0])), &buf[0])
+	if err = mkErr(rc, &buf); err != nil {
+		return nil, nil, nil, nil, err
+	}
+	return assign[:nPending], status[:nGroups], domain[:nGroups], altNode[:nPending*nAlt], nil
 }

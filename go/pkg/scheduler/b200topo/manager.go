@@ -36,6 +36,10 @@ import (
 // (InjectPodGroupLabels sees a template, not a replica: SURVEY.md §8b "Injection into L4").
 const PlacementHintKey = "rbg.workloads.x-k8s.io/b200-topo-placement"
 
+// PlacementAlternatesKey carries RoleID -> ranked next-best node names (DESIGN.md §3.10) beside the hint, written only
+// when the manager is configured with alternates (SetAlternates) and only for replicas that have some.
+const PlacementAlternatesKey = "rbg.workloads.x-k8s.io/b200-topo-alternates"
+
 // inner is the part of scheduler.PodGroupManager this package wraps (declared here to avoid an
 // import cycle with pkg/scheduler, which imports this package in its factory).
 type inner interface {
@@ -55,7 +59,16 @@ type Manager struct {
 	// exclusiveKeys: the topology keys exclusive groups may name (DESIGN.md §3.9), keys[0] = the level-0 label.
 	// nil: every key is treated as the level-0 label (the behaviour before levels existed).
 	exclusiveKeys []string
+	// alternates: next-best nodes per replica carried beside the hint (0 = the single-node hint of before, at most
+	// RBGTOPO_MAX_ALTERNATES); alts holds them per group like hints
+	alternates int
+	alts       sync.Map // "ns/name" -> map[RoleID][]string (node names)
 }
+
+// SetAlternates configures how many ranked next-best nodes every hinted replica carries (DESIGN.md §3.10): 0 (the
+// default) keeps the single-node hint and the call made; n in [1, 8] places through rbgtopo_place_groups_ranked, which
+// places identically.  Values outside [0, 8] are clamped.
+func (m *Manager) SetAlternates(n int) { m.alternates = min(max(n, 0), 8) }
 
 // SetExclusiveKeys configures the topology keys exclusive groups may name; keys[0] must be the level-0 label (the
 // first tier label of the node cache).  nil restores the behaviour without levels.
@@ -114,6 +127,7 @@ func (m *Manager) ReconcilePodGroup(ctx context.Context, rbg *workloadsv1alpha2.
 	}
 	if _, reason := m.exclusiveLevel(rbg); reason != "" {
 		m.hints.Delete(key)
+		m.alts.Delete(key)
 		logger.Info("no placement hint", "rbg", key, "reason", reason)
 		return nil
 	}
@@ -122,6 +136,15 @@ func (m *Manager) ReconcilePodGroup(ctx context.Context, rbg *workloadsv1alpha2.
 		return err // cycle in the role dependencies etc.: the controller reports the same condition
 	}
 	if g.pending == 0 {
+		return nil
+	}
+	if m.alternates > 0 {
+		assign, status, _, altNode, err := m.placer.placeGroupsRanked(g.blob, m.alternates)
+		if err != nil {
+			return m.degrade(logger, key, err)
+		}
+		m.hints.Store(key, g.roleIDMap(assign, snap, status[0]))
+		m.alts.Store(key, g.roleIDAlternates(altNode, m.alternates, snap, status[0]))
 		return nil
 	}
 	assign, status, _, err := m.placer.placeGroups(g.blob)
@@ -137,6 +160,7 @@ func (m *Manager) ReconcilePodGroup(ctx context.Context, rbg *workloadsv1alpha2.
 // input is the shim's own bug or a spec limit: log it, no hint, no requeue loop either.
 func (m *Manager) degrade(logger interface{ Info(string, ...any) }, key string, err error) error {
 	m.hints.Delete(key)
+	m.alts.Delete(key)
 	if pe, ok := err.(*placerError); ok && pe.deviceTrouble() {
 		logger.Info("placement hints disabled for this reconcile", "rbg", key, "reason", pe.Error())
 		return nil
@@ -151,6 +175,11 @@ func (m *Manager) InjectPodGroupLabels(rbg *workloadsv1alpha2.RoleBasedGroup, pt
 	if h, ok := m.hints.Load(rbg.Namespace + "/" + rbg.Name); ok {
 		if b, err := json.Marshal(h); err == nil {
 			pts.WithAnnotations(map[string]string{PlacementHintKey: string(b)})
+		}
+	}
+	if a, ok := m.alts.Load(rbg.Namespace + "/" + rbg.Name); ok && len(a.(map[string][]string)) > 0 {
+		if b, err := json.Marshal(a); err == nil {
+			pts.WithAnnotations(map[string]string{PlacementAlternatesKey: string(b)})
 		}
 	}
 }

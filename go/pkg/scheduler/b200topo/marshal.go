@@ -220,6 +220,31 @@ func (m *marshalled) roleIDMap(assign []int32, snap *snapshot, status int32) map
 	return out
 }
 
+// roleIDAlternates: altNode[] holds nAlt node indices per replica in assign order (-1 = none); RoleID -> node names,
+// replicas without alternates left out.  A gang failure yields an empty map, like roleIDMap.
+func (m *marshalled) roleIDAlternates(altNode []int32, nAlt int, snap *snapshot, status int32) map[string][]string {
+	out := map[string][]string{}
+	if status == 2 {
+		return out
+	}
+	k := 0
+	for _, ri := range m.order {
+		for c := int32(0); c < m.count[ri]; c++ {
+			var names []string
+			for _, node := range altNode[k*nAlt : (k+1)*nAlt] {
+				if node >= 0 {
+					names = append(names, snap.names[node])
+				}
+			}
+			if len(names) > 0 {
+				out[fmt.Sprintf("%s-%s-%d", m.rbgName, m.names[ri], m.first[ri]+c)] = names
+			}
+			k++
+		}
+	}
+	return out
+}
+
 func demandOf(role *workloadsv1alpha2.RoleSpec) int32 {
 	t := role.GetTemplate()
 	if t == nil {

@@ -291,6 +291,24 @@ int32_t rbgtopo_place_groups(rbgtopo_ctx* ctx, const int32_t* groups,
 int32_t rbgtopo_place_groups_committed(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
                                        int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds);
 
+/* Ranked placement (DESIGN.md §3.10).  rbgtopo_place_groups — same GROUPS blob, same validation and
+ * error codes, bit-identical assign / status / domain on every path — plus, per pending replica r (in
+ * assign order): score[r] = its dense-row score at assign[r], and alt_node[r * n_alt + i] /
+ * alt_score[r * n_alt + i], i < n_alt, the next-best nodes of its row in descending key order (score
+ * descending, node ascending) that still have room for one more replica of its role once the group's
+ * own placements of this call are taken off free[], and, for a participating role of an exclusive
+ * group, lie in the group's reported domain.  Never the replica's own node.  The row of a replica is
+ * the one of its wave that produced the final assignment (groups re-run by the host-driven loop
+ * included).  Unfilled slots: node -1, score -inf; an unplaced replica and every replica of a
+ * gang-failed group get score -inf and no alternates.  n_alt in [0, RBGTOPO_MAX_ALTERNATES], else
+ * RBGTOPO_EINVAL; alt_node / alt_score may be NULL when n_alt == 0.
+ * Documented limit: a ctx with world > 1 holds only its slab of every dense row, so the call returns
+ * RBGTOPO_ELIMIT there.  An RBGTOPO_SPLIT_MIN_GROUPS split does not apply to this call. */
+#define RBGTOPO_MAX_ALTERNATES 8
+int32_t rbgtopo_place_groups_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                    int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain,
+                                    float* score, int32_t* alt_node, float* alt_score);
+
 /* rbgtopo_place_groups pipeline, staged: the groups are compiled into a
  * device-resident multi-wave plan (one step blob, wave-major, expanded on the
  * device), so rbgtopo_run_staged runs ONE score launch for the dense rows of every

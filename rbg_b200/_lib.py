@@ -42,6 +42,8 @@ SIGNATURES = {
     "rbgtopo_score_assign": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, i32p, i32p]),
     "rbgtopo_place_groups": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, i32p, i32p]),
     "rbgtopo_place_groups_committed": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, i32p, i32p, i32p]),
+    "rbgtopo_place_groups_ranked": (C.c_int32, [C.c_void_p, i32p, C.c_int64, C.c_int32, i32p, i32p, i32p, f32p, i32p,
+                                                f32p]),
     "rbgtopo_stage_groups": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p]),
     "rbgtopo_stage": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p]),
     "rbgtopo_run_staged": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32]),

@@ -32,6 +32,7 @@
 #include "select_fast.cuh"
 #include "plan_group.cuh"
 #include "p2p.cuh"
+#include "alternates.cuh"
 
 using namespace rbgtopo;
 
@@ -216,6 +217,9 @@ struct Batch {
   DevBuf<int> cm_int;
   DevBuf<int4> cm_claim;
   DevBuf<int2> cm_dclaim;
+  // ranked placement (place_groups_ranked): jobs | placements | own nodes, then the per-replica lists
+  DevBuf<int> alt;
+  PinBuf<int> h_alt;
   ~Batch() {
     if (stream) cudaStreamDestroy(stream);
     if (stream2) cudaStreamDestroy(stream2);
@@ -1402,6 +1406,7 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
   CK(cudaFuncSetAttribute(k_plan_group<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_plan_group<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CK(cudaFuncSetAttribute(k_plan_group_commit, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
+  CK(cudaFuncSetAttribute(k_alternates, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_plan_group_commit, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CK(cudaFuncSetAttribute(emit_tma_fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)emit_tma_smem_bytes(kEmitStages)));
   // k_emit_tma and k_plan_group are meant to share an SM: both ask for the largest shared-memory carve-out,
@@ -1800,13 +1805,36 @@ struct GroupRun {
   std::vector<int> w_role, w_first, w_count;
   bool done() const { return failed || cur_role >= q; }
 };
+
+// ---- ranked placement (rbgtopo_place_groups_ranked, DESIGN.md §3.10)
+struct RankReq {  // the ranked outputs of one call, indexed like assign
+  int n_alt;
+  float* score;
+  int32_t* alt_node;
+  float* alt_score;
+};
+struct AltRow {  // one role row of one wave: where its dense row is, and its replicas [rep0, rep0 + nrep) in assign order
+  int row, group, role, rep0, nrep;
+};
+// Rows of the host-driven loop: the wave's matrix is overwritten by the next wave, so the row of every (wave, role)
+// that placed a replica is copied out first.  The ranking runs once the groups' placements are final.
+struct KeptRows {
+  const RankReq* rk = nullptr;
+  DevBuf<float> rows;  // [cap][slab_stride]
+  size_t cap = 0;
+  std::vector<AltRow> list;
+};
+int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vector<AltRow>& list, const int32_t* gb,
+                   const int32_t* assign, const int32_t* status, const int32_t* domain, const RankReq& rk);
+void alt_clear_group(const int32_t* gb, int g, const RankReq& rk);
 }  // namespace
 
 // The host-driven wave loop: one batched launch pair per wave, placements fed back
 // through the host.  Exact for every case; used for the groups the device-resident
 // plan cannot finish (`only` != null: just those groups) and as its reference.
 static int32_t place_groups_slow(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign,
-                                 int32_t* status, int32_t* domain, const std::vector<char>* only) {
+                                 int32_t* status, int32_t* domain, const std::vector<char>* only,
+                                 KeptRows* kept = nullptr) {
   if (!c || !gb) return fail(RBGTOPO_EINVAL, "null argument");
   if (words < RBGTOPO_HDR_WORDS || gb[0] != RBGTOPO_GROUPS_MAGIC || gb[1] != RBGTOPO_ABI_VERSION ||
       gb[3] != words)
@@ -1950,15 +1978,26 @@ static int32_t place_groups_slow(rbgtopo_ctx* c, const int32_t* gb, int64_t word
         const int ri = r.w_role[p];
         int ord0 = 0;  // index of this role's first replica inside the group's assign range
         for (int k = 0; k < ri; ++k) ord0 += r.roles[4 * k + 1];
+        const int row = off;  // the role's first replica row in this wave's matrix
+        bool placed = false;
         for (int k = 0; k < r.w_count[p]; ++k, ++off) {
           const int node = w_assign[off];
           assign[r.rec[8] + ord0 + r.w_first[p] + k] = node;
           if (node >= 0) {
             any = true;
+            placed = true;
             r.anchors.push_back(node); r.anchors.push_back(ri); r.anchors.push_back(1);
             r.consumed.push_back(node); r.consumed.push_back(r.roles[4 * ri + 2]);
             r.unplaced[ri] -= 1;
           }
+        }
+        if (kept && placed && !rc) {
+          const size_t stride = (size_t)c->slab_stride, slot = kept->list.size();
+          cudaError_t e = slot < kept->cap ? cudaMemcpyAsync(kept->rows.p + slot * stride, b->matrix.p + (size_t)row * stride,
+                                                             stride * 4, cudaMemcpyDeviceToDevice, stream_of(c, b))
+                                           : cudaErrorInvalidValue;
+          if (e != cudaSuccess) rc = fail(RBGTOPO_ECUDA, "keeping a dense row: %s", cudaGetErrorString(e));
+          kept->list.push_back(AltRow{(int)slot, active[i], ri, r.rec[8] + ord0 + r.w_first[p], r.w_count[p]});
         }
       }
       if (excl && w_domain[i] >= 0 && any) r.fixed_domain = w_domain[i];
@@ -1971,6 +2010,7 @@ static int32_t place_groups_slow(rbgtopo_ctx* c, const int32_t* gb, int64_t word
       if (r.cur_taken >= r.roles[4 * r.cur_role + 1]) { ++r.cur_role; r.cur_taken = 0; }
       while (r.cur_role < r.q && r.roles[4 * r.cur_role + 1] == 0) ++r.cur_role;
     }
+    if (rc) break;
   }
   if (!rc) {
     for (int g = 0; g < ng; ++g) {
@@ -1991,6 +2031,12 @@ static int32_t place_groups_slow(rbgtopo_ctx* c, const int32_t* gb, int64_t word
     c->last = total;
   } else {
     cudaStreamSynchronize(stream_of(c, b));
+  }
+  if (!rc && kept) {  // the placements are final now: rank the kept rows
+    for (int g = 0; g < ng; ++g)
+      if (!only || (*only)[g]) alt_clear_group(gb, g, *kept->rk);
+    rc = run_alternates(c, b, kept->rows.p, kept->list, gb, assign, status, domain, *kept->rk);
+    if (rc) cudaStreamSynchronize(stream_of(c, b));
   }
   release_batch(c, b);
   return rc;
@@ -2041,6 +2087,134 @@ int walk_waves(const int32_t* roles, int q, F&& f) {
 }  // extern "C++"
 int gen_waves(const int32_t* roles, int q, PlanWave* out) {  // out == nullptr: count only
   return walk_waves(roles, q, [out](int i, const PlanWave& w) { if (out) out[i] = w; });
+}
+
+// ---- ranked placement (DESIGN.md §3.10): the role rows to rank and the kernel launch
+const int32_t* group_rec(const int32_t* gb, int g) { return gb + RBGTOPO_HDR_WORDS + (int64_t)g * RBGTOPO_GROUP_WORDS; }
+
+// A group's replicas start with no score and no alternates (what an unplaced or gang-failed replica keeps).
+void alt_clear_group(const int32_t* gb, int g, const RankReq& rk) {
+  const int32_t* rec = group_rec(gb, g);
+  for (int k = 0; k < rec[9]; ++k) {
+    const int64_t r = (int64_t)rec[8] + k;
+    rk.score[r] = -INFINITY;
+    for (int i = 0; i < rk.n_alt; ++i) {
+      rk.alt_node[r * rk.n_alt + i] = -1;
+      rk.alt_score[r * rk.n_alt + i] = -INFINITY;
+    }
+  }
+}
+
+// Role rows of group g whose dense row of a replica is its assign index (the direct and the staged plan paths):
+// one per (wave, role) with a placed replica.
+void plan_alt_rows(const int32_t* gb, int g, const int32_t* assign, std::vector<AltRow>* out) {
+  const int32_t* rec = group_rec(gb, g);
+  const int32_t* roles = gb + rec[4];
+  int ord0[RBGTOPO_MAX_GROUP_ROLES];
+  for (int k = 0, acc = 0; k < rec[3]; ++k) { ord0[k] = acc; acc += roles[4 * k + 1]; }
+  walk_waves(roles, rec[3], [&](int, const PlanWave& w) {
+    for (int p = 0; p < w.n; ++p) {
+      const int rep0 = rec[8] + ord0[w.role[p]] + w.first[p];
+      bool placed = false;
+      for (int k = 0; k < w.count[p]; ++k) placed |= assign[rep0 + k] >= 0;
+      if (placed) out->push_back(AltRow{rep0, g, w.role[p], rep0, w.count[p]});
+    }
+  });
+}
+
+// Number of (wave, role) rows of group g: what the host-driven loop may keep for it.
+size_t group_role_rows(const int32_t* gb, int g) {
+  const int32_t* rec = group_rec(gb, g);
+  size_t n = 0;
+  walk_waves(gb + rec[4], rec[3], [&](int, const PlanWave& w) { n += (size_t)w.n; });
+  return n;
+}
+
+// k_alternates over `list` (rows in `rows`, slab_stride floats apart) on the batch's stream, results scattered into
+// rk; synchronises.  Gang-failed groups are skipped.  The caller cleared the outputs of the groups in `list`.
+int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vector<AltRow>& list, const int32_t* gb,
+                   const int32_t* assign, const int32_t* status, const int32_t* domain, const RankReq& rk) {
+  const int F = rk.n_alt;
+  std::vector<AltJob> jobs;
+  std::vector<int2> used, tmp;
+  std::vector<int> own, jrow;  // jrow: first replica (assign index) of every job
+  std::map<int, int2> placed;  // group -> (first, count) of its aggregated placements in `used`
+  for (const AltRow& r : list) {
+    if (status[r.group] == RBGTOPO_GANG_FAILED) continue;
+    const int32_t* rec = group_rec(gb, r.group);
+    const int32_t* roles = gb + rec[4];
+    auto it = placed.find(r.group);
+    if (it == placed.end()) {  // (node, amount) per node the group's replicas of this call took
+      tmp.clear();
+      for (int q = 0, idx = rec[8]; q < rec[3]; ++q)
+        for (int k = 0; k < roles[4 * q + 1]; ++k, ++idx)
+          if (assign[idx] >= 0) tmp.push_back(make_int2(assign[idx], roles[4 * q + 2]));
+      std::sort(tmp.begin(), tmp.end(), [](int2 a, int2 b2) { return a.x < b2.x; });
+      const int first = (int)used.size();
+      for (const int2& u : tmp) {
+        if ((int)used.size() > first && used.back().x == u.x) used.back().y += u.y;
+        else used.push_back(u);
+      }
+      it = placed.emplace(r.group, make_int2(first, (int)used.size() - first)).first;
+    }
+    const bool part = (rec[1] & RBGTOPO_STEP_EXCLUSIVE) && (roles[4 * r.role + 3] & RBGTOPO_ROLE_EXCLUSIVE);
+    AltJob j{};
+    j.row = r.row;
+    j.demand = roles[4 * r.role + 2];
+    j.dom = part ? (domain[r.group] >= 0 ? domain[r.group] : -2) : ALT_DOM_ANY;
+    j.rep0 = (int)own.size();
+    j.nrep = r.nrep;
+    j.used0 = it->second.x;
+    j.nused = it->second.y;
+    jobs.push_back(j);
+    jrow.push_back(r.rep0);
+    own.insert(own.end(), assign + r.rep0, assign + r.rep0 + r.nrep);
+  }
+  if (jobs.empty()) return RBGTOPO_OK;
+  const size_t smem = (size_t)((c->topo.n + 31) / 32) * 4;
+  if (smem > kFastSmemMax) return fail(RBGTOPO_ELIMIT, "ranked placement: %d nodes exceed the room bitmap", c->topo.n);
+  const size_t w_jobs = jobs.size() * 8, w_used = used.size() * 2, w_own = own.size();
+  const size_t w_in = w_jobs + w_used + w_own, w_out = own.size() * (size_t)(1 + 2 * F);
+  cudaStream_t s = stream_of(c, b);
+  CK(b->alt.reserve(w_in + w_out));
+  CK(b->h_alt.reserve(w_in + w_out));
+  int* h = b->h_alt.p;
+  memcpy(h, jobs.data(), w_jobs * 4);
+  memcpy(h + w_jobs, used.data(), w_used * 4);
+  memcpy(h + w_jobs + w_used, own.data(), w_own * 4);
+  int* d = b->alt.p;
+  CK(cudaMemcpyAsync(d, h, w_in * 4, cudaMemcpyHostToDevice, s));
+  k_alternates<<<(unsigned)jobs.size(), ALT_THREADS, smem, s>>>(topo_dev(c), rows, reinterpret_cast<const AltJob*>(d),
+                                                                 reinterpret_cast<const int2*>(d + w_jobs),
+                                                                 d + w_jobs + w_used, F, d + w_in);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(h + w_in, d + w_in, w_out * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  const int* o = h + w_in;
+  for (size_t j = 0; j < jobs.size(); ++j)
+    for (int k = 0; k < jobs[j].nrep; ++k) {
+      const int* e = o + (size_t)(jobs[j].rep0 + k) * (1 + 2 * F);
+      const int64_t r = (int64_t)jrow[j] + k;
+      memcpy(&rk.score[r], e, 4);
+      if (F > 0) {
+        memcpy(rk.alt_node + r * F, e + 1, (size_t)F * 4);
+        memcpy(rk.alt_score + r * F, e + 1 + F, (size_t)F * 4);
+      }
+    }
+  return RBGTOPO_OK;
+}
+
+// Ranking after a plan pass (direct or staged path; the dense row of a replica is its assign index): every group the
+// pass finished.  The dirty ones are ranked by the host-driven loop that re-runs them.
+int rank_plan(rbgtopo_ctx* c, Batch* b, const int32_t* gb, const int32_t* assign, const int32_t* status,
+              const int32_t* domain, const std::vector<char>& dirty, const RankReq& rk) {
+  std::vector<AltRow> list;
+  for (int g = 0; g < gb[2]; ++g) {
+    if (dirty[g]) continue;
+    alt_clear_group(gb, g, rk);
+    plan_alt_rows(gb, g, assign, &list);
+  }
+  return run_alternates(c, b, b->matrix.p, list, gb, assign, status, domain, rk);
 }
 
 // Builds the plan IN PLACE in b->h_in (pinned); *plan_words = its size.  The GROUPS blob is
@@ -3157,7 +3331,7 @@ int direct_pass2(const TopoHost& th, const int32_t* gb, int64_t words, int ng, l
 }
 
 int place_groups_direct(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign, int32_t* status, int32_t* domain,
-                        std::vector<char>* dirty, bool* handled) {
+                        std::vector<char>* dirty, bool* handled, const RankReq* rk = nullptr) {
   *handled = false;
   // world > 1: replicated selection (every rank places every group over all nodes; the dense matrix and its corrections
   // are limited to the rank's column slab by the kernels themselves), exactly as on the staged path
@@ -3306,6 +3480,10 @@ int place_groups_direct(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_
       (*dirty)[g] = st == RBGTOPO_PLACED_PART;  // `need` of the later waves was predicted with every replica placed
       if (status) status[g] = st;
       if (domain) domain[g] = dm;
+    }
+    if (rk) {
+      const int arc = rank_plan(c, b, gb, assign, status, domain, *dirty, *rk);
+      if (arc) return arc;
     }
     if (prof)
       fprintf(stderr, "[rbgtopo direct] stage %.0f us, pass 1 %.0f us, enqueue 1 %.0f us, pass 2 %.0f us, enqueue 2 %.0f us, wait %.0f us, results %.0f us\n",
@@ -3498,9 +3676,10 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
 
 }  // namespace
 
-int32_t rbgtopo_place_groups(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign,
-                             int32_t* status, int32_t* domain) {
-  if (!c || !gb || !assign) return fail(RBGTOPO_EINVAL, "null argument");
+namespace {
+// rbgtopo_place_groups, and its ranked form when rk != nullptr (status and domain are then not null)
+int32_t place_groups_impl(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign, int32_t* status,
+                          int32_t* domain, const RankReq* rk) {
   std::vector<char> dirty;
   {
     std::shared_lock<std::shared_mutex> lk(c->topo_mu);
@@ -3514,10 +3693,10 @@ int32_t rbgtopo_place_groups(rbgtopo_ctx* c, const int32_t* gb, int64_t words, i
     // the first, and unpacks the first half's results while the second runs.  The GROUPS blob is
     // uploaded once.
     const int ng_all = words >= RBGTOPO_HDR_WORDS ? gb[2] : 0;
-    const bool split = ng_all >= kSplitMinGroups && !kVerifyPlan;
+    const bool split = ng_all >= kSplitMinGroups && !kVerifyPlan && !rk;
     // the direct path (no expanded plan, nothing per step on the host) when it applies
     bool handled = false;
-    const int drc = place_groups_direct(c, gb, words, assign, status, domain, &dirty, &handled);
+    const int drc = place_groups_direct(c, gb, words, assign, status, domain, &dirty, &handled, rk);
     if (drc) return drc;
     Batch* b = nullptr;
     int rc = handled ? RBGTOPO_OK : acquire_batch(c, &b);
@@ -3536,6 +3715,7 @@ int32_t rbgtopo_place_groups(rbgtopo_ctx* c, const int32_t* gb, int64_t words, i
       if (!rc) rc = fetch_batch(c, b, nullptr, nullptr, nullptr);
       auto t4 = now();
       if (!rc) plan_results(b, assign, status, domain, &dirty);
+      if (!rc && rk) rc = rank_plan(c, b, gb, assign, status, domain, dirty, *rk);
       if (prof)
         fprintf(stderr, "[rbgtopo host] plan+stage %.0f us, verify %.0f us, enqueue %.0f us, wait+fetch %.0f us, results %.0f us\n",
                 us(t0, t1), us(t1, t2), us(t2, t3), us(t3, t4), us(t4, now()));
@@ -3591,7 +3771,35 @@ int32_t rbgtopo_place_groups(rbgtopo_ctx* c, const int32_t* gb, int64_t words, i
   bool any = false;
   for (char d : dirty) any |= d != 0;
   if (!any) return RBGTOPO_OK;
-  return place_groups_slow(c, gb, words, assign, status, domain, &dirty);
+  if (!rk) return place_groups_slow(c, gb, words, assign, status, domain, &dirty);
+  KeptRows kept;
+  kept.rk = rk;
+  for (int g = 0; g < (int)dirty.size(); ++g)
+    if (dirty[g]) kept.cap += group_role_rows(gb, g);
+  CK(kept.rows.reserve(std::max<size_t>(1, kept.cap) * (size_t)c->slab_stride));
+  return place_groups_slow(c, gb, words, assign, status, domain, &dirty, &kept);
+}
+}  // namespace
+
+int32_t rbgtopo_place_groups(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign,
+                             int32_t* status, int32_t* domain) {
+  if (!c || !gb || !assign) return fail(RBGTOPO_EINVAL, "null argument");
+  return place_groups_impl(c, gb, words, assign, status, domain, nullptr);
+}
+
+int32_t rbgtopo_place_groups_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t n_alt, int32_t* assign,
+                                    int32_t* status, int32_t* domain, float* score, int32_t* alt_node, float* alt_score) {
+  if (!c || !gb || !assign || !score || (n_alt > 0 && (!alt_node || !alt_score))) return fail(RBGTOPO_EINVAL, "null argument");
+  if (n_alt < 0 || n_alt > RBGTOPO_MAX_ALTERNATES)
+    return fail(RBGTOPO_EINVAL, "n_alt %d outside [0, %d]", n_alt, RBGTOPO_MAX_ALTERNATES);
+  if (c->cfg.world > 1)
+    return fail(RBGTOPO_ELIMIT, "ranked placement needs world == 1: a rank holds only its slab of every dense row");
+  const int64_t ng = words >= RBGTOPO_HDR_WORDS ? std::max<int64_t>(0, std::min<int64_t>(gb[2], words / RBGTOPO_GROUP_WORDS)) : 0;
+  std::vector<int32_t> own_status, own_domain;  // status / domain may be NULL: the ranking still needs them
+  if (!status) { own_status.resize((size_t)ng + 1); status = own_status.data(); }
+  if (!domain) { own_domain.resize((size_t)ng + 1); domain = own_domain.data(); }
+  const RankReq rk{n_alt, score, alt_node, alt_score};
+  return place_groups_impl(c, gb, words, assign, status, domain, &rk);
 }
 
 int32_t rbgtopo_place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign,

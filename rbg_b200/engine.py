@@ -150,6 +150,24 @@ class TopoPlacer:
                                                             _p(domain), C.byref(rounds)))
         return assign[:tp], status[:ng], domain[:ng], rounds.value
 
+    def place_groups_ranked(self, groups_blob: np.ndarray, n_alt: int):
+        """place_groups plus ranked alternates (DESIGN.md §3.10): returns (assign, status, domain, score[R],
+        alt_node[R, n_alt], alt_score[R, n_alt]).  assign / status / domain are those of place_groups; score[r] is
+        replica r's dense-row score at its node, alt_node[r] the next-best nodes of its row that still have room once
+        its group is placed (-1 / -inf where there are fewer), nothing for unplaced and gang-failed replicas."""
+        gb = _i32(groups_blob)
+        ng, tp = int(gb[2]), int(gb[4])
+        assign = np.empty(max(tp, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        score = np.empty(max(tp, 1), dtype=np.float32)
+        alt_node = np.empty((max(tp, 1), max(n_alt, 0)), dtype=np.int32)
+        alt_score = np.empty((max(tp, 1), max(n_alt, 0)), dtype=np.float32)
+        self._check(self.lib.rbgtopo_place_groups_ranked(
+            self._h, _p(gb), len(gb), int(n_alt), _p(assign), _p(status), _p(domain), _p(score, _lib.f32p),
+            _p(alt_node) if n_alt > 0 else None, _p(alt_score, _lib.f32p) if n_alt > 0 else None))
+        return assign[:tp], status[:ng], domain[:ng], score[:tp], alt_node[:tp], alt_score[:tp]
+
     # -- staged (device-resident) batches
     def stage(self, blob: np.ndarray) -> int:
         blob = _i32(blob)

@@ -41,6 +41,7 @@ EXCLUSIVE_TOPOLOGY_KEY = RBG_PREFIX + "group-exclusive-topology"   # annotation.
 ROLE_DISABLE_EXCLUSIVE_KEY = RBG_PREFIX + "role-disable-exclusive"  # annotation.go:29,60
 GANG_SCHEDULING_KEY = RBG_PREFIX + "group-gang-scheduling"          # annotation.go:37
 PLACEMENT_HINT_KEY = RBG_PREFIX + "b200-topo-placement"             # new: RoleID -> node map
+PLACEMENT_ALTERNATES_KEY = RBG_PREFIX + "b200-topo-alternates"       # new: RoleID -> ranked fallback nodes
 SCHEDULER_PLUGIN_NAME = "b200-topo"                                 # --scheduler-name value
 # what the wrapped gang plugins inject into the pod template when gang scheduling is on
 KUBE_POD_GROUP_LABEL = "pod-group.scheduling.sigs.k8s.io/name"      # k8s-scheduler-plugin/manager.go:49,91-98
@@ -107,6 +108,7 @@ class Placement:
     nodes: Dict[str, int]            # "{rbg}-{role}-{ordinal}" -> node (-1 = unplaced)
     domain: int = -1
     scores: int = 0                  # (replica x node) scores computed for this group
+    alternates: Dict[str, List[int]] = field(default_factory=dict)  # "{rbg}-{role}-{ordinal}" -> next-best nodes
 
 
 class HostArith:
@@ -292,13 +294,19 @@ class B200TopoPodGroupManager:
     """Third ``PodGroupManager`` implementation (plugin type "b200-topo")."""
 
     def __init__(self, placer: TopoPlacer, inner: Optional[str] = "scheduler-plugins",
-                 exclusive_keys: Optional[Sequence[str]] = None):
+                 exclusive_keys: Optional[Sequence[str]] = None, alternates: int = 0):
         """inner: the gang plugin this manager wraps for the PodGroup CR and the pod-group label —
         "scheduler-plugins" (kube), "volcano" or None (the Go manager takes the implementation object).
         exclusive_keys: the topology keys exclusive groups may name (DESIGN.md §3.9), keys[0] = the level-0 label.
         None: every key is treated as the level-0 label.  With a list, an exclusive group whose key is not keys[0]
         gets no hint and a logged reason (no_hint[(ns, name)]): the library places level 0 only, and a hint into a
-        domain of the wrong key is worse than none."""
+        domain of the wrong key is worse than none.
+        alternates: next-best nodes per replica carried beside the hint (DESIGN.md §3.10, at most 8).  0 keeps the
+        single-node hint; with n > 0 the snapshot call is rbgtopo_place_groups_ranked, which places identically and
+        also ranks, per replica, the nodes that still have room once its group is placed."""
+        if not 0 <= alternates <= 8:
+            raise ValueError(f"alternates must be in [0, 8], got {alternates}")
+        self.alternates = int(alternates)
         self.placer = placer
         self.arith = HostArith()
         self.inner = inner
@@ -368,20 +376,27 @@ class B200TopoPodGroupManager:
         if not rbgs:
             return self._merge(all_rbgs, [], skipped)
         blob, runs = self.groups_blob(rbgs)
+        alt_node = None
         if committed:
             assign, status, domain, _ = self.placer.place_groups_committed(blob)
+        elif self.alternates > 0:
+            assign, status, domain, _, alt_node, _ = self.placer.place_groups_ranked(blob, self.alternates)
         else:
             assign, status, domain = self.placer.place_groups(blob)
         out, off = [], 0
         n_nodes = self.placer.n_nodes
         for i, g in enumerate(runs):
             nodes: Dict[str, int] = {}
+            alts: Dict[str, List[int]] = {}
             for ri in g.order:
                 role = g.rbg.roles[ri]
                 for c in range(g.pending[ri]):
-                    nodes[f"{g.rbg.name}-{role.name}-{g.first_ordinal[ri] + c}"] = int(assign[off])
+                    key = f"{g.rbg.name}-{role.name}-{g.first_ordinal[ri] + c}"
+                    nodes[key] = int(assign[off])
+                    if alt_node is not None:
+                        alts[key] = [int(x) for x in alt_node[off] if x >= 0]
                     off += 1
-            p = Placement(int(status[i]), nodes, int(domain[i]), len(nodes) * n_nodes)
+            p = Placement(int(status[i]), nodes, int(domain[i]), len(nodes) * n_nodes, alts)
             self._hints[(g.rbg.namespace, g.rbg.name)] = p
             out.append(p)
         return self._merge(all_rbgs, out, skipped)
@@ -488,6 +503,9 @@ class B200TopoPodGroupManager:
         ann = meta.setdefault("annotations", {})
         ann[PLACEMENT_HINT_KEY] = json.dumps({k: v for k, v in sorted(p.nodes.items()) if v >= 0},
                                              separators=(",", ":"))
+        alts = {k: v for k, v in sorted(p.alternates.items()) if v}
+        if alts:
+            ann[PLACEMENT_ALTERNATES_KEY] = json.dumps(alts, separators=(",", ":"))
 
 
 def new_pod_group_manager(scheduler_name: str, placer: TopoPlacer) -> B200TopoPodGroupManager:
