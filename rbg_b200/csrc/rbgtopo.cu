@@ -932,9 +932,12 @@ int launch_select_assign(rbgtopo_ctx* c, Batch* b, cudaStream_t s, const BatchDe
   };
   int CAP, HT;
   table(0, ns, &CAP, &HT);
-  const bool fast = fast_smem_bytes(b->m.max_p, HT, CAP) <= kFastSmemMax;
+  // the table has one delta row per warp of the CTA as launched (>= 4 warps), not per role: sized by max_p alone, a
+  // batch of 1-2 role steps would pass this check and then ask for more than kFastSmemMax at launch.  Per-wave launches
+  // below take at most this many warps and table slots.
+  const int nth = std::max(128, 32 * b->m.max_p);
+  const bool fast = fast_smem_bytes(nth / 32, HT, CAP) <= kFastSmemMax;
   if (b->wave_begin.empty()) {
-    const int nth = std::max(128, 32 * b->m.max_p);
     if (fast)
       k_select_assign_fast<<<ns, nth, fast_smem_bytes(nth / 32, HT, CAP), s>>>(topo_dev(c), d, 0, 0, HT, CAP);
     else if (c->cfg.world != 1)
