@@ -137,6 +137,7 @@ struct CommitDev {
   int* dreader;        // [domains] the same for the owner of the domain (exclusive groups)
   int g;               // the group this CTA places (set by the kernel)
   bool excl;           // ... and whether it is exclusive
+  bool occ;            // occupancy mode (§3.9): owners are per node, derived from the pods' records
 };
 // capacity the groups before cm.g took on `node`
 __device__ __forceinline__ int commit_ext(const CommitDev& cm, int node) {
@@ -148,15 +149,18 @@ __device__ __forceinline__ int commit_ext(const CommitDev& cm, int node) {
   }
   return s;
 }
-// owner of domain `dom` for group cm.g: the gid of the LAST earlier exclusive group that reported it, else `owner`
+// owner of a node of domain `dom` for group cm.g, given the snapshot's `owner`: the gid of the LAST earlier exclusive
+// group that reported the domain, else `owner`.  In occupancy mode `owner` is the node's own derived owner_0, which the
+// records may block inside a domain another node of which is free: the claim is merged into it, so that a claim never
+// unblocks what the records block.
 __device__ __forceinline__ int commit_owner(const CommitDev& cm, int dom, int owner) {
-  int last = -1;
+  int last = -1, claim = -1;
   for (int i = cm.dhead[dom]; i >= 0;) {
     const int2 c = cm.dclaim[i];
-    if (i < cm.g && i > last) { last = i; owner = c.x; }
+    if (i < cm.g && i > last) { last = i; claim = c.x; }
     i = c.y;
   }
-  return owner;
+  return last < 0 ? owner : cm.occ ? owner_merge(owner, claim) : claim;
 }
 // The marks only grow within a round, so a plain L2 load that already shows cm.g or more makes the atomic redundant; the
 // CTAs of a round all read the head of the background order, and this keeps them from queueing on the same addresses.

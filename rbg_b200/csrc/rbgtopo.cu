@@ -3609,6 +3609,7 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
     cm.dclaim = b->cm_dclaim.p;
     cm.reader = ci + o_reader;
     cm.dreader = ci + o_dreader;
+    cm.occ = T.occ;
     int first = 0;  // run[first ..) = the groups of the next round
     while (first < n0) {
       if (rounds >= ng) return fail(RBGTOPO_ECUDA, "internal: committed batch did not converge in %d rounds", ng);

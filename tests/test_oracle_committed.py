@@ -1,11 +1,14 @@
 """CPU: the oracle of the committed batch (tests/committed_oracle.py, DESIGN.md §3.8) keeps the invariants the
 section states — no over-committed node, no exclusive domain shared by two gids unless the caller fixed it, gang
 all-or-nothing, group 0 and groups that touch nothing an earlier group took placed as under snapshot semantics —
-and gives the known answer of a hand-built case."""
+and gives the known answers of hand-built cases; its fast variant equals the literal one, and in occupancy mode
+(DESIGN.md §3.9) its placements keep the records' anti-affinity terms."""
 import numpy as np
 import pytest
 
+import commit_gen as cg
 import groups_gen as gg
+import levels_oracle as lo
 from committed_oracle import result_arrays, run_fleet_committed, run_fleet_snapshot
 from oracle import wave_loop
 from rbg_b200 import synth
@@ -137,3 +140,72 @@ def test_exclusive_domain_taken_by_an_earlier_group():
     assert [s.assign_in_group_order() for s in committed] == [[1], [2]]
     same_gid = [wave_loop.OGroup(f"rbg{i}", 7, [wave_loop.ORole("w", 1)], exclusive=True) for i in range(2)]
     assert [s.result()["domain"] for s in run_fleet_committed(topo, same_gid)] == [0, 0]
+
+
+def _same_states(a, b):
+    return len(a) == len(b) and all(same_result(x, y) for x, y in zip(a, b))
+
+
+@pytest.mark.parametrize("seed", range(6))
+@pytest.mark.parametrize("scarce,exclusive,gang", [(False, False, False), (True, False, True), (False, True, False),
+                                                   (True, True, False)])
+def test_fast_committed_oracle_equals_the_literal_one(seed, scarce, exclusive, gang):
+    """The committed loop over oracle_placer.place_fast gives the literal oracle's bits on every contended case."""
+    topo, groups = contended(seed, scarce=scarce, exclusive=exclusive, gang=gang)
+    assert _same_states(run_fleet_committed(topo, groups, fast=True), run_fleet_committed(topo, groups))
+
+
+def test_fast_committed_oracle_equals_the_literal_one_on_the_bench_fleet():
+    """cfg3's fleet (1 024 groups, 10 000 nodes) up to group 160 through both oracles; the whole batch takes the fast
+    oracle about 1 s on one CPU thread."""
+    import bench
+    from rbg_b200.plugin import B200TopoPodGroupManager
+
+    class Shape:
+        n_nodes = 10000
+    topo = synth.make_topology(10000, seed=0)
+    gblob, _ = B200TopoPodGroupManager(Shape()).groups_blob(bench.to_plugin(bench.fleet_spec("mooncake", 1024, 10000, 0)))
+    groups = wave_loop.groups_from_blob(gblob)
+    assert _same_states(run_fleet_committed(topo, groups, limit=160, fast=True),
+                        run_fleet_committed(topo, groups, limit=160))
+
+
+KEYS = [f"example.com/level-{L}" for L in range(8)]
+
+
+def check_records(lv, occ, groups, states):
+    """Every placement of an exclusive group's participating role keeps the records' anti-affinity terms."""
+    for g, s in zip(groups, states):
+        if not g.exclusive:
+            continue
+        res = s.result()["nodes"]
+        for ri, r in enumerate(g.roles):
+            if not r.exclusive:
+                continue
+            for c in range(s.pending[ri]):
+                node = res[f"{g.name}-{r.name}-{s.first[ri] + c}"]
+                assert node < 0 or not lo.violates(lv, KEYS[:len(lv)], occ, g.gid, 0, node), (g.name, r.name, node)
+
+
+def test_a_claim_never_unblocks_a_node_the_records_block():
+    """DESIGN.md §3.9 known answer: node 1 is blocked for gid 7 by gid 9's rack-keyed record; the first gid-7 group
+    reports domain 0 (which holds node 1), and the second gid-7 group still cannot use node 1."""
+    topo, lv, occ, _, gblob = cg.known_occupancy()
+    owner0 = lo.derive_level_owner(lv, occ)[0]
+    assert owner0.tolist() == [-1, 9, 9, 9]
+    assert lo.violates(lv, KEYS[:2], occ, 7, 0, 1)
+    groups = wave_loop.groups_from_blob(gblob)
+    states = run_fleet_committed(topo, groups, owner0=owner0)
+    assert [s.assign_in_group_order() for s in states] == [[0], [-1]]
+    assert [s.result()["domain"] for s in states] == [0, -1]
+    check_records(lv, occ, groups, states)
+    assert _same_states(states, run_fleet_committed(topo, groups, owner0=owner0, fast=True))
+
+
+@pytest.mark.parametrize("i", range(len(cg.occupancy_cases())))
+def test_generated_occupancy_batches_keep_the_records(i):
+    case, lv, occ, owner0 = cg.occupancy_cases()[i]
+    groups = wave_loop.groups_from_blob(case.blob)
+    states = run_fleet_committed(case.topo, groups, owner0=owner0, fast=True)
+    check_invariants(case.topo, groups, states)
+    check_records(lv, occ, groups, states)
