@@ -131,8 +131,14 @@ typedef struct rbgtopo_config {
   int32_t emit_matrix;   /* reserved: the dense (replica x node) matrix is
                             always materialised                                */
   int32_t chunk_nodes;   /* nodes per CTA work item, 0 = default (2048)        */
-  int32_t reserved[2];
+  int32_t flags;         /* RBGTOPO_CFG_*; unknown bits: RBGTOPO_EINVAL        */
+  int32_t reserved;      /* 0                                                  */
 } rbgtopo_config;
+
+/* config flags */
+#define RBGTOPO_CFG_LEVEL_PLACEMENT 1  /* place groups / steps at exclusive levels >= 1
+                                          (rbgtopo_set_exclusive_levels); without it a
+                                          level >= 1 answers RBGTOPO_ELIMIT */
 
 /* Per-call device timing, milliseconds from CUDA events on the call's stream. */
 typedef struct rbgtopo_timing {
@@ -207,8 +213,19 @@ int32_t rbgtopo_update_nodes_delta(rbgtopo_ctx* ctx, int32_t n_changed, const in
  *   Neither form recomputes base or the background order: ownership does not enter them.
  * Limits: n_levels <= RBGTOPO_MAX_EXCL_LEVELS - 1; record node in [0, n), gid >= 0, level in [0, n_levels].
  * Placement: groups and steps at level 0 (word +10 of a GROUPS record, word +14 of a step record = 0) are
- * placed against owner_0 on every entry point.  A non-zero level returns RBGTOPO_EINVAL without installed
- * levels or above n_levels, and RBGTOPO_ELIMIT otherwise: this build places at level 0 only. */
+ * placed against owner_0 on every entry point.  A level above n_levels (or any level >= 1 without installed
+ * levels) returns RBGTOPO_EINVAL.  A level L in [1, n_levels] is placed only by a ctx created with
+ * RBGTOPO_CFG_LEVEL_PLACEMENT; without the flag it returns RBGTOPO_ELIMIT, so that hosts built against a
+ * level-0-only library keep withholding such hints.  With the flag the rules of level 0 apply with every
+ * level-0 quantity replaced by level L's: a participating role may not use n when owner_L[n] is not -1 or
+ * gid (dense rows and selection), D* = dom_L of the best feasible node of the first participating role and
+ * the participating roles select inside dom_L = D*, fixed_domain and the reported domain are level-L domain
+ * ids (fixed_domain >= level_n_domains[L - 1]: RBGTOPO_EINVAL).  Opted-out roles and non-exclusive groups
+ * are unaffected.  Level-0 groups give the same results with and without the flag.  Every entry point
+ * places at levels >= 1 except rbgtopo_place_groups_committed, which keeps returning RBGTOPO_ELIMIT (a
+ * claim of an earlier group crosses levels: a follow-up).  The describe calls accept any level >= 0.  Installing
+ * partitions makes every staged handle with a step at a level >= 1 stale (run / fetch return RBGTOPO_EINVAL; release
+ * still works): its level ids and fixed domains belong to the partitions it was validated against. */
 #define RBGTOPO_MAX_EXCL_LEVELS 8
 int32_t rbgtopo_set_exclusive_levels(rbgtopo_ctx* ctx, int32_t n_levels, const int32_t* level_domain,
                                      const int32_t* level_n_domains, int32_t n_occ, const int32_t* occ,
@@ -287,7 +304,10 @@ int32_t rbgtopo_place_groups(rbgtopo_ctx* ctx, const int32_t* groups,
  * n_groups, one when no group reads a node or domain an earlier group took), *rounds (may be NULL) =
  * selection rounds run.  Valid for any world: every rank returns the identical result.  Gids need not
  * be distinct.  A group whose table of patched nodes does not fit k_plan_group's shared memory makes
- * the call return RBGTOPO_ELIMIT (there is no per-wave fallback for committed batches). */
+ * the call return RBGTOPO_ELIMIT (there is no per-wave fallback for committed batches).  So does a group
+ * at an exclusive level >= 1, even on a ctx with RBGTOPO_CFG_LEVEL_PLACEMENT: a group at key L_h blocks a
+ * later group at key L_g through dom_{L_g} of each of its pods and through dom_{L_h} of its domain, which
+ * the claim lists of this build (one per level-0 domain) do not express. */
 int32_t rbgtopo_place_groups_committed(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
                                        int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds);
 
@@ -297,7 +317,8 @@ int32_t rbgtopo_place_groups_committed(rbgtopo_ctx* ctx, const int32_t* groups, 
  * alt_score[r * n_alt + i], i < n_alt, the next-best nodes of its row in descending key order (score
  * descending, node ascending) that still have room for one more replica of its role once the group's
  * own placements of this call are taken off free[], and, for a participating role of an exclusive
- * group, lie in the group's reported domain.  Never the replica's own node.  The row of a replica is
+ * group, lie in the group's reported domain (a domain of the group's exclusive level: dom_L[n] = domain[g]).
+ * Never the replica's own node.  The row of a replica is
  * the one of its wave that produced the final assignment (groups re-run by the host-driven loop
  * included).  Unfilled slots: node -1, score -inf; an unplaced replica and every replica of a
  * gang-failed group get score -inf and no alternates.  n_alt in [0, RBGTOPO_MAX_ALTERNATES], else

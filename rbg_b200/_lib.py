@@ -18,7 +18,10 @@ f32p = C.POINTER(C.c_float)
 class Config(C.Structure):
     _fields_ = [("device", C.c_int32), ("rank", C.c_int32), ("world", C.c_int32),
                 ("slots", C.c_int32), ("emit_matrix", C.c_int32), ("chunk_nodes", C.c_int32),
-                ("reserved", C.c_int32 * 2)]
+                ("flags", C.c_int32), ("reserved", C.c_int32)]
+
+
+CFG_LEVEL_PLACEMENT = 1  # RBGTOPO_CFG_LEVEL_PLACEMENT: place groups / steps at exclusive levels >= 1
 
 
 class Timing(C.Structure):

@@ -2,7 +2,7 @@
 // placement pass already wrote (rbgtopo_place_groups_ranked, DESIGN.md §3.10).
 //
 // Replicas of one role in one wave share their dense row S, so the unit of work is that role row (a JOB):
-// one CTA reads the row once with 16-byte loads (and the level-0 domain vector when the role is held to its
+// one CTA reads the row once with 16-byte loads (and the domain vector of the group's level when the role is held to its
 // group's exclusive domain), keeps the top ALT_LIST keys key(S[n], n) of the candidates per thread in
 // registers, merges them per warp and across warps, and writes every replica's list: the merged top list
 // without the replica's own node, truncated to n_alt.  A candidate n has S[n] != -inf, room for one more
@@ -25,12 +25,12 @@ static_assert(ALT_WARPS * ALT_LIST <= 96, "cross-warp merge holds three entries 
 struct AltJob {  // one role row of one wave (8 words)
   int row;       // dense row in `rows` (slab_stride floats apart)
   int demand;
-  int dom;       // required level-0 domain, ALT_DOM_ANY = none (a negative value other than that: no node)
+  int dom;       // required domain of `level`, ALT_DOM_ANY = none (a negative value other than that: no node)
   int rep0;      // first replica in the compact replica arrays (own[], out)
   int nrep;      // replicas of the role in the wave (<= RBGTOPO_MAX_STEP_REPLICAS)
   int used0;     // the group's placements: used[used0 .. used0 + nused), one entry per node
   int nused;
-  int pad;
+  int level;     // the group's exclusive level (DESIGN.md §3.9): `dom` is a domain of it
 };
 
 __device__ __forceinline__ float key_score(unsigned long long k) {  // inverse of orderable_u32 on the high word
@@ -70,6 +70,7 @@ k_alternates(TopoDev t, const float* __restrict__ rows, const AltJob* __restrict
   // ---- scan: per-thread top list in registers
   const float* row = rows + (size_t)J.row * (size_t)t.slab_stride;
   const bool need_dom = J.dom != ALT_DOM_ANY;
+  const int* const dom_l = at_level(t, J.level).domain;
   unsigned long long top[ALT_LIST];
 #pragma unroll
   for (int j = 0; j < ALT_LIST; ++j) top[j] = 0;
@@ -78,7 +79,7 @@ k_alternates(TopoDev t, const float* __restrict__ rows, const AltJob* __restrict
     const int n0 = g << 2;
     const float4 s4 = __ldcs(reinterpret_cast<const float4*>(row + n0));  // read once: do not keep it in L2
     int4 d4 = make_int4(J.dom, J.dom, J.dom, J.dom);
-    if (need_dom) d4 = __ldg(reinterpret_cast<const int4*>(t.domain + n0));  // padded past n: safe
+    if (need_dom) d4 = __ldg(reinterpret_cast<const int4*>(dom_l + n0));  // padded past n: safe
     const float s[4] = {s4.x, s4.y, s4.z, s4.w};
     const int d[4] = {d4.x, d4.y, d4.z, d4.w};
 #pragma unroll

@@ -42,8 +42,10 @@ k_emit_rows(TopoDev t, float* __restrict__ matrix, const int2* __restrict__ rtab
   const int nr = min(n_rows - row0, rb);
   if (tid < nr) {
     const int2 r = __ldg(rtab + row0 + tid);
-    const int dem = r.x >> 6;
-    sRow[tid] = make_int2(__float_as_int((float)(r.x & 31)), (EXCL && (r.x & 32)) ? (dem | (int)0x80000000) : dem);
+    const int dem = (r.x >> 6) & 0x7FFF;
+    // exclusive row: bit 31, and the group's level in bits 24..26 (what the owner test below reads)
+    sRow[tid] = make_int2(__float_as_int((float)(r.x & 31)),
+                          (EXCL && (r.x & 32)) ? (dem | ((r.x >> 21) & 7) << 24 | (int)0x80000000) : dem);
     if (EXCL) sGid[tid] = r.y;
   }
   // ---- node operands of this thread's two groups (in flight together with the row records)
@@ -79,12 +81,13 @@ k_emit_rows(TopoDev t, float* __restrict__ matrix, const int2* __restrict__ rtab
     const float need = __int_as_float(r.x);
     int dem = r.y;
     if (EXCL && dem < 0) {  // exclusive row: nodes of domains another group owns are infeasible
-      dem &= 0x7FFFFFFF;
+      const int* const owner = at_level(t, (dem >> 24) & 7).node_owner;
+      dem &= 0xFFFFFF;
       const int gid = sGid[i];
 #pragma unroll
       for (int j = 0; j < GPT; ++j) {
         if (!live[j]) continue;
-        const int4 ow = __ldg(reinterpret_cast<const int4*>(t.node_owner + n0 + ((tid + j * SCORE_THREADS) << 2)));
+        const int4 ow = __ldg(reinterpret_cast<const int4*>(owner + n0 + ((tid + j * SCORE_THREADS) << 2)));
         float4 o4;
         o4.x = (av[j].x >= dem && (ow.x == -1 || ow.x == gid)) ? need * base4[j].x : -INFINITY;
         o4.y = (av[j].y >= dem && (ow.y == -1 || ow.y == gid)) ? need * base4[j].y : -INFINITY;

@@ -52,9 +52,11 @@ __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.a
 // operands itself so that the caller's register arrays never get an address).
 template <int V>
 __device__ __noinline__ void emit_tile_excl(const int* __restrict__ free_, const float* __restrict__ base,
-                                            const int* __restrict__ node_owner, float* st, int n0, int n1, int gid, int demand,
-                                            float need) {
+                                            const int* __restrict__ owner0, const int* __restrict__ lvl_owner, int ls,
+                                            int level, float* st, int n0, int n1, int gid, int demand, float need) {
   const int lane = threadIdx.x & 31;
+  // the owner vector of the step's exclusive level (DESIGN.md §3.9), picked here to keep it off the caller's registers
+  const int* __restrict__ node_owner = level > 0 ? lvl_owner + (size_t)level * ls : owner0;
   const int len4 = (n1 - n0 + 3) >> 2;
 #pragma unroll
   for (int j = 0; j < V; ++j) {
@@ -161,7 +163,8 @@ k_emit_tma(TopoDev t, BatchDev b, const int* __restrict__ etab, int subs, int it
           // rare: exclusive role of an exclusive step — domains owned by another group are infeasible.
           // Kept out of line so that the common path below stays short (inlined and predicated off, it
           // costs issue slots on every tile).
-          emit_tile_excl<V>(t.free_, t.base, t.node_owner, st, n0, n1, gid, demand, need);
+          emit_tile_excl<V>(t.free_, t.base, t.node_owner, t.lvl_owner, level_stride(t.n), step_level(e[1]), st, n0, n1, gid,
+                            demand, need);
         } else {
 #pragma unroll
           for (int j = 0; j < V; ++j) {

@@ -44,13 +44,31 @@ struct TopoDev {
   const int* node_owner;      // owner[domain[n]]
   const unsigned char* fmin;  // min(free, F) as u8, padded to 16 B
   const float* base;          // W·fmin, padded to slab_stride past slab_hi
-  const int* dom_ptr;         // nodes grouped by domain (CSR)
-  const int* dom_nodes;
   // slab nodes sorted by key(base[n], n) descending (one radix sort per snapshot):
   // the "background" order every unpatched row shares (DESIGN.md §4.3)
   const unsigned long long* order;
   const unsigned long long* order_all;  // the same over ALL nodes (== order when world == 1)
+  // exclusive levels (occupancy mode, DESIGN.md §3.9): level L's domain / owner vector at L * level_stride(n).  The
+  // struct keeps its size (the stride is derived from n): a larger kernel parameter block costs the selection kernels
+  // registers
+  const int* lvl_domain;
+  const int* lvl_owner;
 };
+
+// ---- exclusive level of a step or group (DESIGN.md §3.9): bits 8..10 of the step flags on the device (a caller's
+// step blob carries it in word +14, which plans use for the wave link), bits 21..23 of a row-table record
+constexpr int STEP_LEVEL_SHIFT = 8;
+__host__ __device__ __forceinline__ int step_level(int flags) { return (flags >> STEP_LEVEL_SHIFT) & 7; }
+__host__ __device__ __forceinline__ int level_stride(int n) { return (n + 31) & ~31; }
+// The snapshot as a group at level L sees it: domain / node_owner are level L's vectors.  Level 0 keeps the
+// pointers it has (row 0 of lvl_domain / lvl_owner is the same data).
+__device__ __forceinline__ TopoDev at_level(TopoDev t, int L) {
+  if (L > 0) {
+    t.domain = t.lvl_domain + (size_t)L * level_stride(t.n);
+    t.node_owner = t.lvl_owner + (size_t)L * level_stride(t.n);
+  }
+  return t;
+}
 
 struct BatchDev {
   const int* blob;
@@ -91,11 +109,11 @@ __host__ __device__ __forceinline__ int emit_pack_role(int count, int demand, in
   return count | (need << 6) | ((flags & RBGTOPO_ROLE_EXCLUSIVE) << 11) | (demand << 12);
 }
 
-// ---- row table of a multi-wave plan (emit_rows.cuh): per dense row {need | exclusive << 5 | demand << 6, gid}
-// (need <= RBGTOPO_NEED_CAP < 32).  `exclusive` = the step and the role are exclusive: only then does a
-// background row depend on the group (nodes of domains another group owns are infeasible).
-__host__ __device__ __forceinline__ int emit_pack_row(int demand, int need, bool rexcl) {
-  return need | ((rexcl ? 1 : 0) << 5) | (demand << 6);
+// ---- row table of a multi-wave plan (emit_rows.cuh): per dense row {need | exclusive << 5 | demand << 6 | level << 21,
+// gid} (need <= RBGTOPO_NEED_CAP < 32, demand <= 32767).  `exclusive` = the step and the role are exclusive: only then
+// does a background row depend on the group (nodes another group owns at the group's level are infeasible).
+__host__ __device__ __forceinline__ int emit_pack_row(int demand, int need, bool rexcl, int level) {
+  return need | ((rexcl ? 1 : 0) << 5) | (demand << 6) | (level << 21);
 }
 
 // ---------------------------------------------------------------- helpers
@@ -188,7 +206,6 @@ __global__ void k_prep(int n, const int* __restrict__ free_, const int* __restri
 // the per-level domain tables are tab[doff[L] + d] (present) and tab[total_d + doff[L] + d] (keyed).  Owner
 // values merge with  -1 (+) x = x,  x (+) x = x,  anything else -2  (blocked for every group).
 // phase 0: clear the tables; 1: scatter the records (node, gid, level); 2: one gather per node.
-__host__ __device__ __forceinline__ int level_stride(int n) { return (n + 31) & ~31; }
 __device__ __forceinline__ int owner_merge(int a, int b) { return a == -1 ? b : (b == -1 || a == b) ? a : -2; }
 __device__ __forceinline__ void owner_merge_at(int* p, int g) {
   const int old = atomicCAS(p, -1, g);

@@ -111,13 +111,13 @@ __global__ void __launch_bounds__(32 * PLAN_WARPS) k_plan_etab(const int* __rest
       int r0 = S->rec[8] - row_base + S->cum[RBGTOPO_MAX_GROUP_ROLES];  // first dense row of the step
       for (int k = 0; k < lane; ++k) r0 += S->count[k];
       const bool rexcl = (S->rec[1] & RBGTOPO_STEP_EXCLUSIVE) && (S->roles[4 * ri + 3] & RBGTOPO_ROLE_EXCLUSIVE);
-      const int2 rr = make_int2(emit_pack_row(S->roles[4 * ri + 2], need, rexcl), S->rec[0]);
+      const int2 rr = make_int2(emit_pack_row(S->roles[4 * ri + 2], need, rexcl, S->rec[10]), S->rec[0]);
       for (int k = 0; k < S->count[lane]; ++k) rtab[r0 + k] = rr;
     }
     e[4 + lane] = packed;
   } else if (lane == 8) {
     e[0] = S->rec[0];
-    e[1] = S->rec[1] & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG);
+    e[1] = (S->rec[1] & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG)) | S->rec[10] << STEP_LEVEL_SHIFT;
     e[2] = P;
     e[3] = S->rec[8] - row_base + S->cum[RBGTOPO_MAX_GROUP_ROLES];
   }
@@ -191,7 +191,9 @@ __global__ void __launch_bounds__(32 * PLAN_WARPS) k_expand_plan(const int* __re
     int n = 0;
     for (int k = 0; k < P; ++k) n += S->count[k];
     int4 v;
-    if (lane == 0) v = make_int4(gid, gflags & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG), (gflags & RBGTOPO_STEP_EXCLUSIVE) ? gfixed : -1, P);
+    if (lane == 0)
+      v = make_int4(gid, (gflags & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG)) | S->rec[10] << STEP_LEVEL_SHIFT,
+                    (gflags & RBGTOPO_STEP_EXCLUSIVE) ? gfixed : -1, P);
     else if (lane == 1) v = make_int4(sec, q, pair_off, na + i0);
     else if (lane == 2) v = make_int4(anchor_off, i0, cons_off, n);
     else v = make_int4(rep, row, next, i0);

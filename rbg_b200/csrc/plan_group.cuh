@@ -356,7 +356,7 @@ __global__ void __launch_bounds__(32 * RTAB_WARPS) k_group_rtab(const int* __res
       for (int j = 0; j < q; ++j)
         if (sP[wi][ri * q + j] > 0) need += sR[wi][4 * j + 1] - sPl[wi][j];
       const bool rexcl = excl && (sR[wi][4 * ri + 3] & RBGTOPO_ROLE_EXCLUSIVE);
-      sRec[wi][lane] = emit_pack_row(sR[wi][4 * ri + 2], max(0, min(need, RBGTOPO_NEED_CAP)), rexcl);
+      sRec[wi][lane] = emit_pack_row(sR[wi][4 * ri + 2], max(0, min(need, RBGTOPO_NEED_CAP)), rexcl, rec[10] & 7);
     }
     __syncwarp();
     for (int p = 0; p < P; ++p) {
@@ -460,6 +460,8 @@ __device__ __forceinline__ void plan_group_body(TopoDev t, BatchDev b, int QB, i
   } else {
     h = load_hdr(b, step);  // in flight while the table is cleared
   }
+  // every wave of the group is placed at its exclusive level (a committed batch has level-0 groups only)
+  t = at_level(t, DIRECT ? b.blob[RBGTOPO_HDR_WORDS + (size_t)step * RBGTOPO_GROUP_WORDS + 10] : step_level(h.flags));
   for (int i = tid; i < HT; i += nthreads) {
     T.node[i] = -1;
     T.cons[i] = 0;

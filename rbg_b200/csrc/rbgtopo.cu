@@ -154,12 +154,15 @@ struct Topology {
   bool occ = false;
   int n_levels = 0;
   int lvl_total_d = 0;                      // sum of the levels' domain counts
+  std::vector<int> lvl_nd;                  // [n_levels + 1] domain count of every level (fixed_domain checks)
   DevBuf<int> lvl_domain, lvl_owner, lvl_doff, lvl_tab, occ_rec;
 };
 
 struct BatchMeta {
   int n_steps = 0, total_r = 0, total_p = 0, max_p = 1, max_k = 1, max_q = 1;
   bool any_excl_unknown = false;
+  bool any_level = false;    // a step at an exclusive level >= 1: the <true> selection kernels (a caller's blob: stage_into
+                             // moves the level from word +14 into the step flags)
   long long words = 0;
   long long h2d_words = 0;   // what staging actually uploaded
   long long scores = 0;      // sum R * N
@@ -176,6 +179,7 @@ struct Batch {
   bool early_emit = false;    // plan_stage already enqueued the dense-matrix kernel of the next pass (+ its two events)
   bool d2h_enqueued = false;  // enqueue_d2h ran for the last pass; fetch_batch only has to wait
   uint64_t epoch = 0;         // topology epoch the batch was validated / sized against (set_topology bumps it)
+  uint64_t lvl_epoch = 0;     // partition install the batch's levels >= 1 (b->m.any_level) were validated against
   cudaStream_t stream = nullptr;
   cudaStream_t stream2 = nullptr;  // selection of multi-wave plans, concurrent with the dense-matrix kernel
   cudaEvent_t ev[8] = {};          // 0/1 staging, 2/3 fork/join of stream2, 4/5 D2H, 6 snapshot fence
@@ -236,6 +240,8 @@ struct rbgtopo_ctx {
   int slab_lo = 0, slab_hi = 0, slab_stride = 0, lc = 1, chunk = 2048;
   std::shared_mutex topo_mu;  // update = exclusive, score calls = shared
   uint64_t topo_epoch = 0;    // bumped by set_topology: handles staged against an older topology are stale
+  uint64_t lvl_epoch = 0;     // bumped by every partition install: handles with steps at levels >= 1 staged before it
+                              // are stale (their level ids and fixed domains belong to the old partitions)
   std::mutex pool_mu;
   Topology topo;
   std::vector<std::unique_ptr<Batch>> batches;
@@ -285,13 +291,17 @@ inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
 // Exclusive level of a group (word +10) or caller-built step (word +14), DESIGN.md §3.9.  n_levels = the installed
 // levels (0 outside occupancy mode), -1 when unknown (the describe calls accept any level >= 0).  Level 0 is placed
-// everywhere; a higher installed level is a documented limit of this build.
-inline int level_code(int level, int n_levels) {
+// everywhere; an installed level >= 1 only where `place` (a ctx created with RBGTOPO_CFG_LEVEL_PLACEMENT, and not
+// for committed batches): elsewhere it is a documented limit, which hosts read as "no hint".
+inline int level_code(int level, int n_levels, bool place) {
   if (level == 0) return RBGTOPO_OK;
   if (level < 0 || (n_levels >= 0 && level > n_levels)) return RBGTOPO_EINVAL;
-  return n_levels < 0 ? RBGTOPO_OK : RBGTOPO_ELIMIT;
+  return (n_levels < 0 || place) ? RBGTOPO_OK : RBGTOPO_ELIMIT;
 }
 inline int installed_levels(const rbgtopo_ctx* c) { return c->topo.occ ? c->topo.n_levels : 0; }
+inline bool places_levels(const rbgtopo_ctx* c) { return (c->cfg.flags & RBGTOPO_CFG_LEVEL_PLACEMENT) != 0; }
+// Domain count of installed level L (level_code accepted it): the range of a fixed domain at that level.
+inline int level_domains(const Topology& T, int L) { return L == 0 ? T.n_domains : T.lvl_nd[L]; }
 constexpr size_t kFastSmemMax = 200 * 1024;
 constexpr int kMaxExactTerm = 1 << 24;  // pair weights and anchor counts above this can never satisfy spec §3.4
 // Switches, read once when the library loads (INTEGRATION.md §5).
@@ -388,10 +398,10 @@ TopoDev topo_dev(const rbgtopo_ctx* c) {
   t.node_owner = T.occ ? T.lvl_owner.p : T.node_owner.p;  // occupancy mode: owner_0 derived from the pods
   t.fmin = T.fmin.p;
   t.base = T.base.p;
-  t.dom_ptr = T.dom_ptr.p;
-  t.dom_nodes = T.dom_nodes.p;
   t.order = T.order.p;
   t.order_all = c->cfg.world > 1 ? T.order_all.p : T.order.p;
+  t.lvl_domain = T.lvl_domain.p;
+  t.lvl_owner = T.lvl_owner.p;
   return t;
 }
 
@@ -618,7 +628,14 @@ int validate_blob(const rbgtopo_ctx* c, const int32_t* blob, int64_t words, Batc
     if (R < 1 || R > RBGTOPO_MAX_STEP_REPLICAS) STEP_FAIL(RBGTOPO_ELIMIT, "step %d: %d replicas", s, R);
     if (!in(st[4], 4LL * P) || !in(st[6], (long long)P * Q) || !in(st[8], 3LL * na) || !in(st[10], 2LL * nc))
       STEP_FAIL(RBGTOPO_EINVAL, "step %d: section out of bounds", s);
-    if (st[2] < -1 || st[2] >= T.n_domains) STEP_FAIL(RBGTOPO_EINVAL, "step %d: fixed_domain", s);
+    // exclusive level: word +14 of a caller's step, the step flags of a plan (whose word +14 is the wave link)
+    const int lv = trusted ? step_level(st[1]) : st[14];
+    if (!trusted) {
+      if (const int lc = level_code(lv, installed_levels(c), places_levels(c)))
+        STEP_FAIL(lc, "step %d: exclusive level %d (%d installed%s)", s, lv, installed_levels(c),
+                  places_levels(c) ? "" : "; placement at level 0 only");
+    }
+    if (st[2] < -1 || st[2] >= level_domains(T, lv)) STEP_FAIL(RBGTOPO_EINVAL, "step %d: fixed_domain %d (level %d)", s, st[2], lv);
     const int32_t* roles = blob + st[4];
     const int32_t* pair = blob + st[6];
     const int32_t* anc = blob + st[8];
@@ -638,8 +655,6 @@ int validate_blob(const rbgtopo_ctx* c, const int32_t* blob, int64_t words, Batc
       for (int p = 0; p < P; ++p)
         if (roles[4 * p + 3] & ~RBGTOPO_ROLE_EXCLUSIVE) STEP_FAIL(RBGTOPO_EINVAL, "step %d role %d: unknown role flags", s, p);
       if (st[15] != 0) STEP_FAIL(RBGTOPO_EINVAL, "step %d: reserved word 15 must be 0", s);
-      if (const int lc = level_code(st[14], installed_levels(c)))
-        STEP_FAIL(lc, "step %d: exclusive level %d (%d installed; placement at level 0 only)", s, st[14], installed_levels(c));
       for (int i = 0; i < P * Q; ++i)
         if (pair[i] < 0 || pair[i] > kMaxExactTerm) STEP_FAIL(RBGTOPO_EINVAL, "step %d: pair weight out of [0, 2^24]", s);
       for (int a = 0; a < na; ++a) {
@@ -661,7 +676,7 @@ int validate_blob(const rbgtopo_ctx* c, const int32_t* blob, int64_t words, Batc
         STEP_FAIL(RBGTOPO_EINEXACT, "step %d role %d: max score bound >= 2^24 (anchor weight %lld x row weight %lld)", s, p, amax, row_w);
     }
     if (st[4] & 3) STEP_FAIL(RBGTOPO_EINVAL, "step %d: role_off must be a multiple of 4 words", s);
-    if (st[15] < 0 || st[15] > na || (st[14] != 0 && (st[14] <= s || st[14] >= ns)))
+    if (trusted && (st[15] < 0 || st[15] > na || (st[14] != 0 && (st[14] <= s || st[14] >= ns))))
       STEP_FAIL(RBGTOPO_EINVAL, "step %d: bad wave links", s);
     // patched-node scratch: closed neighbourhoods of the anchors + consumed nodes.  Records of
     // earlier waves (the last st[15]) are filled on the device: any node.
@@ -692,6 +707,7 @@ int validate_blob(const rbgtopo_ctx* c, const int32_t* blob, int64_t words, Batc
     m->max_k = std::max(m->max_k, st[11]);
     m->max_q = std::max(m->max_q, st[5]);
     if ((st[1] & RBGTOPO_STEP_EXCLUSIVE) && st[2] < 0) m->any_excl_unknown = true;
+    if (trusted ? step_level(st[1]) != 0 : st[14] != 0) m->any_level = true;
   }
   if (blob[4] != racc || blob[5] != pacc) return fail(RBGTOPO_EINVAL, "blob totals mismatch");
   if (emit_items(ns, c->lc) > 0x7FFFFFF0LL) return fail(RBGTOPO_ELIMIT, "steps x chunks exceed 2^31 work items");
@@ -780,10 +796,17 @@ int stage_into(rbgtopo_ctx* c, Batch* b, const int32_t* blob, int64_t words) {
   if (rc) return rc;
   b->m.h2d_words = (long long)in_words;
   b->epoch = c->topo_epoch;
+  b->lvl_epoch = c->lvl_epoch;
   b->tev = timing_events(c);
   b->perm_n = 0;
   if (b->tev) CK(cudaEventRecord(b->ev[0], s));  // staging touches the batch's own buffers only; run_batch waits for a pending refresh
   if (!in_place) memcpy(b->h_in.p, blob, (size_t)words * 4);
+  if (m.any_level && !in_place)  // the kernels read a step's level from its flags: word +14 is the wave link of plans
+    for (int s2 = 0; s2 < m.n_steps; ++s2) {
+      int32_t* st = b->h_in.p + RBGTOPO_HDR_WORDS + (size_t)s2 * RBGTOPO_STEP_WORDS;
+      st[1] |= st[14] << STEP_LEVEL_SHIFT;
+      st[14] = 0;
+    }
   memcpy(b->h_in.p + words, m.poff.data(), ((size_t)m.n_steps + 1) * 4);
   CK(cudaMemcpyAsync(b->blob.p, b->h_in.p, in_words * 4, cudaMemcpyHostToDevice, s));
   if (b->tev) CK(cudaEventRecord(b->ev[1], s));
@@ -939,11 +962,11 @@ int launch_select_assign(rbgtopo_ctx* c, Batch* b, cudaStream_t s, const BatchDe
   const bool fast = fast_smem_bytes(nth / 32, HT, CAP) <= kFastSmemMax;
   if (b->wave_begin.empty()) {
     if (fast)
-      k_select_assign_fast<<<ns, nth, fast_smem_bytes(nth / 32, HT, CAP), s>>>(topo_dev(c), d, 0, 0, HT, CAP);
+      (b->m.any_level ? k_select_assign_fast<true> : k_select_assign_fast<false>)<<<ns, nth, fast_smem_bytes(nth / 32, HT, CAP), s>>>(topo_dev(c), d, 0, 0, HT, CAP);
     else if (c->cfg.world != 1)
       return fail(RBGTOPO_ELIMIT, "a step's patched set exceeds shared memory: world > 1 must use the shard calls");
     else
-      k_select_assign<<<ns, 32 * b->m.max_p, select_smem_bytes(b->m.max_p), s>>>(topo_dev(c), d, 0, 0);
+      (b->m.any_level ? k_select_assign<true> : k_select_assign<false>)<<<ns, 32 * b->m.max_p, select_smem_bytes(b->m.max_p), s>>>(topo_dev(c), d, 0, 0);
     ++*launches;
     return RBGTOPO_OK;
   }
@@ -982,10 +1005,10 @@ int launch_select_assign(rbgtopo_ctx* c, Batch* b, cudaStream_t s, const BatchDe
     if (fast) {
       const int nth = std::max(128, 32 * b->wave_maxp[w]);
       table(b->wave_begin[w], b->wave_begin[w + 1], &CAP, &HT);
-      k_select_assign_fast<<<n, nth, fast_smem_bytes(nth / 32, HT, CAP), s>>>(
+      (b->m.any_level ? k_select_assign_fast<true> : k_select_assign_fast<false>)<<<n, nth, fast_smem_bytes(nth / 32, HT, CAP), s>>>(
           topo_dev(c), d, b->wave_begin[w], wave_mode, HT, CAP);
     } else
-      k_select_assign<<<n, 32 * b->wave_maxp[w], select_smem_bytes(b->wave_maxp[w]), s>>>(
+      (b->m.any_level ? k_select_assign<true> : k_select_assign<false>)<<<n, 32 * b->wave_maxp[w], select_smem_bytes(b->wave_maxp[w]), s>>>(
           topo_dev(c), d, b->wave_begin[w], wave_mode);
     ++*launches;
   }
@@ -1312,6 +1335,7 @@ Batch* batch_of(rbgtopo_ctx* c, int handle, bool any_epoch = false) {
   Batch* b = c->batches[handle].get();
   if (!(b->in_use && b->staged)) return nullptr;
   if (!any_epoch && b->epoch != c->topo_epoch) return nullptr;  // sizes / offsets belong to the old topology
+  if (!any_epoch && b->m.any_level && b->lvl_epoch != c->lvl_epoch) return nullptr;  // levels of old partitions
   return b;
 }
 
@@ -1378,6 +1402,7 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
   *out = nullptr;
   if (cfg->world < 1 || cfg->rank < 0 || cfg->rank >= cfg->world)
     return fail(RBGTOPO_EINVAL, "rank %d / world %d", cfg->rank, cfg->world);
+  if (cfg->flags & ~RBGTOPO_CFG_LEVEL_PLACEMENT) return fail(RBGTOPO_EINVAL, "unknown config flags 0x%x", cfg->flags);
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess || ndev <= 0)
@@ -1403,8 +1428,10 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
   CK(cudaEventCreate(&c->ev_base_b));
   CK(cudaEventCreateWithFlags(&c->fence_ev, cudaEventDisableTiming));
   for (auto& e : c->stage_ev) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  CK(cudaFuncSetAttribute(k_select_assign_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
-  CK(cudaFuncSetAttribute(k_shard_select, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
+  for (auto* f : {k_select_assign_fast<false>, k_select_assign_fast<true>})
+    CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
+  for (auto* f : {k_shard_select<false>, k_shard_select<true>})
+    CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_plan_group<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_plan_group<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_plan_group<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
@@ -1552,6 +1579,7 @@ int32_t rbgtopo_set_topology(rbgtopo_ctx* c, int32_t n, int64_t e, const int32_t
   T.refresh_ready = false;  // new sizes / pointers: re-capture the refresh chain
   T.occ = false;            // a new topology leaves occupancy mode and drops the levels
   T.n_levels = 0;
+  T.lvl_nd.clear();
   c->delta_repairs = 0;
   int rc = run_base(c, c->topo_stream, true);
   if (rc) return rc;
@@ -1739,6 +1767,9 @@ int32_t rbgtopo_set_exclusive_levels(rbgtopo_ctx* c, int32_t n_levels, const int
     CK(cudaStreamSynchronize(s));  // the caller's level_domain and the local doff may go once the call returns
     T.n_levels = n_levels;
     T.lvl_total_d = doff[n_lv];
+    c->lvl_epoch += 1;
+    T.lvl_nd.resize(n_lv);
+    for (int L = 0; L < n_lv; ++L) T.lvl_nd[L] = doff[L + 1] - doff[L];
     T.occ = true;
   } else {
     int frc = fence_batches(c, false);  // batches already enqueued read the old owners first
@@ -1946,6 +1977,7 @@ static int32_t place_groups_slow(rbgtopo_ctx* c, const int32_t* gb, int64_t word
       st[11] = n;
       st[12] = racc;
       st[13] = rowacc;
+      st[14] = r.rec[10];  // exclusive level
       racc += n;
       rowacc += P;
       memcpy(blob.data() + RBGTOPO_HDR_WORDS + (size_t)i * RBGTOPO_STEP_WORDS, st, sizeof st);
@@ -2169,6 +2201,7 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
     j.nrep = r.nrep;
     j.used0 = it->second.x;
     j.nused = it->second.y;
+    j.level = rec[10];
     jobs.push_back(j);
     jrow.push_back(r.rep0);
     own.insert(own.end(), assign + r.rep0, assign + r.rep0 + r.nrep);
@@ -2261,8 +2294,9 @@ int build_plan(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int64_t* plan_w
       pend += roles[4 * i + 1];
     }
     if (pend > 0x3FFFFFFFLL) GROUP_FAIL(RBGTOPO_ELIMIT, "group %d: pending replicas", g);
-    if (rec[0] < 0 || rec[2] < -1 || rec[2] >= n_domains) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: gid / fixed_domain", g);
-    if (const int lc = level_code(rec[10], installed_levels(c))) GROUP_FAIL(lc, "group %d: exclusive level %d", g, rec[10]);
+    if (rec[0] < 0 || rec[2] < -1 || (rec[10] == 0 && rec[2] >= n_domains)) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: gid / fixed_domain", g);
+    if (const int lc = level_code(rec[10], installed_levels(c), places_levels(c))) GROUP_FAIL(lc, "group %d: exclusive level %d", g, rec[10]);
+    if (rec[2] >= level_domains(c->topo, rec[10])) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: fixed_domain %d (level %d)", g, rec[2], rec[10]);
     if (rec[1] & ~(RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG)) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: unknown flags 0x%x", g, rec[1]);
     for (int i = 0; i < q; ++i)
       if (roles[4 * i + 3] & ~RBGTOPO_ROLE_EXCLUSIVE) GROUP_FAIL(RBGTOPO_EINVAL, "group %d role %d: unknown role flags", g, i);
@@ -2397,7 +2431,7 @@ int build_plan(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int64_t* plan_w
       int32_t* st = out + RBGTOPO_HDR_WORDS + (size_t)s * RBGTOPO_STEP_WORDS;
       int32_t* p = out + seco[s];
       st[0] = rec[0];
-      st[1] = rec[1] & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG);
+      st[1] = (rec[1] & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG)) | rec[10] << STEP_LEVEL_SHIFT;
       st[2] = (rec[1] & RBGTOPO_STEP_EXCLUSIVE) ? rec[2] : -1;
       st[3] = P;
       st[4] = (int32_t)(p - out);
@@ -2469,6 +2503,8 @@ int build_plan(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int64_t* plan_w
 struct TopoHost {
   int n = 0, n_domains = 0;
   int n_levels = -1;  // exclusive levels installed (occupancy mode, 0 outside it); -1: unknown (the describe calls)
+  bool place_levels = false;      // levels >= 1 are placed (level_code)
+  const int* level_nd = nullptr;  // [n_levels + 1] domain counts of the installed levels, or nullptr (describe calls)
   const int* degp1 = nullptr;  // [n] deg + 1, or nullptr = all 1
   int max_degp1 = 1;
   long long wsum_max = 0;
@@ -2598,8 +2634,11 @@ int plan_geometry(const TopoHost& T, int lc, Batch* b, const int32_t* gb, int64_
       v->nw = nw_g;
     }
     if (rec[0] < 0 || rec[2] < -1 || (rec[10] == 0 && rec[2] >= n_domains)) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: gid / fixed_domain", g);
-    if (const int lc = level_code(rec[10], T.n_levels))
-      GROUP_FAIL(lc, "group %d: exclusive level %d (%d installed; placement at level 0 only)", g, rec[10], std::max(0, T.n_levels));
+    if (const int lc = level_code(rec[10], T.n_levels, T.place_levels))
+      GROUP_FAIL(lc, "group %d: exclusive level %d (%d installed%s)", g, rec[10], std::max(0, T.n_levels),
+                 T.place_levels ? "" : "; placement at level 0 only");
+    if (rec[10] > 0 && T.level_nd && rec[2] >= T.level_nd[rec[10]])
+      GROUP_FAIL(RBGTOPO_EINVAL, "group %d: fixed_domain %d outside the %d domains of level %d", g, rec[2], T.level_nd[rec[10]], rec[10]);
     if (rec[1] & ~(RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG)) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: unknown flags 0x%x", g, rec[1]);
     long long pc = 0;  // closed neighbourhoods of the scheduled pods
     for (int a = 0; a < rec[6]; ++a) {
@@ -2636,6 +2675,7 @@ int plan_geometry(const TopoHost& T, int lc, Batch* b, const int32_t* gb, int64_
     if (pacc > 0x3FFFFFF0LL) return fail(RBGTOPO_ELIMIT, "pending replicas exceed 2^30");
     if ((rec[1] & RBGTOPO_STEP_EXCLUSIVE) && rec[2] < 0 && g_nw[g] > 0) m.any_excl_unknown = true;
     if (g_nw[g] > 0) m.max_q = std::max(m.max_q, rec[3]);
+    if (g_nw[g] > 0 && rec[10] != 0) m.any_level = true;
     W = std::max(W, g_nw[g]);
     wv_off[g + 1] = wv_off[g] + g_nw[g];
     if (wv_off[g + 1] > 0x03FFFFFF) return fail(RBGTOPO_ELIMIT, "plan has more than 2^26 steps");
@@ -2904,6 +2944,8 @@ int plan_stage(rbgtopo_ctx* c, Batch* b, const int32_t* gb, int64_t words, bool 
   th.n = T.n;
   th.n_domains = T.n_domains;
   th.n_levels = installed_levels(c);
+  th.place_levels = places_levels(c);
+  th.level_nd = c->topo.lvl_nd.empty() ? nullptr : c->topo.lvl_nd.data();
   th.degp1 = T.h_degp1.data();
   th.max_degp1 = T.max_degp1;
   th.wsum_max = T.wsum_max;
@@ -2924,6 +2966,7 @@ int plan_stage(rbgtopo_ctx* c, Batch* b, const int32_t* gb, int64_t words, bool 
       CK(cudaMemset(b->emit_ctr.p, 0, b->emit_ctr.cap * 4));
     }
     b->epoch = c->topo_epoch;
+    b->lvl_epoch = c->lvl_epoch;
     b->tev = timing_events(c);
     if (b->tev) CK(cudaEventRecord(b->ev[0], s));  // staging touches the batch's own buffers only: no wait for a pending snapshot refresh
     const bool pre = b->prestaged_h && b->prestaged_h == b->h_in.p && b->prestaged_hcap == b->h_in.cap &&
@@ -3066,7 +3109,7 @@ int verify_plan(rbgtopo_ctx* c, Batch* b, const int32_t* gb, int64_t words) {
       const int32_t* r = ref.h_in.p + h[4] + 4 * p2;
       const bool rexcl = (h[1] & RBGTOPO_STEP_EXCLUSIVE) && (r[3] & RBGTOPO_ROLE_EXCLUSIVE);
       for (int k = 0; k < r[0]; ++k, ++row) {
-        if (row < 0 || row >= m.total_r || seen[row] || rtab[row].x != emit_pack_row(r[1], r[2], rexcl) || rtab[row].y != h[0])
+        if (row < 0 || row >= m.total_r || seen[row] || rtab[row].x != emit_pack_row(r[1], r[2], rexcl, step_level(h[1])) || rtab[row].y != h[0])
           return fail(RBGTOPO_ECUDA, "verify_plan: row table entry %d (step %d role %d) differs from the plan", row, st, p2);
         seen[row] = 1;
       }
@@ -3231,8 +3274,11 @@ int group_facts(const TopoHost& T, const int32_t* gb, int64_t words, int g, bool
   }
   if (phase & 1) {
     if (rec[0] < 0 || rec[2] < -1 || (rec[10] == 0 && rec[2] >= T.n_domains)) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: gid / fixed_domain", g);
-    if (const int lc = level_code(rec[10], T.n_levels))
-      GROUP_FAIL(lc, "group %d: exclusive level %d (%d installed; placement at level 0 only)", g, rec[10], std::max(0, T.n_levels));
+    if (const int lc = level_code(rec[10], T.n_levels, T.place_levels))
+      GROUP_FAIL(lc, "group %d: exclusive level %d (%d installed%s)", g, rec[10], std::max(0, T.n_levels),
+                 T.place_levels ? "" : "; placement at level 0 only");
+    if (rec[10] > 0 && T.level_nd && rec[2] >= T.level_nd[rec[10]])
+      GROUP_FAIL(RBGTOPO_EINVAL, "group %d: fixed_domain %d outside the %d domains of level %d", g, rec[2], T.level_nd[rec[10]], rec[10]);
     if (rec[1] & ~(RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG)) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: unknown flags 0x%x", g, rec[1]);
     out->pend = (int)sf->pend;
     out->nw = sf->nw;
@@ -3387,6 +3433,8 @@ int place_groups_direct(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_
   th.n = T.n;
   th.n_domains = T.n_domains;
   th.n_levels = installed_levels(c);
+  th.place_levels = places_levels(c);
+  th.level_nd = c->topo.lvl_nd.empty() ? nullptr : c->topo.lvl_nd.data();
   th.degp1 = T.h_degp1.data();
   th.max_degp1 = T.max_degp1;
   th.wsum_max = T.wsum_max;
@@ -3411,6 +3459,7 @@ int place_groups_direct(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_
     CK(b->out.reserve(out_n + 4));
     CK(b->h_out.reserve(out_n + 4));
     b->epoch = c->topo_epoch;
+    b->lvl_epoch = c->lvl_epoch;
     if (n0 > 0) {
       CK(cudaMemcpyAsync(b->gsrc.p + perm_off, b->h_in.p + perm_off, (size_t)n0 * 4, cudaMemcpyHostToDevice, s));
       if (!rtab_early)  // (pass 1 found gb[4] == total_r, which is what the early launch was given)
@@ -3535,6 +3584,7 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
   th.n = T.n;
   th.n_domains = T.n_domains;
   th.n_levels = installed_levels(c);
+  th.place_levels = false;  // committed batches place level-0 groups only (DESIGN.md §3.9)
   th.degp1 = T.h_degp1.data();
   th.max_degp1 = T.max_degp1;
   th.wsum_max = T.wsum_max;
@@ -4128,7 +4178,7 @@ int32_t rbgtopo_shard_wave_score(rbgtopo_ctx* c, int32_t handle, int32_t wave, v
     wave_table(b, w, &CAP, &HT);
     const int nth = std::max(128, 32 * w.maxp);
     if (fast_smem_bytes(nth / 32, HT, CAP) <= kFastSmemMax) {
-      k_shard_select<<<n, nth, fast_smem_bytes(nth / 32, HT, CAP), s>>>(topo_dev(c), d, w.s0, 0, plan ? SEL_CORRECT : 0, HT, CAP, P2PDev{}, 0, 0, 0ull, nullptr);
+      (b->m.any_level ? k_shard_select<true> : k_shard_select<false>)<<<n, nth, fast_smem_bytes(nth / 32, HT, CAP), s>>>(topo_dev(c), d, w.s0, 0, plan ? SEL_CORRECT : 0, HT, CAP, P2PDev{}, 0, 0, 0ull, nullptr);
     } else {
       if (plan) return fail(RBGTOPO_ELIMIT, "plan step with more than %d patched nodes on the sharded path", CAP);
       k_select<<<n, 32 * w.maxp, select_smem_bytes(w.maxp), s>>>(topo_dev(c), d, 0);
@@ -4179,7 +4229,7 @@ int32_t rbgtopo_shard_wave_merge(rbgtopo_ctx* c, int32_t handle, int32_t wave, c
       wave_table(b, w, &CAP, &HT);
       const int nth = std::max(128, 32 * w.maxp);
       if (fast_smem_bytes(nth / 32, HT, CAP) <= kFastSmemMax)
-        k_shard_select<<<n, nth, fast_smem_bytes(nth / 32, HT, CAP), s>>>(topo_dev(c), d, w.s0, 1, 0, HT, CAP, P2PDev{}, 0, 0, 0ull, nullptr);
+        (b->m.any_level ? k_shard_select<true> : k_shard_select<false>)<<<n, nth, fast_smem_bytes(nth / 32, HT, CAP), s>>>(topo_dev(c), d, w.s0, 1, 0, HT, CAP, P2PDev{}, 0, 0, 0ull, nullptr);
       else
         k_select<<<n, 32 * w.maxp, select_smem_bytes(w.maxp), s>>>(topo_dev(c), d, 1);
       ++launches;
@@ -4373,7 +4423,7 @@ int32_t rbgtopo_run_staged_p2p(rbgtopo_ctx* c, int32_t handle, int32_t iters) {
       P2PWait pw{};
       phase(&seq, &parity, &pw);
       // select + fused push (peer stores of every list, release flags by the last CTA)
-      k_shard_select<<<n, nth, fast_smem_bytes(nth / 32, HT, CAP), s>>>(topo_dev(c), d, w.s0, 0, plan ? SEL_CORRECT : 0, HT, CAP,
+      (b->m.any_level ? k_shard_select<true> : k_shard_select<false>)<<<n, nth, fast_smem_bytes(nth / 32, HT, CAP), s>>>(topo_dev(c), d, w.s0, 0, plan ? SEL_CORRECT : 0, HT, CAP,
                                                                        c->p2p, w.rr0, parity, seq, c->p2p_ctr.p);
       d.parts = W;
       d.part_stride = c->p2p.slot_stride;
@@ -4389,7 +4439,7 @@ int32_t rbgtopo_run_staged_p2p(rbgtopo_ctx* c, int32_t handle, int32_t iters) {
       P2PWait pw2{};
       if (excl_unknown) {
         phase(&seq, &parity, &pw2);
-        k_shard_select<<<n, nth, fast_smem_bytes(nth / 32, HT, CAP), s>>>(topo_dev(c), d, w.s0, 1, 0, HT, CAP, c->p2p, w.rr0, parity, seq,
+        (b->m.any_level ? k_shard_select<true> : k_shard_select<false>)<<<n, nth, fast_smem_bytes(nth / 32, HT, CAP), s>>>(topo_dev(c), d, w.s0, 1, 0, HT, CAP, c->p2p, w.rr0, parity, seq,
                                                                          c->p2p_ctr.p);
         d.excl_all = c->xbuf.p + (long long)parity * W * c->p2p.slot_stride - (long long)w.rr0 * KS;
         d.excl_part_stride = c->p2p.slot_stride;

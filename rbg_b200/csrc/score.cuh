@@ -135,7 +135,7 @@ k_score_emit(TopoDev t, BatchDev b, int items, const int* __restrict__ etab) {
         const int g = tid + j * SCORE_THREADS;
         int4 avx = av[j];  // capacity as seen by exclusive roles: blocked domains are infeasible
         if (excl_step) {
-          const int4 ow = __ldg(reinterpret_cast<const int4*>(t.node_owner + n0 + (g << 2)));
+          const int4 ow = __ldg(reinterpret_cast<const int4*>(at_level(t, step_level(h0.y)).node_owner + n0 + (g << 2)));
           if (!(ow.x == -1 || ow.x == gid)) avx.x = -1;
           if (!(ow.y == -1 || ow.y == gid)) avx.y = -1;
           if (!(ow.z == -1 || ow.z == gid)) avx.z = -1;

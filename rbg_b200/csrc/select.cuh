@@ -376,6 +376,9 @@ __device__ __forceinline__ CandRef stage_candidates(const TopoDev& t, const Batc
   return r;
 }
 
+// LV: the batch has steps at exclusive levels >= 1 (DESIGN.md §3.9).  Level-0 batches launch <false>, whose code is the
+// level-0 code: the level's vectors cost registers the <false> instantiation does not pay.
+template <bool LV>
 __global__ void __launch_bounds__(32 * MAXP) k_select_assign(TopoDev t, BatchDev b, int step_begin, int mode) {
   extern __shared__ __align__(16) unsigned char sel_smem[];
   int* sCand = reinterpret_cast<int*>(sel_smem);
@@ -388,6 +391,7 @@ __global__ void __launch_bounds__(32 * MAXP) k_select_assign(TopoDev t, BatchDev
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int step = step_begin + blockIdx.x;
   const StepHdr h = load_hdr(b, step);
+  if constexpr (LV) t = at_level(t, step_level(h.flags));  // domain / owner of the step's exclusive level
   const bool excl_step = (h.flags & RBGTOPO_STEP_EXCLUSIVE) != 0;
   if (h.flags & STEP_SKIP) {  // an earlier wave of this gang group failed: nothing is placed
     if (warp == 0) {
@@ -451,6 +455,7 @@ __global__ void __launch_bounds__(32 * MAXP) k_select(TopoDev t, BatchDev b, int
   const int warp = threadIdx.x >> 5;
   const int step = blockIdx.x;
   const StepHdr h = load_hdr(b, step);
+  t = at_level(t, step_level(h.flags));  // domain / owner of the step's exclusive level
   const bool excl_step = (h.flags & RBGTOPO_STEP_EXCLUSIVE) != 0;
   const bool unknown = excl_step && h.fixed_domain < 0;
   if (pass2 && !unknown) return;  // CTA-uniform
@@ -506,6 +511,7 @@ __global__ void __launch_bounds__(SEL_THREADS) k_merge(TopoDev t, BatchDev b, in
   if (idx >= count) return;
   const int step = step_begin + idx;
   const StepHdr h = load_hdr(b, step);
+  t = at_level(t, step_level(h.flags));  // domain / owner of the step's exclusive level
   const bool excl_step = (h.flags & RBGTOPO_STEP_EXCLUSIVE) != 0;
   int dstar = excl_step ? h.fixed_domain : -1;
   bool dstar_set = !excl_step || h.fixed_domain >= 0;

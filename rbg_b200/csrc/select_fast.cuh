@@ -268,6 +268,8 @@ __device__ __forceinline__ void build_table(const TopoDev& t, const BatchDev& b,
 
 }
 
+// LV: as k_select_assign (select.cuh).
+template <bool LV>
 __global__ void __launch_bounds__(32 * MAXP)
 k_select_assign_fast(TopoDev t, BatchDev b, int step_begin, int mode, int HT, int CAP) {
   extern __shared__ __align__(16) unsigned char fs_smem[];
@@ -293,6 +295,7 @@ k_select_assign_fast(TopoDev t, BatchDev b, int step_begin, int mode, int HT, in
 
   const int step = step_begin + blockIdx.x;
   const StepHdr h = load_hdr(b, step);
+  if constexpr (LV) t = at_level(t, step_level(h.flags));  // domain / owner of the step's exclusive level
   const bool excl_step = (h.flags & RBGTOPO_STEP_EXCLUSIVE) != 0;
   if (h.flags & STEP_SKIP) {  // an earlier wave of this gang group failed: nothing is placed
     if (warp == 0) {
@@ -392,6 +395,7 @@ k_select_assign_fast(TopoDev t, BatchDev b, int step_begin, int mode, int HT, in
 // px.world > 1: the CTA also stores its rows straight into every rank's exchange buffer (p2p.cuh:
 // slot [parity][this rank], row index relative to px_row0) and the last CTA of the grid publishes the
 // release flags — the all-gather is fused into the kernel that produces the lists.
+template <bool LV>  // as k_select_assign (select.cuh)
 __global__ void __launch_bounds__(32 * MAXP)
 k_shard_select(TopoDev t, BatchDev b, int step_begin, int pass2, int mode, int HT, int CAP, P2PDev px, int px_row0,
                int px_parity, unsigned long long px_seq, int* __restrict__ px_done) {
@@ -415,6 +419,7 @@ k_shard_select(TopoDev t, BatchDev b, int step_begin, int pass2, int mode, int H
   T.sel_order = t.order;
   const int step = step_begin + blockIdx.x;
   const StepHdr h = load_hdr(b, step);
+  if constexpr (LV) t = at_level(t, step_level(h.flags));  // domain / owner of the step's exclusive level
   const bool excl_step = (h.flags & RBGTOPO_STEP_EXCLUSIVE) != 0;
   const bool unknown = excl_step && h.fixed_domain < 0;
   // what this warp's row is worth to the peers: the selected list, or zeros (skipped step, role not reselected)

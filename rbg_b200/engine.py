@@ -48,10 +48,14 @@ class TopoPlacer:
     """Device-resident cluster snapshot + placement entry points."""
 
     def __init__(self, device: int = 0, rank: int = 0, world: int = 1, emit_matrix: bool = True,
-                 chunk_nodes: int = 0):
+                 chunk_nodes: int = 0, level_placement: bool = False):
+        """level_placement: place exclusive groups at levels >= 1 of set_exclusive_levels (RBGTOPO_CFG_LEVEL_PLACEMENT,
+        DESIGN.md §3.9); without it such a group raises RBGTOPO_ELIMIT.  `places_levels` tells callers which it is."""
         self.lib = _lib.load()
         cfg = _lib.Config(device=device, rank=rank, world=world, slots=0,
-                          emit_matrix=1 if emit_matrix else 0, chunk_nodes=chunk_nodes)
+                          emit_matrix=1 if emit_matrix else 0, chunk_nodes=chunk_nodes,
+                          flags=_lib.CFG_LEVEL_PLACEMENT if level_placement else 0)
+        self.places_levels = bool(level_placement)
         h = C.c_void_p()
         self._h = None
         self._check(self.lib.rbgtopo_create(C.byref(cfg), C.byref(h)))

@@ -190,8 +190,9 @@ class _Wave:
 class _GroupRun:
     """Per-group state while its levels/waves are placed."""
 
-    def __init__(self, rbg: RoleBasedGroup, arith: HostArith, plan_waves: bool = True):
+    def __init__(self, rbg: RoleBasedGroup, arith: HostArith, plan_waves: bool = True, excl_level: int = 0):
         self.rbg = rbg
+        self.excl_level = excl_level  # index of the group's exclusive key (DESIGN.md §3.9)
         roles = rbg.roles
         self.Q = len(roles)
         index = {r.name: i for i, r in enumerate(roles)}
@@ -268,7 +269,7 @@ class _GroupRun:
         return Step(gid=self.rbg.gid, roles=roles_rec, pair=pair_rows,
                     anchors=[(n, q, c) for (n, q), c in sorted(self.anchors.items())],
                     consumed=sorted(self.consumed.items()), flags=flags,
-                    fixed_domain=self.fixed_domain if self.exclusive else -1)
+                    fixed_domain=self.fixed_domain if self.exclusive else -1, level=self.excl_level)
 
     def absorb(self, w: int, assign: np.ndarray, status: int, domain: int, n_nodes: int) -> None:
         wave = self.waves[w]
@@ -298,9 +299,12 @@ class B200TopoPodGroupManager:
         """inner: the gang plugin this manager wraps for the PodGroup CR and the pod-group label —
         "scheduler-plugins" (kube), "volcano" or None (the Go manager takes the implementation object).
         exclusive_keys: the topology keys exclusive groups may name (DESIGN.md §3.9), keys[0] = the level-0 label.
-        None: every key is treated as the level-0 label.  With a list, an exclusive group whose key is not keys[0]
-        gets no hint and a logged reason (no_hint[(ns, name)]): the library places level 0 only, and a hint into a
-        domain of the wrong key is worse than none.
+        None: every key is treated as the level-0 label.  With a list, an exclusive group whose key is keys[i] is
+        placed at level i (GROUPS word +10, step word +14) when the placer has `places_levels` (a TopoPlacer created
+        with level_placement=True, whose snapshot holds the partitions of set_exclusive_levels), and its
+        exclusive_domain is a domain of that level.  Otherwise such a group — and any group at level >= 1 of a
+        committed batch, which the library places at level 0 only — gets no hint and a logged reason
+        (no_hint[(ns, name)]): a hint into a domain of the wrong key is worse than none.
         alternates: next-best nodes per replica carried beside the hint (DESIGN.md §3.10, at most 8).  0 keeps the
         single-node hint; with n > 0 the snapshot call is rbgtopo_place_groups_ranked, which places identically and
         also ranks, per replica, the nodes that still have room once its group is placed."""
@@ -314,7 +318,7 @@ class B200TopoPodGroupManager:
         self.no_hint: Dict[Tuple[str, str], str] = {}
         self._hints: Dict[Tuple[str, str], Placement] = {}
 
-    def exclusive_level(self, rbg: RoleBasedGroup) -> Tuple[int, str]:
+    def exclusive_level(self, rbg: RoleBasedGroup, committed: bool = False) -> Tuple[int, str]:
         """(level of the group's exclusive key, reason for no hint or "")."""
         key = rbg.annotations.get(EXCLUSIVE_TOPOLOGY_KEY)
         if key is None or self.exclusive_keys is None:
@@ -322,13 +326,19 @@ class B200TopoPodGroupManager:
         if key not in self.exclusive_keys:
             return -1, f"exclusive key {key!r} is not configured"
         lv = self.exclusive_keys.index(key)
-        return lv, "" if lv == 0 else f"exclusive key {key!r} is not the level-0 label: no placement at that level yet"
+        if lv == 0:
+            return 0, ""
+        if not getattr(self.placer, "places_levels", False):
+            return lv, f"exclusive key {key!r} is not the level-0 label: no placement at that level yet"
+        if committed:
+            return lv, f"exclusive key {key!r} is not the level-0 label: committed batches place level 0 only"
+        return lv, ""
 
-    def _split_no_hint(self, rbgs: Sequence[RoleBasedGroup]):
+    def _split_no_hint(self, rbgs: Sequence[RoleBasedGroup], committed: bool = False):
         """The groups that get a hint, and a no-hint Placement per group that does not (logged, hint dropped)."""
         keep, skipped = [], {}
         for i, r in enumerate(rbgs):
-            _, reason = self.exclusive_level(r)
+            _, reason = self.exclusive_level(r, committed)
             if not reason:
                 keep.append(r)
                 continue
@@ -353,7 +363,7 @@ class B200TopoPodGroupManager:
     def groups_blob(self, rbgs: Sequence[RoleBasedGroup]):
         """Marshal RoleBasedGroups into the GROUPS wire format (the Go shim does
         the same from the typed objects).  Returns (blob, runs)."""
-        runs = [_GroupRun(r, self.arith, plan_waves=False) for r in rbgs]
+        runs = [_GroupRun(r, self.arith, plan_waves=False, excl_level=self.exclusive_level(r)[0]) for r in rbgs]
         gb = GroupsBuilder()
         for g in runs:
             roles = [(g.level_of[ri], g.pending[ri], g.rbg.roles[ri].demand,
@@ -363,7 +373,7 @@ class B200TopoPodGroupManager:
             anchors = [(n, pos[q], c) for (n, q), c in sorted(g.anchors.items())]
             flags = (STEP_EXCLUSIVE if g.exclusive else 0) | (STEP_GANG if g.gang else 0)
             gb.add(Group(gid=g.rbg.gid, roles=roles, pair=pair, anchors=anchors, flags=flags,
-                         fixed_domain=g.fixed_domain if g.exclusive else -1))
+                         fixed_domain=g.fixed_domain if g.exclusive else -1, level=g.excl_level))
         return gb.build(), runs
 
     def reconcile_pod_groups(self, rbgs: Sequence[RoleBasedGroup], committed: bool = False) -> List[Placement]:
@@ -372,7 +382,7 @@ class B200TopoPodGroupManager:
         domains the groups before it took, so the hints of one call never contradict each other (the controller
         passes the groups ordered by namespaced name)."""
         all_rbgs = rbgs
-        rbgs, skipped = self._split_no_hint(rbgs)
+        rbgs, skipped = self._split_no_hint(rbgs, committed)
         if not rbgs:
             return self._merge(all_rbgs, [], skipped)
         blob, runs = self.groups_blob(rbgs)
@@ -406,7 +416,7 @@ class B200TopoPodGroupManager:
     def reconcile_pod_groups_by_waves(self, rbgs: Sequence[RoleBasedGroup]) -> List[Placement]:
         all_rbgs = rbgs
         rbgs, skipped = self._split_no_hint(rbgs)
-        runs = [_GroupRun(r, self.arith) for r in rbgs]
+        runs = [_GroupRun(r, self.arith, excl_level=self.exclusive_level(r)[0]) for r in rbgs]
         n_nodes = self.placer.n_nodes
         w = 0
         while True:
