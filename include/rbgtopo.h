@@ -139,6 +139,9 @@ typedef struct rbgtopo_config {
 #define RBGTOPO_CFG_LEVEL_PLACEMENT 1  /* place groups / steps at exclusive levels >= 1
                                           (rbgtopo_set_exclusive_levels); without it a
                                           level >= 1 answers RBGTOPO_ELIMIT */
+#define RBGTOPO_CFG_COMMIT_LEVELS 2    /* rbgtopo_place_groups_committed also places groups
+                                          at levels >= 1 (claims across levels); valid only
+                                          with RBGTOPO_CFG_LEVEL_PLACEMENT, alone EINVAL */
 
 /* Per-call device timing, milliseconds from CUDA events on the call's stream. */
 typedef struct rbgtopo_timing {
@@ -222,8 +225,9 @@ int32_t rbgtopo_update_nodes_delta(rbgtopo_ctx* ctx, int32_t n_changed, const in
  * the participating roles select inside dom_L = D*, fixed_domain and the reported domain are level-L domain
  * ids (fixed_domain >= level_n_domains[L - 1]: RBGTOPO_EINVAL).  Opted-out roles and non-exclusive groups
  * are unaffected.  Level-0 groups give the same results with and without the flag.  Every entry point
- * places at levels >= 1 except rbgtopo_place_groups_committed, which keeps returning RBGTOPO_ELIMIT (a
- * claim of an earlier group crosses levels: a follow-up).  The describe calls accept any level >= 0.  Installing
+ * places at levels >= 1; rbgtopo_place_groups_committed does so only on a ctx created with
+ * RBGTOPO_CFG_COMMIT_LEVELS as well (flags = 3), where the claims of earlier groups cross levels (see there),
+ * and returns RBGTOPO_ELIMIT without it.  The describe calls accept any level >= 0.  Installing
  * partitions makes every staged handle with a step at a level >= 1 stale (run / fetch return RBGTOPO_EINVAL; release
  * still works): its level ids and fixed domains belong to the partitions it was validated against. */
 #define RBGTOPO_MAX_EXCL_LEVELS 8
@@ -304,10 +308,18 @@ int32_t rbgtopo_place_groups(rbgtopo_ctx* ctx, const int32_t* groups,
  * n_groups, one when no group reads a node or domain an earlier group took), *rounds (may be NULL) =
  * selection rounds run.  Valid for any world: every rank returns the identical result.  Gids need not
  * be distinct.  A group whose table of patched nodes does not fit k_plan_group's shared memory makes
- * the call return RBGTOPO_ELIMIT (there is no per-wave fallback for committed batches).  So does a group
- * at an exclusive level >= 1, even on a ctx with RBGTOPO_CFG_LEVEL_PLACEMENT: a group at key L_h blocks a
- * later group at key L_g through dom_{L_g} of each of its pods and through dom_{L_h} of its domain, which
- * the claim lists of this build (one per level-0 domain) do not express. */
+ * the call return RBGTOPO_ELIMIT (there is no per-wave fallback for committed batches).
+ * Levels (rbgtopo_set_exclusive_levels): a group at an exclusive level >= 1 is placed only by a ctx created
+ * with RBGTOPO_CFG_LEVEL_PLACEMENT | RBGTOPO_CFG_COMMIT_LEVELS; with RBGTOPO_CFG_LEVEL_PLACEMENT alone it
+ * returns RBGTOPO_ELIMIT, so hosts built against the level-0 contract keep withholding those hints.  Levels,
+ * fixed domains and error codes are checked as by rbgtopo_place_groups.  A participating role of exclusive
+ * group g at level L_g may not use node n when owner_{L_g}[n] (+) K (+) P is not -1 or gid_g, where
+ *   K = (+) over the levels L of the batch's exclusive groups of the gid of the LAST earlier exclusive group
+ *       at level L (status != RBGTOPO_GANG_FAILED) that reports dom_L(n) (an earlier group's anti-affinity on
+ *       its own key, which kube-scheduler enforces symmetrically), and
+ *   P = (+) of gid_h over every replica this call placed for a participating role of an earlier exclusive
+ *       group h at a level L_h != L_g on a node m with dom_{L_g}(m) = dom_{L_g}(n) (g's own anti-affinity).
+ * For a batch whose groups are all at level 0 this is the rule above: same results, same rounds. */
 int32_t rbgtopo_place_groups_committed(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
                                        int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds);
 

@@ -138,6 +138,16 @@ struct CommitDev {
   int g;               // the group this CTA places (set by the kernel)
   bool excl;           // ... and whether it is exclusive
   bool occ;            // occupancy mode (§3.9): owners are per node, derived from the pods' records
+  // Batches with a group at a level >= 1 (the <true> variants, §3.9): dhead / dreader are indexed by
+  // doff[L] + (domain of level L), and the placed participating pods of exclusive groups are linked per (level, domain)
+  // into phead / pclaim for every level of `lmask` other than their group's.  Unused by the <false> variants.
+  const int* ldom;     // level L's domain of node n at L * lstride + n (row 0 = level 0)
+  const int* doff;     // [levels + 1] first head of level L in dhead / dreader / phead
+  int* phead;          // first pod claim in (L, d), -1 = none
+  int4* pclaim;        // [rows][popc(lmask)] {group index, gid, next pod claim in the same (L, d), 0}
+  int lstride;
+  int lmask;           // levels of the batch's exclusive groups
+  int level;           // cm.g's exclusive level (set by the kernel)
 };
 // capacity the groups before cm.g took on `node`
 __device__ __forceinline__ int commit_ext(const CommitDev& cm, int node) {
@@ -153,33 +163,75 @@ __device__ __forceinline__ int commit_ext(const CommitDev& cm, int node) {
 // group that reported the domain, else `owner`.  In occupancy mode `owner` is the node's own derived owner_0, which the
 // records may block inside a domain another node of which is free: the claim is merged into it, so that a claim never
 // unblocks what the records block.
-__device__ __forceinline__ int commit_owner(const CommitDev& cm, int dom, int owner) {
-  int last = -1, claim = -1;
-  for (int i = cm.dhead[dom]; i >= 0;) {
-    const int2 c = cm.dclaim[i];
-    if (i < cm.g && i > last) { last = i; claim = c.x; }
-    i = c.y;
+//
+// LV (a batch with a group at a level >= 1, occupancy mode): `owner` is owner_{L_g}[node] and `dom` = dom_{L_g}(node),
+// L_g = cm.level.  The owner is owner ⊕ K ⊕ P (§3.9): K merges, for every level L of the batch's exclusive groups, the
+// gid of the last earlier group that reported dom_L(node) at level L; P merges the gid of every pod an earlier exclusive
+// group of another level placed in dom_{L_g}(node) (pods of cm.g's own level lie in their group's reported domain, which
+// K covers).
+__device__ __forceinline__ int commit_dom(const CommitDev& cm, int L, int node, int dom) {
+  return L == cm.level ? dom : cm.ldom[(size_t)L * cm.lstride + node];
+}
+template <bool LV = false>
+__device__ __forceinline__ int commit_owner(const CommitDev& cm, int node, int dom, int owner) {
+  if constexpr (!LV) {
+    int last = -1, claim = -1;
+    for (int i = cm.dhead[dom]; i >= 0;) {
+      const int2 c = cm.dclaim[i];
+      if (i < cm.g && i > last) { last = i; claim = c.x; }
+      i = c.y;
+    }
+    return last < 0 ? owner : cm.occ ? owner_merge(owner, claim) : claim;
+  } else {
+    for (int m = cm.lmask; m; m &= m - 1) {
+      const int L = __ffs(m) - 1;
+      const int d = cm.doff[L] + commit_dom(cm, L, node, dom);
+      int last = -1, claim = -1;
+      for (int i = cm.dhead[d]; i >= 0;) {
+        const int2 c = cm.dclaim[i];
+        if (i < cm.g && i > last) { last = i; claim = c.x; }
+        i = c.y;
+      }
+      if (last >= 0) owner = owner_merge(owner, claim);
+      if (L == cm.level)
+        for (int i = cm.phead[d]; i >= 0;) {
+          const int4 c = cm.pclaim[i];
+          if (c.x < cm.g) owner = owner_merge(owner, c.y);
+          i = c.z;
+        }
+    }
+    return owner;
   }
-  return last < 0 ? owner : cm.occ ? owner_merge(owner, claim) : claim;
 }
 // The marks only grow within a round, so a plain L2 load that already shows cm.g or more makes the atomic redundant; the
 // CTAs of a round all read the head of the background order, and this keeps them from queueing on the same addresses.
+// LV: an exclusive group marks the node's domain at every level of the batch's exclusive groups (what commit_owner reads).
+template <bool LV = false>
 __device__ __forceinline__ void commit_note_read(const CommitDev& cm, int node, int dom) {
   if (__ldcg(&cm.reader[node]) < cm.g) atomicMax(&cm.reader[node], cm.g);
-  if (cm.excl && __ldcg(&cm.dreader[dom]) < cm.g) atomicMax(&cm.dreader[dom], cm.g);
+  if constexpr (!LV) {
+    if (cm.excl && __ldcg(&cm.dreader[dom]) < cm.g) atomicMax(&cm.dreader[dom], cm.g);
+  } else if (cm.excl) {
+    for (int m = cm.lmask; m; m &= m - 1) {
+      const int L = __ffs(m) - 1;
+      int* const p = &cm.dreader[cm.doff[L] + commit_dom(cm, L, node, dom)];
+      if (__ldcg(p) < cm.g) atomicMax(p, cm.g);
+    }
+  }
 }
 // a background candidate as group cm.g sees it (the selection notes the read where the candidate's capacity or owner
 // can decide anything: not where its domain alone rules it out)
+template <bool LV = false>
 __device__ __forceinline__ void commit_adjust(BgCand& c, const CommitDev& cm) {
   if (c.node < 0) return;
   c.free_ -= commit_ext(cm, c.node);
-  if (cm.excl) c.owner = commit_owner(cm, c.dom, c.owner);
+  if (cm.excl) c.owner = commit_owner<LV>(cm, c.node, c.dom, c.owner);
 }
 
 // top-K of a role row into out[0..KS) (+ capacities): select_role_fast with the
 // delta evaluated from the per-group-role planes.  `first` = bg_load(..., lane, ...) when
 // have_first.  One warp.  COMMIT: the background candidates it loads are seen through `cm` (`first` already is).
-template <bool COMMIT = false>
+template <bool COMMIT = false, bool CLV = false>
 __device__ __forceinline__ void select_role_group(const TopoDev& t, int gid, bool excl_step, const GroupRole& role,
                                                   const float* pair_row, int Q, int K, int dom, const GroupTab& T,
                                                   int cnt, bool have_first, const BgCand& first, int dbg,
@@ -204,7 +256,7 @@ __device__ __forceinline__ void select_role_group(const TopoDev& t, int gid, boo
   auto entry_key = [&](int i) -> unsigned long long {
     const int av = gtab_avail(T, i), dd = T.dDom[i];
     if constexpr (COMMIT)
-      if (dom == DOM_ANY || (dd & 0x7FFFFFFF) == dom) commit_note_read(*cm, T.node[T.dSlot[i]], dd & 0x7FFFFFFF);
+      if (dom == DOM_ANY || (dd & 0x7FFFFFFF) == dom) commit_note_read<CLV>(*cm, T.node[T.dSlot[i]], dd & 0x7FFFFFFF);
     if (av >= demand && !(rexcl && dd < 0) && (dom == DOM_ANY || (dd & 0x7FFFFFFF) == dom)) {
       const int slot = T.dSlot[i];
       return make_key(fmaf(need, T.dBase[i], gtab_delta(T, pair_row, Q, slot)), T.node[slot]);
@@ -250,8 +302,8 @@ __device__ __forceinline__ void select_role_group(const TopoDev& t, int gid, boo
   for (int pos = 0; pos < t.n && acc < K; pos += 32) {
     BgCand c = (pos == 0 && have_first) ? first : bg_load(t, role.need, pos + lane, t.n);
     if constexpr (COMMIT) {
-      if (!(pos == 0 && have_first)) commit_adjust(c, *cm);
-      if (c.node >= 0 && (dom == DOM_ANY || c.dom == dom)) commit_note_read(*cm, c.node, c.dom);
+      if (!(pos == 0 && have_first)) commit_adjust<CLV>(c, *cm);
+      if (c.node >= 0 && (dom == DOM_ANY || c.dom == dom)) commit_note_read<CLV>(*cm, c.node, c.dom);
     }
     bool ok = c.node >= 0 && c.free_ >= demand;
     if (ok && rexcl) ok = (c.owner == -1 || c.owner == gid);
@@ -391,7 +443,7 @@ __global__ void __launch_bounds__(32 * RTAB_WARPS) k_group_rtab(const int* __res
 // attributes — free capacity minus what they took, the owner of a domain they reported — and records what it read.
 // No dense matrix exists: the kernel never touches one.  `need` counts the replicas actually placed by earlier
 // waves (not the planned ones), so every group is exact without the host-driven loop.
-template <bool DIRECT, bool COMMIT>
+template <bool DIRECT, bool COMMIT, bool CLV = false>
 __device__ __forceinline__ void plan_group_body(TopoDev t, BatchDev b, int QB, int HT, int CAP, int record, CommitDev cm) {
   extern __shared__ __align__(16) unsigned char pg_smem[];
   __shared__ int sTakenNode[KS], sTakenAmt[KS], sTakenRole[KS];
@@ -460,8 +512,9 @@ __device__ __forceinline__ void plan_group_body(TopoDev t, BatchDev b, int QB, i
   } else {
     h = load_hdr(b, step);  // in flight while the table is cleared
   }
-  // every wave of the group is placed at its exclusive level (a committed batch has level-0 groups only)
-  t = at_level(t, DIRECT ? b.blob[RBGTOPO_HDR_WORDS + (size_t)step * RBGTOPO_GROUP_WORDS + 10] : step_level(h.flags));
+  // every wave of the group is placed at its exclusive level (in a committed batch: level 0 unless CLV)
+  const int level = DIRECT ? b.blob[RBGTOPO_HDR_WORDS + (size_t)step * RBGTOPO_GROUP_WORDS + 10] : step_level(h.flags);
+  t = at_level(t, level);
   for (int i = tid; i < HT; i += nthreads) {
     T.node[i] = -1;
     T.cons[i] = 0;
@@ -479,6 +532,7 @@ __device__ __forceinline__ void plan_group_body(TopoDev t, BatchDev b, int QB, i
   if constexpr (COMMIT) {
     cm.g = step;
     cm.excl = excl_step;
+    if constexpr (CLV) cm.level = level;
   }
   int fixed = excl_step ? h.fixed_domain : -1;
   g_dom = fixed;  // DIRECT: an exclusive group confirms the domain it already occupies
@@ -547,7 +601,7 @@ __device__ __forceinline__ void plan_group_body(TopoDev t, BatchDev b, int QB, i
     const bool have_first = warp < h.P;
     if (have_first) first = bg_attrs(t, sRole[warp].need, lane, t.n, ob0);
     if constexpr (COMMIT)
-      if (have_first) commit_adjust(first, cm);
+      if (have_first) commit_adjust<CLV>(first, cm);
     // closed neighbourhoods of the placements: one flat pass over all their CSR entries
     {
       int total = 0;
@@ -577,7 +631,7 @@ __device__ __forceinline__ void plan_group_body(TopoDev t, BatchDev b, int QB, i
       int dd = t.domain[node];
       if (excl_step) {
         int o = t.node_owner[node];
-        if constexpr (COMMIT) o = commit_owner(cm, dd, o);
+        if constexpr (COMMIT) o = commit_owner<CLV>(cm, node, dd, o);
         if (!(o == -1 || o == gid)) dd |= 0x80000000;
       }
       T.dBase[d] = t.base[node];
@@ -599,7 +653,7 @@ __device__ __forceinline__ void plan_group_body(TopoDev t, BatchDev b, int QB, i
       if (warp == 0) {
         int d = -1;
         if (pstar >= 0) {
-          select_role_group<COMMIT>(t, gid, excl_step, sRole[pstar], sPair + pstar * QB, Q, 1, DOM_ANY, T,
+          select_role_group<COMMIT, CLV>(t, gid, excl_step, sRole[pstar], sPair + pstar * QB, Q, 1, DOM_ANY, T,
                                     cnt, pstar == 0, first, 29, sAcc, sAccAv, sPat, sPatAv, sList, sListAv, &cm);
           const unsigned long long top = sList[0];
           d = top ? t.domain[key_node(top)] : -1;
@@ -616,7 +670,7 @@ __device__ __forceinline__ void plan_group_body(TopoDev t, BatchDev b, int QB, i
       int K = 0;
       for (int q = 0; q <= p; ++q) K += sRole[q].count;
       K = min(K, t.n);
-      select_role_group<COMMIT>(t, gid, excl_step, sRole[p], sPair + p * QB, Q, K, dom, T, cnt, true, first,
+      select_role_group<COMMIT, CLV>(t, gid, excl_step, sRole[p], sPair + p * QB, Q, K, dom, T, cnt, true, first,
                                 warp == 0 ? wave_i * 8 + 6 : -1, sAcc + p * KS, sAccAv + p * KS, sPat + p * KS,
                                 sPatAv + p * KS, sList + p * KS, sListAv + p * KS, &cm);
       if (!DIRECT) b.merged[(size_t)(h.rolerow_off + p) * KS + lane] = sList[p * KS + lane];
@@ -801,32 +855,53 @@ __global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group(TopoDev t, BatchDev
 }
 
 // One round of a committed batch (DESIGN.md §3.8): b.perm[0 .. gridDim.x) = the groups of the round (ascending).
+// LV: a batch with a group at an exclusive level >= 1 (claims across levels, §3.9); <false> is the level-0 code.
+template <bool LV>
 __global__ void __launch_bounds__(32 * MAXP, 4) k_plan_group_commit(TopoDev t, BatchDev b, int QB, int HT, int CAP, CommitDev cm) {
-  plan_group_body<true, true>(t, b, QB, HT, CAP, 0, cm);
+  plan_group_body<true, true, LV>(t, b, QB, HT, CAP, 0, cm);
 }
 
 // Claims of a committed batch, one warp per group, from the results of the last round (assign / domain_out of the
 // plan kernel, the blob for groups with nothing pending): every placed replica links its dense row into the list of
 // its node, every exclusive group that reports a domain links itself into the list of the domain.  head / dhead are
 // -1 on entry.  A failed gang has no placements and reports no domain.
+// LV: the domain is linked at (group level L_h, D), i.e. into dhead[doff[L_h] + D], and every placed replica of a
+// participating role of an exclusive group also links into the pod list of (L, dom_L(node)) for every level L of
+// cm.lmask other than L_h (slot k = L's rank in lmask; cm.phead is -1 on entry).
+template <bool LV>
 __global__ void __launch_bounds__(32 * RTAB_WARPS) k_commit_claims(const int* __restrict__ grp, int n_groups,
                                                                  const int* __restrict__ assign, const int* __restrict__ domain,
-                                                                 int* head, int4* claim, int* dhead, int2* dclaim) {
+                                                                 int* head, int4* claim, int* dhead, int2* dclaim, CommitDev cm) {
   const int lane = threadIdx.x & 31;
   const int g = blockIdx.x * RTAB_WARPS + (threadIdx.x >> 5);
   if (g >= n_groups) return;
   const int* rec = grp + RBGTOPO_HDR_WORDS + (size_t)g * RBGTOPO_GROUP_WORDS;
   const int q = rec[3], roff = rec[4], row0 = rec[8], pend = rec[9];
-  if (lane == 0 && (rec[1] & RBGTOPO_STEP_EXCLUSIVE)) {
+  const bool excl = (rec[1] & RBGTOPO_STEP_EXCLUSIVE) != 0;
+  if (lane == 0 && excl) {
     const int d = pend > 0 ? domain[g] : rec[2];  // nothing pending: the group confirms the domain it occupies
-    if (d >= 0) dclaim[g] = make_int2(rec[0], atomicExch(&dhead[d], g));
+    if (d >= 0) dclaim[g] = make_int2(rec[0], atomicExch(&dhead[(LV ? cm.doff[rec[10]] : 0) + d], g));
   }
+  const int nl = LV ? __popc(cm.lmask) : 0;
   int pre = 0;  // a group's rows are its roles' pending replicas in role order
   for (int r = 0; r < q; ++r) {
     const int pr = grp[roff + 4 * r + 1], dem = grp[roff + 4 * r + 2];
+    const bool pod = LV && excl && (grp[roff + 4 * r + 3] & RBGTOPO_ROLE_EXCLUSIVE);
     for (int i = lane; i < pr; i += 32) {
       const int row = row0 + pre + i, node = assign[row];
-      if (node >= 0) claim[row] = make_int4(g, dem, atomicExch(&head[node], row), 0);
+      if (node < 0) continue;
+      claim[row] = make_int4(g, dem, atomicExch(&head[node], row), 0);
+      if constexpr (LV)
+        if (pod) {
+          int k = 0;
+          for (int m = cm.lmask; m; m &= m - 1, ++k) {
+            const int L = __ffs(m) - 1;
+            if (L == rec[10]) continue;
+            const int e = row * nl + k;
+            int* const ph = cm.phead + cm.doff[L] + cm.ldom[(size_t)L * cm.lstride + node];
+            cm.pclaim[e] = make_int4(g, rec[0], atomicExch(ph, e), 0);
+          }
+        }
     }
     pre += pr;
   }
@@ -838,11 +913,15 @@ __global__ void __launch_bounds__(32 * RTAB_WARPS) k_commit_claims(const int* __
 // (reader[n] > g), a changed domain only when a later exclusive group read a node of it.  *cmin = the lowest group with
 // a claim that matters: groups up to it saw exactly the claims they will see from now on, the next round re-runs the
 // groups above it.
+// LV: a changed domain is (L_h, D); a changed placement of a participating role of an exclusive group also matters when
+// a later exclusive group read a node of (L, dom_L) of its old or new node at a level L != L_h of cm.lmask (the pod
+// claims of k_commit_claims).  Marks may over-report (a re-run round); they never under-report.
+template <bool LV>
 __global__ void __launch_bounds__(32 * RTAB_WARPS) k_commit_diff(const int* __restrict__ grp, const int* __restrict__ groups,
                                                                int n_run, const int* __restrict__ assign,
                                                                const int* __restrict__ domain, int* prev_assign,
                                                                int* prev_domain, const int* __restrict__ reader,
-                                                               const int* __restrict__ dreader, int* cmin) {
+                                                               const int* __restrict__ dreader, int* cmin, CommitDev cm) {
   const int lane = threadIdx.x & 31;
   const int k = blockIdx.x * RTAB_WARPS + (threadIdx.x >> 5);
   if (k >= n_run) return;
@@ -850,17 +929,45 @@ __global__ void __launch_bounds__(32 * RTAB_WARPS) k_commit_diff(const int* __re
   const int* rec = grp + RBGTOPO_HDR_WORDS + (size_t)g * RBGTOPO_GROUP_WORDS;
   const int row0 = rec[8], pend = rec[9];
   bool hit = false;
-  for (int i = lane; i < pend; i += 32) {
-    const int a = assign[row0 + i], o = prev_assign[row0 + i];
-    if (a != o) {
-      hit |= (a >= 0 && reader[a] > g) || (o >= 0 && reader[o] > g);
-      prev_assign[row0 + i] = a;
+  if constexpr (!LV) {
+    for (int i = lane; i < pend; i += 32) {
+      const int a = assign[row0 + i], o = prev_assign[row0 + i];
+      if (a != o) {
+        hit |= (a >= 0 && reader[a] > g) || (o >= 0 && reader[o] > g);
+        prev_assign[row0 + i] = a;
+      }
+    }
+  } else {
+    const int q = rec[3], roff = rec[4], lh = rec[10];
+    const bool excl = (rec[1] & RBGTOPO_STEP_EXCLUSIVE) != 0;
+    auto dread = [&](int node) {  // a later exclusive group read (L, dom_L(node)), L != L_h
+      bool r = false;
+      for (int m = cm.lmask; m; m &= m - 1) {
+        const int L = __ffs(m) - 1;
+        if (L != lh) r |= dreader[cm.doff[L] + cm.ldom[(size_t)L * cm.lstride + node]] > g;
+      }
+      return r;
+    };
+    int pre = 0;
+    for (int r = 0; r < q; ++r) {
+      const int pr = grp[roff + 4 * r + 1];
+      const bool pod = excl && (grp[roff + 4 * r + 3] & RBGTOPO_ROLE_EXCLUSIVE);
+      for (int i = lane; i < pr; i += 32) {
+        const int row = row0 + pre + i, a = assign[row], o = prev_assign[row];
+        if (a != o) {
+          hit |= (a >= 0 && reader[a] > g) || (o >= 0 && reader[o] > g);
+          if (pod) hit |= (a >= 0 && dread(a)) || (o >= 0 && dread(o));
+          prev_assign[row] = a;
+        }
+      }
+      pre += pr;
     }
   }
   if (lane == 0) {
     const int d = domain[g], od = prev_domain[g];
     if (d != od) {
-      hit |= (d >= 0 && dreader[d] > g) || (od >= 0 && dreader[od] > g);
+      const int* const dr = LV ? dreader + cm.doff[rec[10]] : dreader;
+      hit |= (d >= 0 && dr[d] > g) || (od >= 0 && dr[od] > g);
       prev_domain[g] = d;
     }
   }

@@ -216,10 +216,12 @@ struct Batch {
   std::vector<int> grp_flags, grp_assign_off, grp_pending, grp_fixed;
   DevBuf<int> out;  // assign[total_r] | status[n] | domain[n] | dstar[n]
   PinBuf<int> h_in, h_out;
-  // committed batches (place_groups_committed): head[nodes] | dhead[domains] | reader[nodes] | dreader[domains] |
-  // previous round's assign[total_r] and domain[n] | lowest group whose changed claims matter; the claim lists
+  // committed batches (place_groups_committed): head[nodes] | dhead[domains] | phead[domains] | reader[nodes] |
+  // dreader[domains] | previous round's assign[total_r] and domain[n] | lowest group whose changed claims matter; the
+  // claim lists.  Domains are level 0's, or (a group at a level >= 1) those of every installed level; phead and the
+  // pod claims exist only then.
   DevBuf<int> cm_int;
-  DevBuf<int4> cm_claim;
+  DevBuf<int4> cm_claim, cm_pclaim;
   DevBuf<int2> cm_dclaim;
   // ranked placement (place_groups_ranked): jobs | placements | own nodes, then the per-replica lists
   DevBuf<int> alt;
@@ -300,6 +302,8 @@ inline int level_code(int level, int n_levels, bool place) {
 }
 inline int installed_levels(const rbgtopo_ctx* c) { return c->topo.occ ? c->topo.n_levels : 0; }
 inline bool places_levels(const rbgtopo_ctx* c) { return (c->cfg.flags & RBGTOPO_CFG_LEVEL_PLACEMENT) != 0; }
+// committed batches at levels >= 1 (create accepts the flag only together with RBGTOPO_CFG_LEVEL_PLACEMENT)
+inline bool commits_levels(const rbgtopo_ctx* c) { return (c->cfg.flags & RBGTOPO_CFG_COMMIT_LEVELS) != 0; }
 // Domain count of installed level L (level_code accepted it): the range of a fixed domain at that level.
 inline int level_domains(const Topology& T, int L) { return L == 0 ? T.n_domains : T.lvl_nd[L]; }
 constexpr size_t kFastSmemMax = 200 * 1024;
@@ -1402,7 +1406,10 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
   *out = nullptr;
   if (cfg->world < 1 || cfg->rank < 0 || cfg->rank >= cfg->world)
     return fail(RBGTOPO_EINVAL, "rank %d / world %d", cfg->rank, cfg->world);
-  if (cfg->flags & ~RBGTOPO_CFG_LEVEL_PLACEMENT) return fail(RBGTOPO_EINVAL, "unknown config flags 0x%x", cfg->flags);
+  if (cfg->flags & ~(RBGTOPO_CFG_LEVEL_PLACEMENT | RBGTOPO_CFG_COMMIT_LEVELS))
+    return fail(RBGTOPO_EINVAL, "unknown config flags 0x%x", cfg->flags);
+  if ((cfg->flags & RBGTOPO_CFG_COMMIT_LEVELS) && !(cfg->flags & RBGTOPO_CFG_LEVEL_PLACEMENT))
+    return fail(RBGTOPO_EINVAL, "RBGTOPO_CFG_COMMIT_LEVELS needs RBGTOPO_CFG_LEVEL_PLACEMENT (flags 0x%x)", cfg->flags);
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess || ndev <= 0)
@@ -1435,9 +1442,11 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
   CK(cudaFuncSetAttribute(k_plan_group<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_plan_group<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_plan_group<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-  CK(cudaFuncSetAttribute(k_plan_group_commit, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
+  for (auto* f : {k_plan_group_commit<false>, k_plan_group_commit<true>}) {
+    CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
+    CK(cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  }
   CK(cudaFuncSetAttribute(k_alternates, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
-  CK(cudaFuncSetAttribute(k_plan_group_commit, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   CK(cudaFuncSetAttribute(emit_tma_fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)emit_tma_smem_bytes(kEmitStages)));
   // k_emit_tma and k_plan_group are meant to share an SM: both ask for the largest shared-memory carve-out,
   // otherwise the persistent emit CTA pins the SM at the small carve-out it needs alone and the CTAs of
@@ -3584,7 +3593,8 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
   th.n = T.n;
   th.n_domains = T.n_domains;
   th.n_levels = installed_levels(c);
-  th.place_levels = false;  // committed batches place level-0 groups only (DESIGN.md §3.9)
+  th.place_levels = commits_levels(c);  // levels >= 1 only on a ctx that opted into committed levels (DESIGN.md §3.9)
+  th.level_nd = c->topo.lvl_nd.empty() ? nullptr : c->topo.lvl_nd.data();
   th.degp1 = T.h_degp1.data();
   th.max_degp1 = T.max_degp1;
   th.wsum_max = T.wsum_max;
@@ -3606,6 +3616,15 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
     if (facts[g].nw > 0) run.push_back(g);
   const int n0 = (int)run.size();
   const long long total_r = G.total_r;
+  // A group at a level >= 1 (validated: the ctx commits levels, and they are installed) selects the <true> kernels:
+  // claims per (level, domain) over the levels of the batch's exclusive groups (lmask).
+  bool lv = false;
+  int lmask = 0;
+  for (int g = 0; g < ng; ++g) {
+    const int32_t* rec = gb + RBGTOPO_HDR_WORDS + (int64_t)g * RBGTOPO_GROUP_WORDS;
+    lv |= rec[10] > 0;
+    if (rec[1] & RBGTOPO_STEP_EXCLUSIVE) lmask |= 1 << rec[10];
+  }
   const size_t out_n = (size_t)total_r + 2 * (size_t)ng;
   Batch* b = nullptr;
   rc = acquire_batch(c, &b);
@@ -3622,12 +3641,14 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
     CK(b->gsrc.reserve(src_words));
     CK(b->out.reserve(out_n + 4));
     CK(b->h_out.reserve(out_n + 4));
-    const int N = T.n, ND = T.n_domains;
-    const size_t o_dhead = (size_t)N, o_reader = o_dhead + ND, o_dreader = o_reader + N, o_prev = o_dreader + ND,
-                 o_cmin = o_prev + out_n, n_int = o_cmin + 1;
+    // ND = domain heads: level 0's, or (lv) those of every installed level at lvl_doff[L], and as many pod heads
+    const int N = T.n, ND = lv ? T.lvl_total_d : T.n_domains, NP = lv ? ND : 0, NL = lv ? __builtin_popcount(lmask) : 0;
+    const size_t o_dhead = (size_t)N, o_phead = o_dhead + ND, o_reader = o_phead + NP, o_dreader = o_reader + N,
+                 o_prev = o_dreader + ND, o_cmin = o_prev + out_n, n_int = o_cmin + 1;
     CK(b->cm_int.reserve(n_int));
     CK(b->cm_claim.reserve((size_t)std::max<long long>(total_r, 1)));
     CK(b->cm_dclaim.reserve((size_t)std::max(ng, 1)));
+    if (lv) CK(b->cm_pclaim.reserve((size_t)std::max<long long>(total_r * NL, 1)));
     memcpy(b->h_in.p, gb, (size_t)words * 4);
     memcpy(b->h_in.p + run_off, run.data(), (size_t)n0 * 4);
     CK(cudaMemcpyAsync(b->gsrc.p, b->h_in.p, src_words * 4, cudaMemcpyHostToDevice, s));
@@ -3637,10 +3658,29 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
     // nothing placed and no domain reported yet: the claims before round 0 are those of groups with nothing pending
     CK(cudaMemsetAsync(b->out.p, 0xFF, out_n * 4, s));
     CK(cudaMemsetAsync(ci + o_prev, 0xFF, out_n * 4, s));
-    CK(cudaMemsetAsync(ci, 0xFF, (size_t)(N + ND) * 4, s));
+    CK(cudaMemsetAsync(ci, 0xFF, (size_t)(N + ND + NP) * 4, s));
+    CommitDev cm{};
+    cm.head = ci;
+    cm.claim = b->cm_claim.p;
+    cm.dhead = ci + o_dhead;
+    cm.dclaim = b->cm_dclaim.p;
+    cm.reader = ci + o_reader;
+    cm.dreader = ci + o_dreader;
+    cm.occ = T.occ;
+    if (lv) {
+      cm.ldom = T.lvl_domain.p;
+      cm.doff = T.lvl_doff.p;
+      cm.phead = ci + o_phead;
+      cm.pclaim = b->cm_pclaim.p;
+      cm.lstride = level_stride(N);
+      cm.lmask = lmask;
+    }
+    const auto claims = lv ? k_commit_claims<true> : k_commit_claims<false>;
+    const auto diff = lv ? k_commit_diff<true> : k_commit_diff<false>;
+    const auto plan = lv ? k_plan_group_commit<true> : k_plan_group_commit<false>;
     const int claim_grid = (ng + RTAB_WARPS - 1) / RTAB_WARPS;
-    k_commit_claims<<<claim_grid, 32 * RTAB_WARPS, 0, s>>>(b->gsrc.p, ng, o_assign, o_domain, ci, b->cm_claim.p, ci + o_dhead,
-                                                           b->cm_dclaim.p);
+    claims<<<claim_grid, 32 * RTAB_WARPS, 0, s>>>(b->gsrc.p, ng, o_assign, o_domain, ci, b->cm_claim.p, ci + o_dhead,
+                                                  b->cm_dclaim.p, cm);
     CK(cudaStreamWaitEvent(s, c->topo_ready, 0));  // a pending snapshot refresh: free, owners, base and the order
     BatchDev d{};
     d.blob = b->gsrc.p;
@@ -3652,14 +3692,6 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
     d.status = b->out.p + total_r;
     d.domain_out = o_domain;
     d.dstar = o_domain;
-    CommitDev cm{};
-    cm.head = ci;
-    cm.claim = b->cm_claim.p;
-    cm.dhead = ci + o_dhead;
-    cm.dclaim = b->cm_dclaim.p;
-    cm.reader = ci + o_reader;
-    cm.dreader = ci + o_dreader;
-    cm.occ = T.occ;
     int first = 0;  // run[first ..) = the groups of the next round
     while (first < n0) {
       if (rounds >= ng) return fail(RBGTOPO_ECUDA, "internal: committed batch did not converge in %d rounds", ng);
@@ -3668,15 +3700,15 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
       CK(cudaMemsetAsync(ci + o_reader, 0xFF, (size_t)(N + ND) * 4, s));  // reader and dreader: -1
       CK(cudaMemsetAsync(ci + o_cmin, 0x7F, 4, s));                        // > any group index
       if (timed) CK(cudaEventRecord(b->ev[0], s));
-      k_plan_group_commit<<<n_run, G.nth, G.smem, s>>>(topo_dev(c), d, G.max_q, G.HT, G.CAP, cm);
+      plan<<<n_run, G.nth, G.smem, s>>>(topo_dev(c), d, G.max_q, G.HT, G.CAP, cm);
       CK(cudaGetLastError());
       if (timed) CK(cudaEventRecord(b->ev[1], s));
-      k_commit_diff<<<(n_run + RTAB_WARPS - 1) / RTAB_WARPS, 32 * RTAB_WARPS, 0, s>>>(
+      diff<<<(n_run + RTAB_WARPS - 1) / RTAB_WARPS, 32 * RTAB_WARPS, 0, s>>>(
           b->gsrc.p, d.perm, n_run, o_assign, o_domain, ci + o_prev, ci + o_prev + total_r + ng, ci + o_reader,
-          ci + o_dreader, ci + o_cmin);
-      CK(cudaMemsetAsync(ci, 0xFF, (size_t)(N + ND) * 4, s));  // head and dhead
-      k_commit_claims<<<claim_grid, 32 * RTAB_WARPS, 0, s>>>(b->gsrc.p, ng, o_assign, o_domain, ci, b->cm_claim.p,
-                                                             ci + o_dhead, b->cm_dclaim.p);
+          ci + o_dreader, ci + o_cmin, cm);
+      CK(cudaMemsetAsync(ci, 0xFF, (size_t)(N + ND + NP) * 4, s));  // head, dhead and phead
+      claims<<<claim_grid, 32 * RTAB_WARPS, 0, s>>>(b->gsrc.p, ng, o_assign, o_domain, ci, b->cm_claim.p, ci + o_dhead,
+                                                    b->cm_dclaim.p, cm);
       CK(cudaMemcpyAsync(b->h_out.p + out_n, ci + o_cmin, 4, cudaMemcpyDeviceToHost, s));
       CK(cudaStreamSynchronize(s));
       CK(cudaGetLastError());

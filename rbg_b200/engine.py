@@ -48,14 +48,18 @@ class TopoPlacer:
     """Device-resident cluster snapshot + placement entry points."""
 
     def __init__(self, device: int = 0, rank: int = 0, world: int = 1, emit_matrix: bool = True,
-                 chunk_nodes: int = 0, level_placement: bool = False):
+                 chunk_nodes: int = 0, level_placement: bool = False, committed_levels: bool = False):
         """level_placement: place exclusive groups at levels >= 1 of set_exclusive_levels (RBGTOPO_CFG_LEVEL_PLACEMENT,
-        DESIGN.md §3.9); without it such a group raises RBGTOPO_ELIMIT.  `places_levels` tells callers which it is."""
+        DESIGN.md §3.9); without it such a group raises RBGTOPO_ELIMIT.  `places_levels` tells callers which it is.
+        committed_levels: place_groups_committed places them too, with claims across levels (RBGTOPO_CFG_COMMIT_LEVELS,
+        §3.8; implies level_placement).  `places_committed_levels` tells callers which it is."""
         self.lib = _lib.load()
+        level_placement = level_placement or committed_levels
+        flags = (_lib.CFG_LEVEL_PLACEMENT if level_placement else 0) | (_lib.CFG_COMMIT_LEVELS if committed_levels else 0)
         cfg = _lib.Config(device=device, rank=rank, world=world, slots=0,
-                          emit_matrix=1 if emit_matrix else 0, chunk_nodes=chunk_nodes,
-                          flags=_lib.CFG_LEVEL_PLACEMENT if level_placement else 0)
+                          emit_matrix=1 if emit_matrix else 0, chunk_nodes=chunk_nodes, flags=flags)
         self.places_levels = bool(level_placement)
+        self.places_committed_levels = bool(committed_levels)
         h = C.c_void_p()
         self._h = None
         self._check(self.lib.rbgtopo_create(C.byref(cfg), C.byref(h)))

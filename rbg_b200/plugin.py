@@ -302,8 +302,8 @@ class B200TopoPodGroupManager:
         None: every key is treated as the level-0 label.  With a list, an exclusive group whose key is keys[i] is
         placed at level i (GROUPS word +10, step word +14) when the placer has `places_levels` (a TopoPlacer created
         with level_placement=True, whose snapshot holds the partitions of set_exclusive_levels), and its
-        exclusive_domain is a domain of that level.  Otherwise such a group — and any group at level >= 1 of a
-        committed batch, which the library places at level 0 only — gets no hint and a logged reason
+        exclusive_domain is a domain of that level.  In a committed batch this also needs `places_committed_levels`
+        (a TopoPlacer created with committed_levels=True).  Otherwise such a group gets no hint and a logged reason
         (no_hint[(ns, name)]): a hint into a domain of the wrong key is worse than none.
         alternates: next-best nodes per replica carried beside the hint (DESIGN.md §3.10, at most 8).  0 keeps the
         single-node hint; with n > 0 the snapshot call is rbgtopo_place_groups_ranked, which places identically and
@@ -330,7 +330,7 @@ class B200TopoPodGroupManager:
             return 0, ""
         if not getattr(self.placer, "places_levels", False):
             return lv, f"exclusive key {key!r} is not the level-0 label: no placement at that level yet"
-        if committed:
+        if committed and not getattr(self.placer, "places_committed_levels", False):
             return lv, f"exclusive key {key!r} is not the level-0 label: committed batches place level 0 only"
         return lv, ""
 
