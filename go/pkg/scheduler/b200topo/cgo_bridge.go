@@ -82,11 +82,19 @@ static int32_t rbgtopo_go_place_groups_ranked(rbgtopo_ctx* ctx, const int32_t* g
   rbgtopo_go_err(ctx, rc, err);
   return rc;
 }
+static int32_t rbgtopo_go_place_groups_lw(rbgtopo_ctx* ctx, const int32_t* groups, int64_t words, const int32_t* role_pods,
+                                          int64_t role_pods_words, int32_t* assign, int32_t* status, int32_t* domain,
+                                          char* err) {
+  int32_t rc = rbgtopo_place_groups_lw(ctx, groups, words, role_pods, role_pods_words, assign, status, domain);
+  rbgtopo_go_err(ctx, rc, err);
+  return rc;
+}
 */
 import "C"
 
 import (
 	"fmt"
+	"sync/atomic"
 	"unsafe"
 )
 
@@ -130,7 +138,8 @@ func mkErr(rc C.int32_t, buf *[C.RBGTOPO_GO_ERRLEN]C.char) error {
 // concurrent use by --max-concurrent-reconciles goroutines (cmd/rbgs/main.go:140-143): the library
 // takes an internal slot per call (include/rbgtopo.h, "Rules of the ABI").
 type placer struct {
-	ctx *C.rbgtopo_ctx
+	ctx     *C.rbgtopo_ctx
+	nLevels atomic.Int32 // exclusive levels above 0 the snapshot holds (setExclusiveLevels; setTopology clears them)
 }
 
 func newPlacer(device int) (*placer, error) {
@@ -156,6 +165,9 @@ func (p *placer) setTopology(s *snapshot) error {
 	var buf [C.RBGTOPO_GO_ERRLEN]C.char
 	rc := C.rbgtopo_go_set_topology(p.ctx, C.int32_t(len(s.names)), C.int64_t(len(s.colIdx)), p32(s.rowPtr), p32(s.colIdx),
 		p32(s.edgeW), p32(s.free), p32(s.domain), C.int32_t(len(s.owner)), p32(s.owner), C.uint64_t(s.topoGen), &buf[0])
+	if rc == C.RBGTOPO_OK {
+		p.nLevels.Store(0)
+	}
 	return mkErr(rc, &buf)
 }
 
@@ -180,6 +192,9 @@ func (p *placer) setExclusiveLevels(nLevels int, levelDomain, levelNDomains, occ
 	var buf [C.RBGTOPO_GO_ERRLEN]C.char
 	rc := C.rbgtopo_go_set_exclusive_levels(p.ctx, C.int32_t(nLevels), p32(levelDomain), p32(levelNDomains),
 		C.int32_t(len(occ)/3), p32(occ), C.uint64_t(gen), &buf[0])
+	if rc == C.RBGTOPO_OK && levelDomain != nil {
+		p.nLevels.Store(int32(nLevels))
+	}
 	return mkErr(rc, &buf)
 }
 
@@ -232,4 +247,21 @@ func (p *placer) placeGroupsRanked(blob []int32, nAlt int) (assign, status, doma
 		return nil, nil, nil, nil, err
 	}
 	return assign[:nPending], status[:nGroups], domain[:nGroups], altNode[:nPending*nAlt], nil
+}
+
+// placeGroupsLW: placeGroups where a replica of a role can be several pods (DESIGN.md §3.11): rolePods holds (S, C) per
+// role of every group in blob order, nPods = sum of pending * S; assign has one node per pod in (group, role, ordinal,
+// pod index) order.
+func (p *placer) placeGroupsLW(blob, rolePods []int32, nPods int) (assign, status, domain []int32, err error) {
+	nGroups := int(blob[2])
+	assign = make([]int32, max(nPods, 1))
+	status = make([]int32, max(nGroups, 1))
+	domain = make([]int32, max(nGroups, 1))
+	var buf [C.RBGTOPO_GO_ERRLEN]C.char
+	rc := C.rbgtopo_go_place_groups_lw(p.ctx, p32(blob), C.int64_t(len(blob)), p32(rolePods), C.int64_t(len(rolePods)),
+		p32(assign), p32(status), p32(domain), &buf[0])
+	if err = mkErr(rc, &buf); err != nil {
+		return nil, nil, nil, err
+	}
+	return assign[:nPods], status[:nGroups], domain[:nGroups], nil
 }

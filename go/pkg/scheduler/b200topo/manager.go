@@ -21,6 +21,7 @@ package b200topo
 import (
 	"context"
 	"encoding/json"
+	"fmt"
 	"sync"
 
 	corev1 "k8s.io/api/core/v1"
@@ -39,6 +40,10 @@ const PlacementHintKey = "rbg.workloads.x-k8s.io/b200-topo-placement"
 // PlacementAlternatesKey carries RoleID -> ranked next-best node names (DESIGN.md §3.10) beside the hint, written only
 // when the manager is configured with alternates (SetAlternates) and only for replicas that have some.
 const PlacementAlternatesKey = "rbg.workloads.x-k8s.io/b200-topo-alternates"
+
+// ColocateKey, a role annotation, names the topology key one domain of which must hold every pod of a multi-pod
+// replica of the role (DESIGN.md §3.11); it resolves against the exclusive keys (SetExclusiveKeys).
+const ColocateKey = "rbg.workloads.x-k8s.io/b200-topo-colocate"
 
 // inner is the part of scheduler.PodGroupManager this package wraps (declared here to avoid an
 // import cycle with pkg/scheduler, which imports this package in its factory).
@@ -63,6 +68,43 @@ type Manager struct {
 	// RBGTOPO_MAX_ALTERNATES); alts holds them per group like hints
 	alternates int
 	alts       sync.Map // "ns/name" -> map[RoleID][]string (node names)
+	// leaderWorker: groups with a multi-pod role are placed through rbgtopo_place_groups_lw, hints keyed by pod name
+	leaderWorker bool
+}
+
+// SetLeaderWorker opts into leader-worker placement (DESIGN.md §3.11): a group with a role of LeaderWorkerPattern.Size
+// > 1 is placed pod by pod, every replica's pods all or nothing and, with the ColocateKey annotation, inside one domain
+// of that key; its hints are keyed by pod name.  Off (the default): such groups are placed one pod per replica.
+func (m *Manager) SetLeaderWorker(on bool) { m.leaderWorker = on }
+
+// colocateLevels: the co-location level per role (rbg.Spec.Roles order, -1 none), or a reason for giving no hint.
+func (m *Manager) colocateLevels(rbg *workloadsv1alpha2.RoleBasedGroup) ([]int32, string) {
+	out := make([]int32, len(rbg.Spec.Roles))
+	for i := range rbg.Spec.Roles {
+		out[i] = -1
+		key, ok := rbg.Spec.Roles[i].Annotations[ColocateKey]
+		if !ok {
+			continue
+		}
+		if m.exclusiveKeys == nil {
+			out[i] = 0
+			continue
+		}
+		found := false
+		for L, k := range m.exclusiveKeys {
+			if k == key {
+				out[i], found = int32(L), true
+			}
+		}
+		if !found {
+			return nil, "co-location key " + key + " of role " + rbg.Spec.Roles[i].Name + " is not configured"
+		}
+		if out[i] > m.placer.nLevels.Load() {
+			return nil, fmt.Sprintf("co-location key %s of role %s: the snapshot holds no level %d", key,
+				rbg.Spec.Roles[i].Name, out[i])
+		}
+	}
+	return out, ""
 }
 
 // SetAlternates configures how many ranked next-best nodes every hinted replica carries (DESIGN.md §3.10): 0 (the
@@ -136,6 +178,25 @@ func (m *Manager) ReconcilePodGroup(ctx context.Context, rbg *workloadsv1alpha2.
 		return err // cycle in the role dependencies etc.: the controller reports the same condition
 	}
 	if g.pending == 0 {
+		return nil
+	}
+	if m.leaderWorker && g.leaderWorker() {
+		colocate, reason := m.colocateLevels(rbg)
+		if reason == "" && m.alternates > 0 {
+			reason = "leader-worker replicas: no ranked alternates for them"
+		}
+		if reason != "" {
+			m.hints.Delete(key)
+			m.alts.Delete(key)
+			logger.Info("no placement hint", "rbg", key, "reason", reason)
+			return nil
+		}
+		table, pods := g.rolePods(colocate)
+		assign, status, _, err := m.placer.placeGroupsLW(g.blob, table, pods)
+		if err != nil {
+			return m.degrade(logger, key, err)
+		}
+		m.hints.Store(key, g.podIDMap(assign, snap, status[0]))
 		return nil
 	}
 	if m.alternates > 0 {

@@ -38,6 +38,9 @@ type marshalled struct {
 	count   []int32  // pending replicas per role
 	names   []string // role names, rbg.Spec.Roles order
 	rbgName string
+	// leader-worker placement (DESIGN.md §3.11): pods per replica (LeaderWorkerPattern.Size, 1 for standalone roles)
+	// per role, rbg.Spec.Roles order
+	size []int32
 }
 
 // dependencyLevels restates dependencyOrder (pkg/dependency/dependency.go:129-205, unexported):
@@ -118,7 +121,8 @@ func marshalGroup(rbg *workloadsv1alpha2.RoleBasedGroup, pods []corev1.Pod, snap
 	for k, ri := range order {
 		pos[ri] = k
 	}
-	m := &marshalled{order: order, first: make([]int32, q), count: make([]int32, q), names: make([]string, q), rbgName: rbg.Name}
+	m := &marshalled{order: order, first: make([]int32, q), count: make([]int32, q), names: make([]string, q), rbgName: rbg.Name,
+		size: make([]int32, q)}
 	// pair matrix (DESIGN.md §3.2): same role, dependency edge, both in one CoordinatedPolicy rule
 	pair := make([]int32, q*q)
 	for i := range roles {
@@ -149,6 +153,10 @@ func marshalGroup(rbg *workloadsv1alpha2.RoleBasedGroup, pods []corev1.Pod, snap
 	for _, ri := range order {
 		role := &roles[ri]
 		m.names[ri] = role.Name
+		m.size[ri] = 1
+		if lwp := role.GetLeaderWorkerPattern(); lwp != nil && lwp.Size != nil && *lwp.Size > 1 {
+			m.size[ri] = *lwp.Size
+		}
 		cur := int32(0)
 		if st, ok := rbg.GetRoleStatus(role.Name); ok {
 			cur = st.Replicas
@@ -215,6 +223,52 @@ func (m *marshalled) roleIDMap(assign []int32, snap *snapshot, status int32) map
 				out[fmt.Sprintf("%s-%s-%d", m.rbgName, m.names[ri], m.first[ri]+c)] = snap.names[node]
 			}
 			k++
+		}
+	}
+	return out
+}
+
+// leaderWorker: a role of the group runs multi-pod replicas.
+func (m *marshalled) leaderWorker() bool {
+	for _, s := range m.size {
+		if s > 1 {
+			return true
+		}
+	}
+	return false
+}
+
+// rolePods: the (S, C) table of rbgtopo_place_groups_lw in blob role order and the pods it places; colocate[ri] = the
+// co-location level of role ri (-1 none).
+func (m *marshalled) rolePods(colocate []int32) (table []int32, pods int) {
+	for _, ri := range m.order {
+		table = append(table, m.size[ri], colocate[ri])
+		pods += int(m.count[ri]) * int(m.size[ri])
+	}
+	return table, pods
+}
+
+// podIDMap: roleIDMap for the leader-worker call, whose assign[] has one node per pod.  A multi-pod replica's pods are
+// "{rbg}-{role}-{ordinal}-{k}", k = 0 the leader (pkg/reconciler/roleinstance/utils/instance_utils.go:76-89);
+// standalone roles keep the RoleID.
+func (m *marshalled) podIDMap(assign []int32, snap *snapshot, status int32) map[string]string {
+	out := map[string]string{}
+	if status == 2 {
+		return out
+	}
+	k := 0
+	for _, ri := range m.order {
+		for c := int32(0); c < m.count[ri]; c++ {
+			for pod := int32(0); pod < m.size[ri]; pod++ {
+				if node := assign[k]; node >= 0 {
+					id := fmt.Sprintf("%s-%s-%d", m.rbgName, m.names[ri], m.first[ri]+c)
+					if m.size[ri] > 1 {
+						id = fmt.Sprintf("%s-%d", id, pod)
+					}
+					out[id] = snap.names[node]
+				}
+				k++
+			}
 		}
 	}
 	return out

@@ -342,6 +342,36 @@ int32_t rbgtopo_place_groups_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int
                                     int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain,
                                     float* score, int32_t* alt_node, float* alt_score);
 
+/* Leader-worker replicas (DESIGN.md §3.11).  The GROUPS blob of rbgtopo_place_groups — same validation and
+ * error codes — where a replica of a role can be several pods (a leaderWorkerPattern of size S: one leader and
+ * S - 1 workers), optionally all inside one domain of a co-location level.
+ *   role_pods[2 * sum of q over the groups] (role_pods_words): per role of every group, in blob order, (S, C):
+ *     S in [1, RBGTOPO_MAX_STEP_REPLICAS] pods per replica; C = -1 (no co-location), 0 (domain[]) or a level
+ *     1..n_levels of rbgtopo_set_exclusive_levels.  Anything else: RBGTOPO_EINVAL.  C needs no config flag; a
+ *     group's own exclusive level keeps the RBGTOPO_CFG_LEVEL_PLACEMENT rule.
+ *   assign[sum over groups and roles of pending * S]: one node per POD, ordered by (group, role in blob order,
+ *     ordinal, pod index k; k = 0 is the leader), -1 = unplaced; status[n_groups]; domain[n_groups] as by
+ *     rbgtopo_place_groups.
+ * Rules: a wave holds at most RBGTOPO_MAX_STEP_REPLICAS pods and RBGTOPO_MAX_STEP_ROLES role rows and never
+ * splits a replica; need_rho counts unplaced pods, demand is per pod, every placed pod is an anchor
+ * (node, role, 1) and consumes (node, demand) for the later waves.  Per replica, in order, a candidate node has
+ * a finite score and room for one pod (free - consumed - taken in this wave >= demand), and for a participating
+ * role of an exclusive group lies in D* (§3.5).  C = -1: the S pods take, one after the other, the candidate with
+ * the largest key (score desc, node asc) that still has room.  C >= 0: the pods go to the level-C domain with
+ * the best candidate among the domains whose candidates hold all S pods (sum of floor(room / demand) >= S; any
+ * candidate when demand = 0), and take its best candidates one after the other.  A replica whose S pods do not
+ * all fit is placed all or nothing (all its pods -1).  status counts whole replicas; gang fails the group when
+ * any replica is unplaced.  With S = 1 and C = -1 everywhere the results are bit-identical to
+ * rbgtopo_place_groups.
+ * Exactness (§3.4) is checked before any wave runs, against the worst wave the call can stage: for a non-gang
+ * group that includes waves after unplaced pods (each raises need and drops an anchor), so such a group can be
+ * refused with RBGTOPO_EINEXACT a little below the bound rbgtopo_place_groups applies; no wave fails midway.
+ * Documented limits: a ctx with world > 1 holds only its slab of every dense row, so the call returns
+ * RBGTOPO_ELIMIT there; more nodes than a shared-memory room bitmap of 200 KB holds (1 638 400): RBGTOPO_ELIMIT. */
+int32_t rbgtopo_place_groups_lw(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                const int32_t* role_pods, int64_t role_pods_words, int32_t* assign,
+                                int32_t* status, int32_t* domain);
+
 /* rbgtopo_place_groups pipeline, staged: the groups are compiled into a
  * device-resident multi-wave plan (one step blob, wave-major, expanded on the
  * device), so rbgtopo_run_staged runs ONE score launch for the dense rows of every

@@ -33,6 +33,7 @@
 #include "plan_group.cuh"
 #include "p2p.cuh"
 #include "alternates.cuh"
+#include "lw_assign.cuh"
 
 using namespace rbgtopo;
 
@@ -230,6 +231,10 @@ struct Batch {
   // ranked placement (place_groups_ranked): jobs | placements | own nodes, then the per-replica lists
   DevBuf<int> alt;
   PinBuf<int> h_alt;
+  // leader-worker placement (place_groups_lw): the wave's (S, C) side table, the per-CTA level-C domain scratch
+  DevBuf<int> lw, lw_cap;
+  PinBuf<int> h_lw;
+  DevBuf<unsigned long long> lw_best;
   ~Batch() {
     if (stream) cudaStreamDestroy(stream);
     if (stream2) cudaStreamDestroy(stream2);
@@ -1401,6 +1406,7 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
     CK(cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   }
   CK(cudaFuncSetAttribute(k_alternates, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
+  CK(cudaFuncSetAttribute(k_lw_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_plan_group<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
 #ifdef RBGTOPO_PHASE_CLOCKS
   {
@@ -3172,8 +3178,9 @@ struct ShapeFacts {
 // size_group (same messages), the exactness bound is taken per role over its worst wave.
 // phase 1: the group record, role table and pair matrix (what the row table and the dense matrix depend on);
 // phase 2: the scheduled pods (ranges, neighbourhood sizes) and the exactness bound; phase 3 = both.
+// role_bound: the per-role wave bound of another wave rule (place_groups_lw: pods, §3.11) instead of the replica waves'.
 int group_facts(const TopoHost& T, const int32_t* gb, int64_t words, int g, bool report, long long amax_limit, long long row_w,
-                GroupFacts* out, int phase = 3) {
+                GroupFacts* out, int phase = 3, const long long* role_bound = nullptr) {
   auto in = [&](long long off, long long cnt) { return off >= 0 && cnt >= 0 && off + cnt <= words; };
   const int32_t* rec = gb + RBGTOPO_HDR_WORDS + (int64_t)g * RBGTOPO_GROUP_WORDS;
   const int q = rec[3];
@@ -3271,7 +3278,7 @@ int group_facts(const TopoHost& T, const int32_t* gb, int64_t words, int g, bool
   if (sf->nw > 0)
     for (int ri = 0; ri < q; ++ri) {
       if (roles[4 * ri + 1] <= 0) continue;  // a role without pending replicas has no row
-      const long long amax = std::min(anch_w[ri] + sf->role_bound[ri], sat);
+      const long long amax = std::min(anch_w[ri] + (role_bound ? role_bound : sf->role_bound)[ri], sat);
       if (amax >= amax_limit)
         GROUP_FAIL(RBGTOPO_EINEXACT, "group %d role %d: max score bound >= 2^24 (anchor weight %lld x row weight %lld)", g, ri, amax, row_w);
     }
@@ -3855,6 +3862,344 @@ int32_t place_groups_impl(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int3
 }
 }  // namespace
 
+// ---- leader-worker replicas (rbgtopo_place_groups_lw, DESIGN.md §3.11)
+namespace {
+// The next pod wave of a group from replica cursor (cr, taken): the roles of one level in order, at most
+// RBGTOPO_MAX_STEP_ROLES role rows and RBGTOPO_MAX_STEP_REPLICAS pods, a replica's S pods never split.  Returns the
+// role rows; w[k] = (role, first replica, replicas).
+int lw_wave(const int32_t* roles, int q, const int32_t* rp, int cr, int taken, int (*w)[3]) {
+  while (cr < q && roles[4 * cr + 1] - taken <= 0) { ++cr; taken = 0; }
+  if (cr >= q) return 0;
+  const int level = roles[4 * cr];
+  int P = 0, n = 0;
+  while (cr < q && roles[4 * cr] == level && P < RBGTOPO_MAX_STEP_ROLES) {
+    const int left = roles[4 * cr + 1] - taken;
+    if (left <= 0) { ++cr; taken = 0; continue; }
+    const int S = rp[2 * cr];
+    const int take = std::min(left, (RBGTOPO_MAX_STEP_REPLICAS - n) / S);
+    if (take == 0) break;
+    w[P][0] = cr; w[P][1] = taken; w[P][2] = take;
+    ++P;
+    n += take * S;
+    taken += take;
+    if (taken == roles[4 * cr + 1]) { ++cr; taken = 0; }
+  }
+  return P;
+}
+
+struct LwRun {  // one group while its pod waves are placed
+  const int32_t* rec = nullptr;
+  const int32_t* roles = nullptr;
+  const int32_t* pair = nullptr;
+  const int32_t* rp = nullptr;  // (S, C) per role
+  int q = 0, fixed_domain = -1, status = RBGTOPO_PLACED_ALL;
+  bool failed = false;
+  int cur_role = 0, cur_taken = 0;  // replica cursor
+  long long pod0 = 0;               // the group's first pod in assign
+  int ord0[RBGTOPO_MAX_GROUP_ROLES] = {0};      // first pod of every role inside the group's range
+  int unplaced[RBGTOPO_MAX_GROUP_ROLES] = {0};  // pods
+  std::vector<int32_t> anchors;     // (node, role, count)*
+  std::map<int, int> consumed;      // node -> amount
+  int w[RBGTOPO_MAX_STEP_ROLES][3];
+  int P = 0;
+  bool done() const { return failed || cur_role >= q; }
+};
+
+// Validation: the checks and messages of rbgtopo_place_groups (group_facts phase 1, offsets), the role_pods table, then
+// group_facts phase 2 (scheduled pods, exactness bound) with the bound taken over the pod waves.
+int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
+                long long* total_pods) {
+  if (words < RBGTOPO_HDR_WORDS || gb[0] != RBGTOPO_GROUPS_MAGIC || gb[1] != RBGTOPO_ABI_VERSION || gb[3] != words)
+    return fail(RBGTOPO_EINVAL, "bad groups blob header");
+  const int ng = gb[2];
+  if (ng < 0 || (int64_t)RBGTOPO_HDR_WORDS + (int64_t)ng * RBGTOPO_GROUP_WORDS > words)
+    return fail(RBGTOPO_EINVAL, "group table exceeds blob");
+  const Topology& T = c->topo;
+  TopoHost th;
+  th.n = T.n;
+  th.n_domains = T.n_domains;
+  th.n_levels = installed_levels(c);
+  th.place_levels = places_levels(c);
+  th.level_nd = T.lvl_nd.empty() ? nullptr : T.lvl_nd.data();
+  th.degp1 = T.h_degp1.data();
+  th.max_degp1 = T.max_degp1;
+  th.wsum_max = T.wsum_max;
+  const long long row_w = T.wsum_max + RBGTOPO_SELF_W;
+  const long long amax_limit = ((1LL << 24) + row_w - 1) / row_w;
+  GroupFacts f;
+  for (int g = 0; g < ng; ++g) {
+    int rc = group_facts(th, gb, words, g, true, amax_limit, row_w, &f, 1);
+    if (rc) return rc;
+  }
+  long long pacc = 0, qsum = 0;
+  for (int g = 0; g < ng; ++g) {
+    const int32_t* rec = group_rec(gb, g);
+    long long pend = 0;
+    for (int i = 0; i < rec[3]; ++i) pend += gb[rec[4] + 4 * i + 1];
+    if (rec[8] != pacc || rec[9] != pend) return fail(RBGTOPO_EINVAL, "group %d: bad assign_off/n_pending", g);
+    pacc += pend;
+    if (pacc > 0x3FFFFFF0LL) return fail(RBGTOPO_ELIMIT, "pending replicas exceed 2^30");
+    qsum += rec[3];
+  }
+  if (gb[4] != pacc) return fail(RBGTOPO_EINVAL, "total pending mismatch");
+  if (!rp || rp_words != 2 * qsum)
+    return fail(RBGTOPO_EINVAL, "role_pods: %lld words for %lld roles (2 per role)", (long long)rp_words, qsum);
+  const int nl = installed_levels(c);
+  long long pods = 0;
+  const long long sat = 1LL << 40;
+  for (int g = 0, r0 = 0; g < ng; ++g) {
+    const int32_t* rec = group_rec(gb, g);
+    const int q = rec[3];
+    const int32_t* roles = gb + rec[4];
+    const int32_t* pair = gb + rec[5];
+    const int32_t* grp = rp + 2LL * r0;
+    r0 += q;
+    for (int i = 0; i < q; ++i) {
+      if (grp[2 * i] < 1 || grp[2 * i] > RBGTOPO_MAX_STEP_REPLICAS)
+        return fail(RBGTOPO_EINVAL, "group %d role %d: %d pods per replica (1 .. %d)", g, i, grp[2 * i], RBGTOPO_MAX_STEP_REPLICAS);
+      if (grp[2 * i + 1] < -1 || grp[2 * i + 1] > nl)
+        return fail(RBGTOPO_EINVAL, "group %d role %d: co-location level %d (-1 .. %d installed)", g, i, grp[2 * i + 1], nl);
+      pods += (long long)roles[4 * i + 1] * grp[2 * i];
+    }
+    if (pods > 0x3FFFFFF0LL) return fail(RBGTOPO_ELIMIT, "pending pods exceed 2^30");
+    // The exactness bound of §3.4 per role over the pod waves: the largest need·F_CAP + sum_j pair·(pods of j placed
+    // before the wave) any wave of the call can stage.  A gang group stops at its first wave with an unplaced replica,
+    // so every earlier pod is placed.  Any other group may reach a wave with pods of earlier waves unplaced: each one
+    // raises need by 1 (up to the cap) and lowers the anchor weight by its pair weight, so the bound takes the worst
+    // such mix — the per-wave validation can then never find an inexact step in the middle of a call.
+    const bool gang = (rec[1] & RBGTOPO_STEP_GANG) != 0;
+    long long bound[RBGTOPO_MAX_GROUP_ROLES] = {0}, placed[RBGTOPO_MAX_GROUP_ROLES] = {0};
+    int cr = 0, taken = 0, w[RBGTOPO_MAX_STEP_ROLES][3];
+    for (int P; (P = lw_wave(roles, q, grp, cr, taken, w)) > 0;) {
+      for (int k = 0; k < P; ++k) {
+        const int ri = w[k][0];
+        long long need = 0, bnd = 0;
+        for (int j = 0; j < q; ++j) {
+          if (pair[ri * q + j] > 0) need += (long long)roles[4 * j + 1] * grp[2 * j] - placed[j];
+          bnd = std::min(bnd + (long long)pair[ri * q + j] * placed[j], sat);
+        }
+        bnd += std::min<long long>(need, RBGTOPO_NEED_CAP) * RBGTOPO_F_CAP;
+        long long left[RBGTOPO_MAX_GROUP_ROLES];  // earlier pods that may still be unplaced, per role
+        for (int j = 0; j < q; ++j) left[j] = gang ? 0 : placed[j];
+        for (long long room = RBGTOPO_NEED_CAP - std::min<long long>(need, RBGTOPO_NEED_CAP); room > 0;) {
+          int best = -1;  // the smallest pair weight in (0, F_CAP) gains the most per unplaced pod
+          for (int j = 0; j < q; ++j)
+            if (left[j] > 0 && pair[ri * q + j] > 0 && pair[ri * q + j] < RBGTOPO_F_CAP &&
+                (best < 0 || pair[ri * q + j] < pair[ri * q + best]))
+              best = j;
+          if (best < 0) break;
+          const long long u = std::min(room, left[best]);
+          bnd += u * (RBGTOPO_F_CAP - pair[ri * q + best]);
+          room -= u;
+          left[best] = 0;
+        }
+        bound[ri] = std::max(bound[ri], bnd);
+      }
+      for (int k = 0; k < P; ++k) placed[w[k][0]] += (long long)w[k][2] * grp[2 * w[k][0]];
+      cr = w[P - 1][0];
+      taken = w[P - 1][1] + w[P - 1][2];
+    }
+    int rc = group_facts(th, gb, words, g, true, amax_limit, row_w, &f, 2, bound);
+    if (rc) return rc;
+  }
+  *total_pods = pods;
+  return RBGTOPO_OK;
+}
+
+// One CTA per step up to the CTAs that fit the device at once; with a co-location level in the wave, no more CTAs
+// than kLwScratchBytes of level-C domain scratch (12 bytes per domain) allow.
+constexpr size_t kLwScratchBytes = 64u << 20;
+
+int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
+                    int32_t* assign, int32_t* status, int32_t* domain) {
+  long long total_pods = 0;
+  int rc = lw_validate(c, gb, words, rp, rp_words, &total_pods);
+  if (rc) return rc;
+  const Topology& T = c->topo;
+  const size_t smem = (size_t)((T.n + 31) / 32) * 4;
+  if (smem > kFastSmemMax) return fail(RBGTOPO_ELIMIT, "leader-worker placement: %d nodes exceed the room bitmap", T.n);
+  const int ng = gb[2];
+  std::vector<LwRun> runs(ng);
+  long long pod_acc = 0;
+  for (int g = 0, r0 = 0; g < ng; ++g) {
+    LwRun& r = runs[g];
+    r.rec = group_rec(gb, g);
+    r.q = r.rec[3];
+    r.roles = gb + r.rec[4];
+    r.pair = gb + r.rec[5];
+    r.rp = rp + 2LL * r0;
+    r0 += r.q;
+    r.fixed_domain = r.rec[2];
+    r.pod0 = pod_acc;
+    for (int i = 0, acc = 0; i < r.q; ++i) {
+      r.ord0[i] = acc;
+      r.unplaced[i] = r.roles[4 * i + 1] * r.rp[2 * i];
+      acc += r.unplaced[i];
+    }
+    for (int i = 0; i < r.q; ++i) pod_acc += r.unplaced[i];
+    r.anchors.assign(gb + r.rec[7], gb + r.rec[7] + 3LL * r.rec[6]);
+    while (r.cur_role < r.q && r.roles[4 * r.cur_role + 1] == 0) ++r.cur_role;
+  }
+  for (long long k = 0; k < total_pods; ++k) assign[k] = -1;
+  LwLevels lv{};
+  for (int L = 0; L <= installed_levels(c); ++L) lv.nd[L] = level_domains(T, L);
+
+  Batch* b = nullptr;
+  rc = acquire_batch(c, &b);
+  if (rc) return rc;
+  cudaStream_t s = stream_of(c, b);
+  rbgtopo_timing total{};
+  std::vector<int32_t> blob, w_assign, w_status, w_domain, side;
+  std::vector<int> active;
+  while (true) {
+    active.clear();
+    for (int g = 0; g < ng; ++g)
+      if (!runs[g].done()) active.push_back(g);
+    if (active.empty()) break;
+    // ---- this wave's step blob: role counts in pods, need over unplaced pods
+    const int ns = (int)active.size();
+    blob.assign((size_t)RBGTOPO_HDR_WORDS + (size_t)ns * RBGTOPO_STEP_WORDS, 0);
+    side.assign((size_t)ns * MAXP, 0);
+    int racc = 0, rowacc = 0, dmax = 0;
+    for (int i = 0; i < ns; ++i) {
+      LwRun& r = runs[active[i]];
+      r.P = lw_wave(r.roles, r.q, r.rp, r.cur_role, r.cur_taken, r.w);
+      int32_t st[RBGTOPO_STEP_WORDS] = {0};
+      st[0] = r.rec[0];
+      st[1] = r.rec[1] & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG);
+      st[2] = (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) ? r.fixed_domain : -1;
+      st[3] = r.P;
+      while (blob.size() & 3) blob.push_back(0);  // role records are read as 16-byte vectors
+      st[4] = (int32_t)blob.size();
+      int n = 0;
+      for (int p = 0; p < r.P; ++p) {
+        const int ri = r.w[p][0], S = r.rp[2 * ri], C = r.rp[2 * ri + 1];
+        int need = 0;
+        for (int q = 0; q < r.q; ++q)
+          if (r.pair[ri * r.q + q] > 0) need += r.unplaced[q];
+        blob.push_back(r.w[p][2] * S);
+        blob.push_back(r.roles[4 * ri + 2]);
+        blob.push_back(std::min(need, RBGTOPO_NEED_CAP));
+        blob.push_back(r.roles[4 * ri + 3] & RBGTOPO_ROLE_EXCLUSIVE);
+        side[(size_t)i * MAXP + p] = lw_pack_role(S, C);
+        if (C >= 0) dmax = std::max(dmax, lv.nd[C]);
+        n += r.w[p][2] * S;
+      }
+      st[5] = r.q;
+      st[6] = (int32_t)blob.size();
+      for (int p = 0; p < r.P; ++p) blob.insert(blob.end(), r.pair + r.w[p][0] * r.q, r.pair + (r.w[p][0] + 1) * r.q);
+      st[7] = (int32_t)(r.anchors.size() / 3);
+      st[8] = (int32_t)blob.size();
+      blob.insert(blob.end(), r.anchors.begin(), r.anchors.end());
+      st[9] = (int32_t)r.consumed.size();
+      st[10] = (int32_t)blob.size();
+      for (const auto& kv : r.consumed) { blob.push_back(kv.first); blob.push_back(kv.second); }  // by node, one per node
+      st[11] = n;
+      st[12] = racc;
+      st[13] = rowacc;
+      st[14] = r.rec[10];  // exclusive level
+      racc += n;
+      rowacc += r.P;
+      memcpy(blob.data() + RBGTOPO_HDR_WORDS + (size_t)i * RBGTOPO_STEP_WORDS, st, sizeof st);
+    }
+    blob[0] = RBGTOPO_BLOB_MAGIC;
+    blob[1] = RBGTOPO_ABI_VERSION;
+    blob[2] = ns;
+    blob[3] = (int32_t)blob.size();
+    blob[4] = racc;
+    blob[5] = rowacc;
+    w_assign.resize(racc);
+    w_status.resize(ns);
+    w_domain.resize(ns);
+    rc = stage_into(c, b, blob.data(), (int64_t)blob.size());
+    if (rc) break;
+    rc = [&]() -> int {
+      // grid: every step resident at once if the device holds them, the level-C scratch bounded by kLwScratchBytes
+      int per_sm = 0;
+      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_lw_assign, LW_THREADS, smem));
+      long long grid = std::min<long long>(ns, (long long)std::max(1, per_sm) * c->sm_count);
+      if (dmax > 0) grid = std::min<long long>(grid, std::max<long long>(1, kLwScratchBytes / (12LL * dmax)));
+      CK(b->lw.reserve(side.size()));
+      CK(b->h_lw.reserve(side.size()));
+      CK(b->lw_best.reserve((size_t)grid * dmax + 1));
+      CK(b->lw_cap.reserve((size_t)grid * dmax + 1));
+      memcpy(b->h_lw.p, side.data(), side.size() * 4);
+      CK(cudaMemcpyAsync(b->lw.p, b->h_lw.p, side.size() * 4, cudaMemcpyHostToDevice, s));
+      CK(cudaStreamWaitEvent(s, c->base_ready, 0));  // a pending snapshot refresh
+      CK(cudaStreamWaitEvent(s, c->topo_ready, 0));
+      int r2 = launch_score(c, b, s);
+      if (r2) return r2;
+      k_lw_assign<<<(unsigned)grid, LW_THREADS, smem, s>>>(topo_dev(c), batch_dev(c, b), b->lw.p, b->lw_best.p,
+                                                           b->lw_cap.p, dmax, lv);
+      CK(cudaGetLastError());
+      b->pend_launches += 2;
+      b->ran = true;
+      return RBGTOPO_OK;
+    }();
+    if (!rc) rc = fetch_batch(c, b, w_assign.data(), w_status.data(), w_domain.data());
+    if (rc) break;
+    {
+      std::lock_guard<std::mutex> g(c->stat_mu);
+      c->launches += 2;
+      total.h2d_ms += c->last.h2d_ms; total.d2h_ms += c->last.d2h_ms;
+      total.total_ms += c->last.total_ms; total.launches += c->last.launches;
+      total.scores += c->last.scores; total.algo_bytes += c->last.algo_bytes;
+      total.h2d_words += c->last.h2d_words;
+    }
+    // ---- absorb the placements: every pod placed is an anchor (node, role, 1) and consumes (node, demand)
+    int off = 0;
+    for (int i = 0; i < ns; ++i) {
+      LwRun& r = runs[active[i]];
+      bool any = false;
+      for (int p = 0; p < r.P; ++p) {
+        const int ri = r.w[p][0], S = r.rp[2 * ri];
+        const long long first = r.pod0 + r.ord0[ri] + (long long)r.w[p][1] * S;
+        for (int k = 0; k < r.w[p][2] * S; ++k, ++off) {
+          const int node = w_assign[off];
+          assign[first + k] = node;
+          if (node < 0) continue;
+          any = true;
+          r.anchors.push_back(node); r.anchors.push_back(ri); r.anchors.push_back(1);
+          r.consumed[node] += r.roles[4 * ri + 2];
+          r.unplaced[ri] -= 1;
+        }
+      }
+      if ((r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) && w_domain[i] >= 0 && any) r.fixed_domain = w_domain[i];
+      r.status = std::max(r.status, w_status[i]);
+      if ((r.rec[1] & RBGTOPO_STEP_GANG) && w_status[i] != RBGTOPO_PLACED_ALL) r.failed = true;
+      r.cur_role = r.w[r.P - 1][0];
+      r.cur_taken = r.w[r.P - 1][1] + r.w[r.P - 1][2];
+      if (r.cur_taken >= r.roles[4 * r.cur_role + 1]) { ++r.cur_role; r.cur_taken = 0; }
+      while (r.cur_role < r.q && r.roles[4 * r.cur_role + 1] == 0) ++r.cur_role;
+    }
+  }
+  if (!rc) {
+    for (int g = 0; g < ng; ++g) {
+      const LwRun& r = runs[g];
+      const bool excl = (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) != 0;
+      if (r.failed) {  // gang: nothing of the group is placed
+        long long pods = 0;
+        for (int i = 0; i < r.q; ++i) pods += (long long)r.roles[4 * i + 1] * r.rp[2 * i];
+        for (long long k = 0; k < pods; ++k) assign[r.pod0 + k] = -1;
+        if (status) status[g] = RBGTOPO_GANG_FAILED;
+        if (domain) domain[g] = -1;
+      } else {
+        if (status) status[g] = r.status;
+        if (domain) domain[g] = excl ? r.fixed_domain : -1;
+      }
+    }
+    harvest_base_ms(c);
+    std::lock_guard<std::mutex> g(c->stat_mu);
+    total.base_ms = c->topo.base_ms;
+    c->last = total;
+  } else {
+    cudaStreamSynchronize(s);
+  }
+  release_batch(c, b);
+  return rc;
+}
+}  // namespace
+
 int32_t rbgtopo_place_groups(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign,
                              int32_t* status, int32_t* domain) {
   if (!c || !gb || !assign) return fail(RBGTOPO_EINVAL, "null argument");
@@ -3887,6 +4232,17 @@ int32_t rbgtopo_place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_
   const int rc = place_groups_committed(c, gb, words, assign, status, domain, &r);
   if (rounds) *rounds = r;
   return rc;
+}
+
+int32_t rbgtopo_place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* role_pods,
+                                int64_t role_pods_words, int32_t* assign, int32_t* status, int32_t* domain) {
+  if (!c || !gb || !assign || !role_pods) return fail(RBGTOPO_EINVAL, "null argument");
+  if (c->cfg.world > 1)
+    return fail(RBGTOPO_ELIMIT, "leader-worker placement needs world == 1: a rank holds only its slab of every dense row");
+  std::shared_lock<std::shared_mutex> lk(c->topo_mu);
+  if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
+  CK(cudaSetDevice(c->cfg.device));
+  return place_groups_lw(c, gb, words, role_pods, role_pods_words, assign, status, domain);
 }
 
 int32_t rbgtopo_plan_describe(const int32_t* gb, int64_t words, int32_t n_nodes, int32_t n_domains,

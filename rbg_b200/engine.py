@@ -176,6 +176,33 @@ class TopoPlacer:
             _p(alt_node) if n_alt > 0 else None, _p(alt_score, _lib.f32p) if n_alt > 0 else None))
         return assign[:tp], status[:ng], domain[:ng], score[:tp], alt_node[:tp], alt_score[:tp]
 
+    def place_groups_lw(self, groups_blob: np.ndarray, role_pods) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """Leader-worker replicas (DESIGN.md §3.11): role_pods holds (S, C) per role of every group in blob order —
+        S pods per replica, all inside one domain of co-location level C (-1: none).  Returns (assign per pod in
+        (group, role, ordinal, pod) order, status, domain)."""
+        gb = _i32(groups_blob)
+        rp = _i32(np.asarray(role_pods, dtype=np.int64).reshape(-1))
+        ng = int(gb[2])
+        pods = 0
+        if len(rp) % 2 == 0 and len(gb) >= 8:
+            S = rp[0::2].astype(np.int64)
+            k = 0
+            for g in range(ng):
+                rec = 8 + 12 * g
+                if rec + 12 > len(gb):
+                    break
+                q, role_off = int(gb[rec + 3]), int(gb[rec + 4])
+                if q < 0 or k + q > len(S) or role_off < 0 or role_off + 4 * q > len(gb):
+                    break
+                pods += int((gb[role_off + 1:role_off + 4 * q:4].astype(np.int64) * np.maximum(S[k:k + q], 0)).sum())
+                k += q
+        assign = np.empty(max(pods, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        self._check(self.lib.rbgtopo_place_groups_lw(self._h, _p(gb), len(gb), _p(rp), len(rp), _p(assign),
+                                                     _p(status), _p(domain)))
+        return assign[:pods], status[:ng], domain[:ng]
+
     # -- staged (device-resident) batches
     def stage(self, blob: np.ndarray) -> int:
         blob = _i32(blob)

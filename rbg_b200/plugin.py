@@ -42,6 +42,7 @@ ROLE_DISABLE_EXCLUSIVE_KEY = RBG_PREFIX + "role-disable-exclusive"  # annotation
 GANG_SCHEDULING_KEY = RBG_PREFIX + "group-gang-scheduling"          # annotation.go:37
 PLACEMENT_HINT_KEY = RBG_PREFIX + "b200-topo-placement"             # new: RoleID -> node map
 PLACEMENT_ALTERNATES_KEY = RBG_PREFIX + "b200-topo-alternates"       # new: RoleID -> ranked fallback nodes
+COLOCATE_KEY = RBG_PREFIX + "b200-topo-colocate"                     # new, per role: topology key of one replica's pods
 SCHEDULER_PLUGIN_NAME = "b200-topo"                                 # --scheduler-name value
 # what the wrapped gang plugins inject into the pod template when gang scheduling is on
 KUBE_POD_GROUP_LABEL = "pod-group.scheduling.sigs.k8s.io/name"      # k8s-scheduler-plugin/manager.go:49,91-98
@@ -295,7 +296,7 @@ class B200TopoPodGroupManager:
     """Third ``PodGroupManager`` implementation (plugin type "b200-topo")."""
 
     def __init__(self, placer: TopoPlacer, inner: Optional[str] = "scheduler-plugins",
-                 exclusive_keys: Optional[Sequence[str]] = None, alternates: int = 0):
+                 exclusive_keys: Optional[Sequence[str]] = None, alternates: int = 0, leader_worker: bool = False):
         """inner: the gang plugin this manager wraps for the PodGroup CR and the pod-group label —
         "scheduler-plugins" (kube), "volcano" or None (the Go manager takes the implementation object).
         exclusive_keys: the topology keys exclusive groups may name (DESIGN.md §3.9), keys[0] = the level-0 label.
@@ -307,7 +308,14 @@ class B200TopoPodGroupManager:
         (no_hint[(ns, name)]): a hint into a domain of the wrong key is worse than none.
         alternates: next-best nodes per replica carried beside the hint (DESIGN.md §3.10, at most 8).  0 keeps the
         single-node hint; with n > 0 the snapshot call is rbgtopo_place_groups_ranked, which places identically and
-        also ranks, per replica, the nodes that still have room once its group is placed."""
+        also ranks, per replica, the nodes that still have room once its group is placed.
+        leader_worker: a group with a role of lws_size > 1 is placed through rbgtopo_place_groups_lw (DESIGN.md
+        §3.11): every replica of such a role is lws_size pods, placed all or nothing, and the hints are keyed by pod
+        name, "{rbg}-{role}-{ordinal}-{k}" (k = 0 the leader); standalone roles keep "{rbg}-{role}-{ordinal}".  A
+        role annotation COLOCATE_KEY names the topology key whose one domain must hold all pods of a replica; it
+        resolves against exclusive_keys like an exclusive key (None: the level-0 label).  An unknown key, a level
+        the snapshot does not hold, a committed batch or alternates leave such a group without a hint and log why.
+        False (default): those groups are placed as before, one pod per replica."""
         if not 0 <= alternates <= 8:
             raise ValueError(f"alternates must be in [0, 8], got {alternates}")
         self.alternates = int(alternates)
@@ -315,6 +323,7 @@ class B200TopoPodGroupManager:
         self.arith = HostArith()
         self.inner = inner
         self.exclusive_keys = None if exclusive_keys is None else tuple(exclusive_keys)
+        self.leader_worker = bool(leader_worker)
         self.no_hint: Dict[Tuple[str, str], str] = {}
         self._hints: Dict[Tuple[str, str], Placement] = {}
 
@@ -339,6 +348,13 @@ class B200TopoPodGroupManager:
         keep, skipped = [], {}
         for i, r in enumerate(rbgs):
             _, reason = self.exclusive_level(r, committed)
+            if not reason and self.is_leader_worker(r):
+                if committed:
+                    reason = "leader-worker replicas: committed batches place one pod per replica"
+                elif self.alternates:
+                    reason = "leader-worker replicas: no ranked alternates for them"
+                else:
+                    reason = self.role_pods(r)[1]
             if not reason:
                 keep.append(r)
                 continue
@@ -347,6 +363,27 @@ class B200TopoPodGroupManager:
             logging.getLogger(__name__).info("no placement hint for %s/%s: %s", r.namespace, r.name, reason)
             skipped[i] = Placement(RBGTOPO_NO_HINT, {}, -1, 0)
         return keep, skipped
+
+    def is_leader_worker(self, rbg: RoleBasedGroup) -> bool:
+        """Placed through rbgtopo_place_groups_lw: the manager was asked to and a role runs multi-pod replicas."""
+        return self.leader_worker and any(r.lws_size > 1 for r in rbg.roles)
+
+    def role_pods(self, rbg: RoleBasedGroup) -> Tuple[List[Tuple[int, int]], str]:
+        """((pods per replica S, co-location level C) per role in spec order, reason for no hint or "")."""
+        out = []
+        for r in rbg.roles:
+            key, level = r.annotations.get(COLOCATE_KEY), -1
+            if key is not None:
+                if self.exclusive_keys is None:
+                    level = 0
+                elif key not in self.exclusive_keys:
+                    return [], f"co-location key {key!r} of role {r.name} is not configured"
+                else:
+                    level = self.exclusive_keys.index(key)
+                    if level > getattr(self.placer, "_n_levels", 0):
+                        return [], f"co-location key {key!r} of role {r.name}: the snapshot holds no level {level}"
+            out.append((max(1, r.lws_size), level))
+        return out, ""
 
     @staticmethod
     def _merge(rbgs, placed, skipped):
@@ -385,14 +422,32 @@ class B200TopoPodGroupManager:
         rbgs, skipped = self._split_no_hint(rbgs, committed)
         if not rbgs:
             return self._merge(all_rbgs, [], skipped)
-        blob, runs = self.groups_blob(rbgs)
-        alt_node = None
-        if committed:
-            assign, status, domain, _ = self.placer.place_groups_committed(blob)
-        elif self.alternates > 0:
-            assign, status, domain, _, alt_node, _ = self.placer.place_groups_ranked(blob, self.alternates)
-        else:
-            assign, status, domain = self.placer.place_groups(blob)
+        lw = [i for i, r in enumerate(rbgs) if self.is_leader_worker(r)]
+        plain = [i for i, r in enumerate(rbgs) if not self.is_leader_worker(r)]
+        done: List[Optional[Placement]] = [None] * len(rbgs)   # by position in rbgs
+        if plain:
+            blob, runs = self.groups_blob([rbgs[i] for i in plain])
+            alt_node = None
+            if committed:
+                assign, status, domain, _ = self.placer.place_groups_committed(blob)
+            elif self.alternates > 0:
+                assign, status, domain, _, alt_node, _ = self.placer.place_groups_ranked(blob, self.alternates)
+            else:
+                assign, status, domain = self.placer.place_groups(blob)
+            for i, p in zip(plain, self._placements(runs, assign, status, domain, alt_node, None)):
+                done[i] = p
+        if lw:
+            blob, runs = self.groups_blob([rbgs[i] for i in lw])
+            pods = [self.role_pods(g.rbg)[0] for g in runs]
+            role_pods = [pods[k][ri] for k, g in enumerate(runs) for ri in g.order]
+            assign, status, domain = self.placer.place_groups_lw(blob, role_pods)
+            for i, p in zip(lw, self._placements(runs, assign, status, domain, None, pods)):
+                done[i] = p
+        return self._merge(all_rbgs, done, skipped)
+
+    def _placements(self, runs, assign, status, domain, alt_node, pods) -> List[Placement]:
+        """Per group: the hints of one placement call.  pods: (S, C) per role of every group (leader-worker call) —
+        a role with S > 1 gets one key per pod, "{rbg}-{role}-{ordinal}-{k}" — or None (one pod per replica)."""
         out, off = [], 0
         n_nodes = self.placer.n_nodes
         for i, g in enumerate(runs):
@@ -400,16 +455,19 @@ class B200TopoPodGroupManager:
             alts: Dict[str, List[int]] = {}
             for ri in g.order:
                 role = g.rbg.roles[ri]
+                S = 1 if pods is None else pods[i][ri][0]
                 for c in range(g.pending[ri]):
                     key = f"{g.rbg.name}-{role.name}-{g.first_ordinal[ri] + c}"
-                    nodes[key] = int(assign[off])
-                    if alt_node is not None:
-                        alts[key] = [int(x) for x in alt_node[off] if x >= 0]
-                    off += 1
+                    for k in range(S):
+                        pod = key if S == 1 else f"{key}-{k}"
+                        nodes[pod] = int(assign[off])
+                        if alt_node is not None:
+                            alts[pod] = [int(x) for x in alt_node[off] if x >= 0]
+                        off += 1
             p = Placement(int(status[i]), nodes, int(domain[i]), len(nodes) * n_nodes, alts)
             self._hints[(g.rbg.namespace, g.rbg.name)] = p
             out.append(p)
-        return self._merge(all_rbgs, out, skipped)
+        return out
 
     # -- the same loop in Python over single-level batches (rbgtopo_score_assign):
     #    kept as the readable mirror of the C++ loop and for cross-checks.
