@@ -89,6 +89,15 @@ static int32_t rbgtopo_go_place_groups_lw(rbgtopo_ctx* ctx, const int32_t* group
   rbgtopo_go_err(ctx, rc, err);
   return rc;
 }
+static int32_t rbgtopo_go_place_groups_lw_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t words,
+                                                 const int32_t* role_pods, int64_t role_pods_words, int32_t n_alt,
+                                                 int32_t* assign, int32_t* status, int32_t* domain, float* score,
+                                                 int32_t* alt_node, float* alt_score, char* err) {
+  int32_t rc = rbgtopo_place_groups_lw_ranked(ctx, groups, words, role_pods, role_pods_words, n_alt, assign, status,
+                                              domain, score, alt_node, alt_score);
+  rbgtopo_go_err(ctx, rc, err);
+  return rc;
+}
 */
 import "C"
 
@@ -264,4 +273,25 @@ func (p *placer) placeGroupsLW(blob, rolePods []int32, nPods int) (assign, statu
 		return nil, nil, nil, err
 	}
 	return assign[:nPods], status[:nGroups], domain[:nGroups], nil
+}
+
+// placeGroupsLWRanked: placeGroupsLW plus, per pod, up to nAlt next-best nodes that still have room once its group is
+// placed and that keep a co-located replica inside its domain (DESIGN.md §3.12); altNode[p*nAlt+i] = -1 where there
+// are fewer.  assign / status / domain are placeGroupsLW's.
+func (p *placer) placeGroupsLWRanked(blob, rolePods []int32, nPods, nAlt int) (assign, status, domain, altNode []int32, err error) {
+	nGroups := int(blob[2])
+	assign = make([]int32, max(nPods, 1))
+	status = make([]int32, max(nGroups, 1))
+	domain = make([]int32, max(nGroups, 1))
+	score := make([]float32, max(nPods, 1))
+	altNode = make([]int32, max(nPods*nAlt, 1))
+	altScore := make([]float32, max(nPods*nAlt, 1))
+	var buf [C.RBGTOPO_GO_ERRLEN]C.char
+	rc := C.rbgtopo_go_place_groups_lw_ranked(p.ctx, p32(blob), C.int64_t(len(blob)), p32(rolePods),
+		C.int64_t(len(rolePods)), C.int32_t(nAlt), p32(assign), p32(status), p32(domain),
+		(*C.float)(unsafe.Pointer(&score[0])), p32(altNode), (*C.float)(unsafe.Pointer(&altScore[0])), &buf[0])
+	if err = mkErr(rc, &buf); err != nil {
+		return nil, nil, nil, nil, err
+	}
+	return assign[:nPods], status[:nGroups], domain[:nGroups], altNode[:nPods*nAlt], nil
 }

@@ -74,7 +74,9 @@ type Manager struct {
 
 // SetLeaderWorker opts into leader-worker placement (DESIGN.md §3.11): a group with a role of LeaderWorkerPattern.Size
 // > 1 is placed pod by pod, every replica's pods all or nothing and, with the ColocateKey annotation, inside one domain
-// of that key; its hints are keyed by pod name.  Off (the default): such groups are placed one pod per replica.
+// of that key; its hints are keyed by pod name.  With SetAlternates the call is rbgtopo_place_groups_lw_ranked
+// (§3.12) and the alternates are keyed by pod name too, each inside its replica's co-location domain.  Off (the
+// default): such groups are placed one pod per replica.
 func (m *Manager) SetLeaderWorker(on bool) { m.leaderWorker = on }
 
 // colocateLevels: the co-location level per role (rbg.Spec.Roles order, -1 none), or a reason for giving no hint.
@@ -182,9 +184,6 @@ func (m *Manager) ReconcilePodGroup(ctx context.Context, rbg *workloadsv1alpha2.
 	}
 	if m.leaderWorker && g.leaderWorker() {
 		colocate, reason := m.colocateLevels(rbg)
-		if reason == "" && m.alternates > 0 {
-			reason = "leader-worker replicas: no ranked alternates for them"
-		}
 		if reason != "" {
 			m.hints.Delete(key)
 			m.alts.Delete(key)
@@ -192,6 +191,15 @@ func (m *Manager) ReconcilePodGroup(ctx context.Context, rbg *workloadsv1alpha2.
 			return nil
 		}
 		table, pods := g.rolePods(colocate)
+		if m.alternates > 0 {
+			assign, status, _, altNode, err := m.placer.placeGroupsLWRanked(g.blob, table, pods, m.alternates)
+			if err != nil {
+				return m.degrade(logger, key, err)
+			}
+			m.hints.Store(key, g.podIDMap(assign, snap, status[0]))
+			m.alts.Store(key, g.podIDAlternates(altNode, m.alternates, snap, status[0]))
+			return nil
+		}
 		assign, status, _, err := m.placer.placeGroupsLW(g.blob, table, pods)
 		if err != nil {
 			return m.degrade(logger, key, err)

@@ -299,6 +299,37 @@ func (m *marshalled) roleIDAlternates(altNode []int32, nAlt int, snap *snapshot,
 	return out
 }
 
+// podIDAlternates: roleIDAlternates for the ranked leader-worker call (DESIGN.md §3.12), whose altNode[] holds nAlt
+// node indices per pod in assign order: keyed like podIDMap, pods without alternates left out.
+func (m *marshalled) podIDAlternates(altNode []int32, nAlt int, snap *snapshot, status int32) map[string][]string {
+	out := map[string][]string{}
+	if status == 2 {
+		return out
+	}
+	k := 0
+	for _, ri := range m.order {
+		for c := int32(0); c < m.count[ri]; c++ {
+			for pod := int32(0); pod < m.size[ri]; pod++ {
+				var names []string
+				for _, node := range altNode[k*nAlt : (k+1)*nAlt] {
+					if node >= 0 {
+						names = append(names, snap.names[node])
+					}
+				}
+				if len(names) > 0 {
+					id := fmt.Sprintf("%s-%s-%d", m.rbgName, m.names[ri], m.first[ri]+c)
+					if m.size[ri] > 1 {
+						id = fmt.Sprintf("%s-%d", id, pod)
+					}
+					out[id] = names
+				}
+				k++
+			}
+		}
+	}
+	return out
+}
+
 func demandOf(role *workloadsv1alpha2.RoleSpec) int32 {
 	t := role.GetTemplate()
 	if t == nil {

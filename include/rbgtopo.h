@@ -372,6 +372,24 @@ int32_t rbgtopo_place_groups_lw(rbgtopo_ctx* ctx, const int32_t* groups, int64_t
                                 const int32_t* role_pods, int64_t role_pods_words, int32_t* assign,
                                 int32_t* status, int32_t* domain);
 
+/* Ranked alternates for leader-worker pods (DESIGN.md §3.12).  rbgtopo_place_groups_lw — same inputs, validation,
+ * exactness bound, error codes and limits, bit-identical assign / status / domain — plus, per pod p (in assign
+ * order): score[p] = its dense-row score at assign[p], and alt_node[p * n_alt + i] / alt_score[p * n_alt + i],
+ * i < n_alt, the next-best nodes of its row in descending key order (score descending, node ascending).  The row
+ * of a pod is the one of its replica's (wave, role), the row its selection read.  A candidate n has a finite score,
+ * is not assign[p], and has room for one more pod of the role once the group's own pods of this call are taken off
+ * free[] (free[n] - used_g[n] >= demand); for a participating role of an exclusive group it lies in domain[g] (a
+ * domain of the group's exclusive level), and for a role with C >= 0 in the level-C domain of the pod's replica
+ * (dom_C(n) = dom_C(assign[p])), so an alternate never breaks the replica's co-location; with a level whose
+ * domains are single nodes there are none.  Unfilled slots: node -1, score -inf; an unplaced pod and every pod of a
+ * gang-failed group get score -inf and no alternates.  n_alt in [0, RBGTOPO_MAX_ALTERNATES], else RBGTOPO_EINVAL;
+ * status / domain may be NULL; alt_node / alt_score may be NULL when n_alt == 0.  With S = 1 and C = -1 everywhere
+ * all six outputs are bit-identical to rbgtopo_place_groups_ranked's. */
+int32_t rbgtopo_place_groups_lw_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                       const int32_t* role_pods, int64_t role_pods_words, int32_t n_alt,
+                                       int32_t* assign, int32_t* status, int32_t* domain, float* score,
+                                       int32_t* alt_node, float* alt_score);
+
 /* rbgtopo_place_groups pipeline, staged: the groups are compiled into a
  * device-resident multi-wave plan (one step blob, wave-major, expanded on the
  * device), so rbgtopo_run_staged runs ONE score launch for the dense rows of every

@@ -7,10 +7,11 @@
 // registers, merges them per warp and across warps, and writes every replica's list: the merged top list
 // without the replica's own node, truncated to n_alt.  A candidate n has S[n] != -inf, room for one more
 // replica of the role once the group's own placements are taken off free[n], and lies in the required
-// domain.  The room test costs one shared-memory bit per node whatever the group's size: the CTA first marks
-// the nodes where free[n] - used_g[n] < demand from the group's aggregated placements (node, amount).
+// domain, and in the replicas' co-location domain when the role places leader-worker pods (§3.12: there the replicas
+// of a job are the pods of one role row whose replicas chose the same domain D_r).  The room test costs one
+// shared-memory bit per node whatever the group's size: the CTA first marks the nodes where free[n] - used_g[n] < demand from the group's aggregated placements (node, amount).
 // S[n] != -inf already implies free[n] >= demand (§3.3), so free[] is read only for those nodes.
-// Bandwidth-bound: 4 bytes per node and job (+ 4 for the domain of exclusive roles).
+// Bandwidth-bound: 4 bytes per node and job (+ 4 for each domain condition).
 #pragma once
 #include "kernels.cuh"
 
@@ -22,15 +23,17 @@ constexpr int ALT_LIST = RBGTOPO_MAX_ALTERNATES + 1;  // the replica's own node 
 constexpr int ALT_DOM_ANY = -1;                        // job.dom: no domain condition
 static_assert(ALT_WARPS * ALT_LIST <= 96, "cross-warp merge holds three entries per lane");
 
-struct AltJob {  // one role row of one wave (8 words)
+struct AltJob {  // one role row of one wave, or its pods in one co-location domain (10 words)
   int row;       // dense row in `rows` (slab_stride floats apart)
   int demand;
   int dom;       // required domain of `level`, ALT_DOM_ANY = none (a negative value other than that: no node)
   int rep0;      // first replica in the compact replica arrays (own[], out)
-  int nrep;      // replicas of the role in the wave (<= RBGTOPO_MAX_STEP_REPLICAS)
+  int nrep;      // replicas (pods) of the job (<= RBGTOPO_MAX_STEP_REPLICAS)
   int used0;     // the group's placements: used[used0 .. used0 + nused), one entry per node
   int nused;
   int level;     // the group's exclusive level (DESIGN.md §3.9): `dom` is a domain of it
+  int cdom;      // required domain of `clevel`: the co-location domain D_r of the job's pods, ALT_DOM_ANY = none
+  int clevel;
 };
 
 __device__ __forceinline__ float key_score(unsigned long long k) {  // inverse of orderable_u32 on the high word
@@ -49,6 +52,9 @@ __device__ __forceinline__ void alt_insert(unsigned long long (&top)[ALT_LIST], 
 
 // grid: one CTA per job.  Dynamic shared memory: ceil(n / 32) words (the room bitmap).
 // out: per compact replica 1 + 2 * n_alt words — score, n_alt nodes, n_alt scores (fp32 bits).
+// COLOC: some job has a co-location condition.  The <false> form is the ranked placement of one-pod replicas with the
+// registers it had before the condition existed (40; the condition costs 5 more, one CTA per SM less).
+template <bool COLOC>
 __global__ void __launch_bounds__(ALT_THREADS)
 k_alternates(TopoDev t, const float* __restrict__ rows, const AltJob* __restrict__ jobs, const int2* __restrict__ used,
              const int* __restrict__ own, int n_alt, int* __restrict__ out) {
@@ -69,8 +75,9 @@ k_alternates(TopoDev t, const float* __restrict__ rows, const AltJob* __restrict
 
   // ---- scan: per-thread top list in registers
   const float* row = rows + (size_t)J.row * (size_t)t.slab_stride;
-  const bool need_dom = J.dom != ALT_DOM_ANY;
+  const bool need_dom = J.dom != ALT_DOM_ANY, need_col = COLOC && J.cdom != ALT_DOM_ANY;
   const int* const dom_l = at_level(t, J.level).domain;
+  const int* const dom_c = at_level(t, J.clevel).domain;
   unsigned long long top[ALT_LIST];
 #pragma unroll
   for (int j = 0; j < ALT_LIST; ++j) top[j] = 0;
@@ -80,12 +87,15 @@ k_alternates(TopoDev t, const float* __restrict__ rows, const AltJob* __restrict
     const float4 s4 = __ldcs(reinterpret_cast<const float4*>(row + n0));  // read once: do not keep it in L2
     int4 d4 = make_int4(J.dom, J.dom, J.dom, J.dom);
     if (need_dom) d4 = __ldg(reinterpret_cast<const int4*>(dom_l + n0));  // padded past n: safe
+    int4 c4 = make_int4(J.cdom, J.cdom, J.cdom, J.cdom);
+    if (need_col) c4 = __ldg(reinterpret_cast<const int4*>(dom_c + n0));
     const float s[4] = {s4.x, s4.y, s4.z, s4.w};
     const int d[4] = {d4.x, d4.y, d4.z, d4.w};
+    const int cd[4] = {c4.x, c4.y, c4.z, c4.w};
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int m = n0 + j;
-      if (m >= n || s[j] == -INFINITY || d[j] != J.dom) continue;
+      if (m >= n || s[j] == -INFINITY || d[j] != J.dom || (COLOC && cd[j] != J.cdom)) continue;
       const unsigned long long k = make_key(s[j], m);
       if (k <= top[ALT_LIST - 1]) continue;
       if ((sFull[m >> 5] >> (m & 31)) & 1u) continue;

@@ -156,6 +156,7 @@ struct Topology {
   int n_levels = 0;
   int lvl_total_d = 0;                      // sum of the levels' domain counts
   std::vector<int> lvl_nd;                  // [n_levels + 1] domain count of every level (fixed_domain checks)
+  std::vector<int> h_lvl_domain;            // [n_levels][n] levels 1..n_levels on the host (co-located alternates)
   DevBuf<int> lvl_domain, lvl_owner, lvl_doff, lvl_tab, occ_rec;
 };
 
@@ -235,6 +236,7 @@ struct Batch {
   DevBuf<int> lw, lw_cap;
   PinBuf<int> h_lw;
   DevBuf<unsigned long long> lw_best;
+  DevBuf<float> lw_kept;  // its ranked form: the dense rows of every (wave, role), kept across calls like the matrix
   ~Batch() {
     if (stream) cudaStreamDestroy(stream);
     if (stream2) cudaStreamDestroy(stream2);
@@ -1405,7 +1407,8 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
     CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
     CK(cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   }
-  CK(cudaFuncSetAttribute(k_alternates, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
+  for (auto* f : {k_alternates<false>, k_alternates<true>})
+    CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_lw_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_plan_group<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
 #ifdef RBGTOPO_PHASE_CLOCKS
@@ -1730,6 +1733,7 @@ int32_t rbgtopo_set_exclusive_levels(rbgtopo_ctx* c, int32_t n_levels, const int
     CK(cudaMemcpyAsync(T.lvl_doff.p, doff.data(), (size_t)n_lv * 4 + 4, cudaMemcpyHostToDevice, s));
     CK(cudaStreamSynchronize(s));  // the caller's level_domain and the local doff may go once the call returns
     T.n_levels = n_levels;
+    T.h_lvl_domain.assign(level_domain, level_domain + (size_t)n_levels * n);
     T.lvl_total_d = doff[n_lv];
     c->lvl_epoch += 1;
     T.lvl_nd.resize(n_lv);
@@ -1823,8 +1827,9 @@ struct KeptRows {
   std::vector<AltRow> list;
 };
 int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vector<AltRow>& list, const int32_t* gb,
-                   const int32_t* assign, const int32_t* status, const int32_t* domain, const RankReq& rk);
-void alt_clear_group(const int32_t* gb, int g, const RankReq& rk);
+                   const int32_t* rp, const int32_t* assign, const int32_t* status, const int32_t* domain,
+                   const RankReq& rk);
+void alt_clear(const RankReq& rk, int64_t first, int64_t count);
 }  // namespace
 
 // The host-driven wave loop: one batched launch pair per wave, placements fed back
@@ -2033,8 +2038,8 @@ static int32_t place_groups_slow(rbgtopo_ctx* c, const int32_t* gb, int64_t word
   }
   if (!rc && kept) {  // the placements are final now: rank the kept rows
     for (int g = 0; g < ng; ++g)
-      if (!only || (*only)[g]) alt_clear_group(gb, g, *kept->rk);
-    rc = run_alternates(c, b, kept->rows.p, kept->list, gb, assign, status, domain, *kept->rk);
+      if (!only || (*only)[g]) alt_clear(*kept->rk, runs[g].rec[8], runs[g].rec[9]);
+    rc = run_alternates(c, b, kept->rows.p, kept->list, gb, nullptr, assign, status, domain, *kept->rk);
     if (rc) cudaStreamSynchronize(stream_of(c, b));
   }
   release_batch(c, b);
@@ -2091,11 +2096,11 @@ int gen_waves(const int32_t* roles, int q, PlanWave* out) {  // out == nullptr: 
 // ---- ranked placement (DESIGN.md §3.10): the role rows to rank and the kernel launch
 const int32_t* group_rec(const int32_t* gb, int g) { return gb + RBGTOPO_HDR_WORDS + (int64_t)g * RBGTOPO_GROUP_WORDS; }
 
-// A group's replicas start with no score and no alternates (what an unplaced or gang-failed replica keeps).
-void alt_clear_group(const int32_t* gb, int g, const RankReq& rk) {
-  const int32_t* rec = group_rec(gb, g);
-  for (int k = 0; k < rec[9]; ++k) {
-    const int64_t r = (int64_t)rec[8] + k;
+// Replicas (pods) [first, first + count) start with no score and no alternates (what an unplaced or gang-failed one
+// keeps).
+void alt_clear(const RankReq& rk, int64_t first, int64_t count) {
+  for (int64_t k = 0; k < count; ++k) {
+    const int64_t r = first + k;
     rk.score[r] = -INFINITY;
     for (int i = 0; i < rk.n_alt; ++i) {
       rk.alt_node[r * rk.n_alt + i] = -1;
@@ -2133,23 +2138,40 @@ size_t group_role_rows(const int32_t* gb, int g) {
 
 // k_alternates over `list` (rows in `rows`, slab_stride floats apart) on the batch's stream, results scattered into
 // rk; synchronises.  Gang-failed groups are skipped.  The caller cleared the outputs of the groups in `list`.
+// rp: the (S, C) table of place_groups_lw (§3.12), whose `list` entries and assign indices count pods, or nullptr (one
+// pod per replica, no co-location).  used_g sums the demand of every placed pod of the group.  A role with C >= 0
+// makes one job per co-location domain D_r its row's placed replicas chose; its unplaced replicas make none.
 int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vector<AltRow>& list, const int32_t* gb,
-                   const int32_t* assign, const int32_t* status, const int32_t* domain, const RankReq& rk) {
+                   const int32_t* rp, const int32_t* assign, const int32_t* status, const int32_t* domain,
+                   const RankReq& rk) {
   const int F = rk.n_alt;
+  const int ng = gb[2];
+  std::vector<int> r0((size_t)ng + 1, 0);        // first role of every group in rp
+  std::vector<int64_t> pod0((size_t)ng + 1, 0);  // first pod of every group in assign
+  for (int g = 0; g < ng; ++g) {
+    const int32_t* rec = group_rec(gb, g);
+    r0[g + 1] = r0[g] + rec[3];
+    pod0[g + 1] = pod0[g];
+    for (int q = 0; q < rec[3]; ++q) pod0[g + 1] += (int64_t)gb[rec[4] + 4 * q + 1] * (rp ? rp[2 * (r0[g] + q)] : 1);
+  }
+  const Topology& T = c->topo;
   std::vector<AltJob> jobs;
   std::vector<int2> used, tmp;
-  std::vector<int> own, jrow;  // jrow: first replica (assign index) of every job
+  std::vector<int> own, idx, doms;  // own / idx: node and assign index of every compact replica
   std::map<int, int2> placed;  // group -> (first, count) of its aggregated placements in `used`
+  bool coloc = false;
   for (const AltRow& r : list) {
     if (status[r.group] == RBGTOPO_GANG_FAILED) continue;
     const int32_t* rec = group_rec(gb, r.group);
     const int32_t* roles = gb + rec[4];
+    const int32_t* grp = rp ? rp + 2 * r0[r.group] : nullptr;
     auto it = placed.find(r.group);
-    if (it == placed.end()) {  // (node, amount) per node the group's replicas of this call took
+    if (it == placed.end()) {  // (node, amount) per node the group's pods of this call took
       tmp.clear();
-      for (int q = 0, idx = rec[8]; q < rec[3]; ++q)
-        for (int k = 0; k < roles[4 * q + 1]; ++k, ++idx)
-          if (assign[idx] >= 0) tmp.push_back(make_int2(assign[idx], roles[4 * q + 2]));
+      int64_t i = pod0[r.group];
+      for (int q = 0; q < rec[3]; ++q)
+        for (int64_t k = 0; k < (int64_t)roles[4 * q + 1] * (grp ? grp[2 * q] : 1); ++k, ++i)
+          if (assign[i] >= 0) tmp.push_back(make_int2(assign[i], roles[4 * q + 2]));
       std::sort(tmp.begin(), tmp.end(), [](int2 a, int2 b2) { return a.x < b2.x; });
       const int first = (int)used.size();
       for (const int2& u : tmp) {
@@ -2159,23 +2181,46 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
       it = placed.emplace(r.group, make_int2(first, (int)used.size() - first)).first;
     }
     const bool part = (rec[1] & RBGTOPO_STEP_EXCLUSIVE) && (roles[4 * r.role + 3] & RBGTOPO_ROLE_EXCLUSIVE);
+    const int S = grp ? grp[2 * r.role] : 1, C = grp ? grp[2 * r.role + 1] : -1;
     AltJob j{};
     j.row = r.row;
     j.demand = roles[4 * r.role + 2];
     j.dom = part ? (domain[r.group] >= 0 ? domain[r.group] : -2) : ALT_DOM_ANY;
-    j.rep0 = (int)own.size();
-    j.nrep = r.nrep;
     j.used0 = it->second.x;
     j.nused = it->second.y;
     j.level = rec[10];
-    jobs.push_back(j);
-    jrow.push_back(r.rep0);
-    own.insert(own.end(), assign + r.rep0, assign + r.rep0 + r.nrep);
+    j.cdom = ALT_DOM_ANY;
+    auto add = [&](int p, int cnt) {
+      for (int k = 0; k < cnt; ++k) { own.push_back(assign[p + k]); idx.push_back(p + k); }
+    };
+    if (C < 0) {
+      j.rep0 = (int)own.size();
+      add(r.rep0, r.nrep);
+      j.nrep = (int)own.size() - j.rep0;
+      jobs.push_back(j);
+      continue;
+    }
+    // D_r = dom_C of the replica's nodes (all S pods lie in it), in the order of first appearance
+    const int* dc = C == 0 ? T.h_domain.data() : T.h_lvl_domain.data() + (size_t)(C - 1) * T.n;
+    doms.clear();
+    for (int p = r.rep0; p < r.rep0 + r.nrep; p += S)
+      if (assign[p] >= 0 && std::find(doms.begin(), doms.end(), dc[assign[p]]) == doms.end()) doms.push_back(dc[assign[p]]);
+    for (int d : doms) {
+      j.cdom = d;
+      j.clevel = C;
+      j.rep0 = (int)own.size();
+      for (int p = r.rep0; p < r.rep0 + r.nrep; p += S)
+        if (assign[p] >= 0 && dc[assign[p]] == d) add(p, S);
+      j.nrep = (int)own.size() - j.rep0;
+      jobs.push_back(j);
+      coloc = true;
+    }
   }
   if (jobs.empty()) return RBGTOPO_OK;
   const size_t smem = (size_t)((c->topo.n + 31) / 32) * 4;
   if (smem > kFastSmemMax) return fail(RBGTOPO_ELIMIT, "ranked placement: %d nodes exceed the room bitmap", c->topo.n);
-  const size_t w_jobs = jobs.size() * 8, w_used = used.size() * 2, w_own = own.size();
+  static_assert(sizeof(AltJob) % 4 == 0, "jobs are staged as words");
+  const size_t w_jobs = jobs.size() * (sizeof(AltJob) / 4), w_used = used.size() * 2, w_own = own.size();
   const size_t w_in = w_jobs + w_used + w_own, w_out = own.size() * (size_t)(1 + 2 * F);
   cudaStream_t s = stream_of(c, b);
   CK(b->alt.reserve(w_in + w_out));
@@ -2186,23 +2231,22 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
   memcpy(h + w_jobs + w_used, own.data(), w_own * 4);
   int* d = b->alt.p;
   CK(cudaMemcpyAsync(d, h, w_in * 4, cudaMemcpyHostToDevice, s));
-  k_alternates<<<(unsigned)jobs.size(), ALT_THREADS, smem, s>>>(topo_dev(c), rows, reinterpret_cast<const AltJob*>(d),
-                                                                 reinterpret_cast<const int2*>(d + w_jobs),
-                                                                 d + w_jobs + w_used, F, d + w_in);
+  (coloc ? k_alternates<true> : k_alternates<false>)<<<(unsigned)jobs.size(), ALT_THREADS, smem, s>>>(
+      topo_dev(c), rows, reinterpret_cast<const AltJob*>(d), reinterpret_cast<const int2*>(d + w_jobs),
+      d + w_jobs + w_used, F, d + w_in);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(h + w_in, d + w_in, w_out * 4, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   const int* o = h + w_in;
-  for (size_t j = 0; j < jobs.size(); ++j)
-    for (int k = 0; k < jobs[j].nrep; ++k) {
-      const int* e = o + (size_t)(jobs[j].rep0 + k) * (1 + 2 * F);
-      const int64_t r = (int64_t)jrow[j] + k;
-      memcpy(&rk.score[r], e, 4);
-      if (F > 0) {
-        memcpy(rk.alt_node + r * F, e + 1, (size_t)F * 4);
-        memcpy(rk.alt_score + r * F, e + 1 + F, (size_t)F * 4);
-      }
+  for (size_t e = 0; e < own.size(); ++e) {
+    const int* v = o + e * (1 + 2 * F);
+    const int64_t r = idx[e];
+    memcpy(&rk.score[r], v, 4);
+    if (F > 0) {
+      memcpy(rk.alt_node + r * F, v + 1, (size_t)F * 4);
+      memcpy(rk.alt_score + r * F, v + 1 + F, (size_t)F * 4);
     }
+  }
   return RBGTOPO_OK;
 }
 
@@ -2212,10 +2256,10 @@ int rank_plan(rbgtopo_ctx* c, Batch* b, const int32_t* gb, const int32_t* assign
               const int32_t* domain, const std::vector<char>& dirty, const RankReq& rk) {
   std::vector<AltRow> list;
   for (int g = 0, row = 0; g < gb[2]; ++g) {
-    if (!dirty[g]) alt_clear_group(gb, g, rk);
+    if (!dirty[g]) alt_clear(rk, group_rec(gb, g)[8], group_rec(gb, g)[9]);
     row += plan_alt_rows(gb, g, assign, row, dirty[g] ? nullptr : &list);
   }
-  return run_alternates(c, b, b->matrix.p, list, gb, assign, status, domain, rk);
+  return run_alternates(c, b, b->matrix.p, list, gb, nullptr, assign, status, domain, rk);
 }
 
 // Builds the plan IN PLACE in b->h_in (pinned); *plan_words = its size.  The GROUPS blob is
@@ -4010,8 +4054,23 @@ int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t*
 // than kLwScratchBytes of level-C domain scratch (12 bytes per domain) allow.
 constexpr size_t kLwScratchBytes = 64u << 20;
 
+// (wave, role) rows of a group's pod waves: what the ranked form may keep for it.
+size_t lw_role_rows(const int32_t* roles, int q, const int32_t* grp) {
+  size_t n = 0;
+  int w[RBGTOPO_MAX_STEP_ROLES][3];
+  for (int cr = 0, taken = 0, P; (P = lw_wave(roles, q, grp, cr, taken, w)) > 0;) {
+    n += (size_t)P;
+    cr = w[P - 1][0];
+    taken = w[P - 1][1] + w[P - 1][2];
+  }
+  return n;
+}
+
+// rk != nullptr: the ranked form (§3.12).  The matrix is overwritten by every wave, so each wave's rows are copied
+// out before the next wave scores (one copy per wave); once the placements are final one k_alternates launch ranks
+// the rows of every (wave, role) that placed a pod.
 int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
-                    int32_t* assign, int32_t* status, int32_t* domain) {
+                    int32_t* assign, int32_t* status, int32_t* domain, const RankReq* rk = nullptr) {
   long long total_pods = 0;
   int rc = lw_validate(c, gb, words, rp, rp_words, &total_pods);
   if (rc) return rc;
@@ -4020,6 +4079,8 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
   if (smem > kFastSmemMax) return fail(RBGTOPO_ELIMIT, "leader-worker placement: %d nodes exceed the room bitmap", T.n);
   const int ng = gb[2];
   std::vector<LwRun> runs(ng);
+  std::vector<AltRow> kept;  // rk: the (wave, role) rows that placed a pod, in b->lw_kept
+  size_t kept_cap = 0, kept_used = 0;
   long long pod_acc = 0;
   for (int g = 0, r0 = 0; g < ng; ++g) {
     LwRun& r = runs[g];
@@ -4039,6 +4100,7 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
     for (int i = 0; i < r.q; ++i) pod_acc += r.unplaced[i];
     r.anchors.assign(gb + r.rec[7], gb + r.rec[7] + 3LL * r.rec[6]);
     while (r.cur_role < r.q && r.roles[4 * r.cur_role + 1] == 0) ++r.cur_role;
+    if (rk) kept_cap += lw_role_rows(r.roles, r.q, r.rp);
   }
   for (long long k = 0; k < total_pods; ++k) assign[k] = -1;
   LwLevels lv{};
@@ -4048,6 +4110,13 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
   rc = acquire_batch(c, &b);
   if (rc) return rc;
   cudaStream_t s = stream_of(c, b);
+  if (rk) {
+    cudaError_t e = b->lw_kept.reserve(std::max<size_t>(1, kept_cap) * (size_t)c->slab_stride);
+    if (e != cudaSuccess) {
+      release_batch(c, b);
+      return fail(RBGTOPO_ECUDA, "rows of the ranked leader-worker placement: %s", cudaGetErrorString(e));
+    }
+  }
   rbgtopo_timing total{};
   std::vector<int32_t> blob, w_assign, w_status, w_domain, side;
   std::vector<int> active;
@@ -4137,6 +4206,15 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
       return RBGTOPO_OK;
     }();
     if (!rc) rc = fetch_batch(c, b, w_assign.data(), w_status.data(), w_domain.data());
+    const size_t slot0 = kept_used;  // this wave's rows in b->lw_kept, in matrix order
+    if (!rc && rk) {
+      const size_t stride = (size_t)c->slab_stride;
+      cudaError_t e = slot0 + rowacc <= kept_cap ? cudaMemcpyAsync(b->lw_kept.p + slot0 * stride, b->matrix.p,
+                                                                    (size_t)rowacc * stride * 4, cudaMemcpyDeviceToDevice, s)
+                                                 : cudaErrorInvalidValue;
+      if (e != cudaSuccess) rc = fail(RBGTOPO_ECUDA, "keeping the dense rows of a wave: %s", cudaGetErrorString(e));
+      kept_used += (size_t)rowacc;
+    }
     if (rc) break;
     {
       std::lock_guard<std::mutex> g(c->stat_mu);
@@ -4154,14 +4232,19 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
       for (int p = 0; p < r.P; ++p) {
         const int ri = r.w[p][0], S = r.rp[2 * ri];
         const long long first = r.pod0 + r.ord0[ri] + (long long)r.w[p][1] * S;
+        bool placed = false;
         for (int k = 0; k < r.w[p][2] * S; ++k, ++off) {
           const int node = w_assign[off];
           assign[first + k] = node;
           if (node < 0) continue;
-          any = true;
+          any = placed = true;
           r.anchors.push_back(node); r.anchors.push_back(ri); r.anchors.push_back(1);
           r.consumed[node] += r.roles[4 * ri + 2];
           r.unplaced[ri] -= 1;
+        }
+        if (rk && placed) {
+          const int row = blob[RBGTOPO_HDR_WORDS + (size_t)i * RBGTOPO_STEP_WORDS + 13] + p;  // in this wave's matrix
+          kept.push_back(AltRow{(int)slot0 + row, active[i], ri, (int)first, r.w[p][2] * S});
         }
       }
       if ((r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) && w_domain[i] >= 0 && any) r.fixed_domain = w_domain[i];
@@ -4194,6 +4277,11 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
     c->last = total;
   } else {
     cudaStreamSynchronize(s);
+  }
+  if (!rc && rk) {  // the placements are final now: rank the kept rows
+    alt_clear(*rk, 0, total_pods);
+    rc = run_alternates(c, b, b->lw_kept.p, kept, gb, rp, assign, status, domain, *rk);
+    if (rc) cudaStreamSynchronize(s);
   }
   release_batch(c, b);
   return rc;
@@ -4243,6 +4331,26 @@ int32_t rbgtopo_place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words
   if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
   CK(cudaSetDevice(c->cfg.device));
   return place_groups_lw(c, gb, words, role_pods, role_pods_words, assign, status, domain);
+}
+
+int32_t rbgtopo_place_groups_lw_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* role_pods,
+                                       int64_t role_pods_words, int32_t n_alt, int32_t* assign, int32_t* status,
+                                       int32_t* domain, float* score, int32_t* alt_node, float* alt_score) {
+  if (!c || !gb || !assign || !role_pods || !score || (n_alt > 0 && (!alt_node || !alt_score)))
+    return fail(RBGTOPO_EINVAL, "null argument");
+  if (n_alt < 0 || n_alt > RBGTOPO_MAX_ALTERNATES)
+    return fail(RBGTOPO_EINVAL, "n_alt %d outside [0, %d]", n_alt, RBGTOPO_MAX_ALTERNATES);
+  if (c->cfg.world > 1)
+    return fail(RBGTOPO_ELIMIT, "leader-worker placement needs world == 1: a rank holds only its slab of every dense row");
+  std::shared_lock<std::shared_mutex> lk(c->topo_mu);
+  if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
+  CK(cudaSetDevice(c->cfg.device));
+  const int64_t ng = words >= RBGTOPO_HDR_WORDS ? std::max<int64_t>(0, std::min<int64_t>(gb[2], words / RBGTOPO_GROUP_WORDS)) : 0;
+  std::vector<int32_t> own_status, own_domain;  // status / domain may be NULL: the ranking still needs them
+  if (!status) { own_status.resize((size_t)ng + 1); status = own_status.data(); }
+  if (!domain) { own_domain.resize((size_t)ng + 1); domain = own_domain.data(); }
+  const RankReq rk{n_alt, score, alt_node, alt_score};
+  return place_groups_lw(c, gb, words, role_pods, role_pods_words, assign, status, domain, &rk);
 }
 
 int32_t rbgtopo_plan_describe(const int32_t* gb, int64_t words, int32_t n_nodes, int32_t n_domains,

@@ -60,6 +60,7 @@ class TopoPlacer:
                           emit_matrix=1 if emit_matrix else 0, chunk_nodes=chunk_nodes, flags=flags)
         self.places_levels = bool(level_placement)
         self.places_committed_levels = bool(committed_levels)
+        self.places_lw_ranked = True   # place_groups_lw_ranked: alternates for leader-worker pods (DESIGN.md §3.12)
         h = C.c_void_p()
         self._h = None
         self._check(self.lib.rbgtopo_create(C.byref(cfg), C.byref(h)))
@@ -176,14 +177,10 @@ class TopoPlacer:
             _p(alt_node) if n_alt > 0 else None, _p(alt_score, _lib.f32p) if n_alt > 0 else None))
         return assign[:tp], status[:ng], domain[:ng], score[:tp], alt_node[:tp], alt_score[:tp]
 
-    def place_groups_lw(self, groups_blob: np.ndarray, role_pods) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
-        """Leader-worker replicas (DESIGN.md §3.11): role_pods holds (S, C) per role of every group in blob order —
-        S pods per replica, all inside one domain of co-location level C (-1: none).  Returns (assign per pod in
-        (group, role, ordinal, pod) order, status, domain)."""
-        gb = _i32(groups_blob)
-        rp = _i32(np.asarray(role_pods, dtype=np.int64).reshape(-1))
-        ng = int(gb[2])
-        pods = 0
+    @staticmethod
+    def _lw_pods(gb: np.ndarray, rp: np.ndarray) -> int:
+        """Pods of the assign vector (sum of pending * S); read defensively, the library validates."""
+        ng, pods = int(gb[2]), 0
         if len(rp) % 2 == 0 and len(gb) >= 8:
             S = rp[0::2].astype(np.int64)
             k = 0
@@ -196,12 +193,41 @@ class TopoPlacer:
                     break
                 pods += int((gb[role_off + 1:role_off + 4 * q:4].astype(np.int64) * np.maximum(S[k:k + q], 0)).sum())
                 k += q
+        return pods
+
+    def place_groups_lw(self, groups_blob: np.ndarray, role_pods) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """Leader-worker replicas (DESIGN.md §3.11): role_pods holds (S, C) per role of every group in blob order —
+        S pods per replica, all inside one domain of co-location level C (-1: none).  Returns (assign per pod in
+        (group, role, ordinal, pod) order, status, domain)."""
+        gb = _i32(groups_blob)
+        rp = _i32(np.asarray(role_pods, dtype=np.int64).reshape(-1))
+        ng, pods = int(gb[2]), self._lw_pods(gb, rp)
         assign = np.empty(max(pods, 1), dtype=np.int32)
         status = np.empty(max(ng, 1), dtype=np.int32)
         domain = np.empty(max(ng, 1), dtype=np.int32)
         self._check(self.lib.rbgtopo_place_groups_lw(self._h, _p(gb), len(gb), _p(rp), len(rp), _p(assign),
                                                      _p(status), _p(domain)))
         return assign[:pods], status[:ng], domain[:ng]
+
+    def place_groups_lw_ranked(self, groups_blob: np.ndarray, role_pods, n_alt: int):
+        """place_groups_lw plus ranked alternates per pod (DESIGN.md §3.12): returns (assign, status, domain,
+        score[P], alt_node[P, n_alt], alt_score[P, n_alt]).  assign / status / domain are those of place_groups_lw;
+        score[p] is pod p's dense-row score at its node, alt_node[p] the next-best nodes of its row that still have
+        room once its group is placed and that keep the replica in its co-location domain (-1 / -inf where there are
+        fewer), nothing for unplaced pods and gang-failed groups."""
+        gb = _i32(groups_blob)
+        rp = _i32(np.asarray(role_pods, dtype=np.int64).reshape(-1))
+        ng, pods = int(gb[2]), self._lw_pods(gb, rp)
+        assign = np.empty(max(pods, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        score = np.empty(max(pods, 1), dtype=np.float32)
+        alt_node = np.empty((max(pods, 1), max(n_alt, 0)), dtype=np.int32)
+        alt_score = np.empty((max(pods, 1), max(n_alt, 0)), dtype=np.float32)
+        self._check(self.lib.rbgtopo_place_groups_lw_ranked(
+            self._h, _p(gb), len(gb), _p(rp), len(rp), int(n_alt), _p(assign), _p(status), _p(domain),
+            _p(score, _lib.f32p), _p(alt_node) if n_alt > 0 else None, _p(alt_score, _lib.f32p) if n_alt > 0 else None))
+        return assign[:pods], status[:ng], domain[:ng], score[:pods], alt_node[:pods], alt_score[:pods]
 
     # -- staged (device-resident) batches
     def stage(self, blob: np.ndarray) -> int:

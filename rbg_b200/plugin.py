@@ -314,7 +314,10 @@ class B200TopoPodGroupManager:
         name, "{rbg}-{role}-{ordinal}-{k}" (k = 0 the leader); standalone roles keep "{rbg}-{role}-{ordinal}".  A
         role annotation COLOCATE_KEY names the topology key whose one domain must hold all pods of a replica; it
         resolves against exclusive_keys like an exclusive key (None: the level-0 label).  An unknown key, a level
-        the snapshot does not hold, a committed batch or alternates leave such a group without a hint and log why.
+        the snapshot does not hold or a committed batch leave such a group without a hint and log why.  With
+        alternates, such a group is placed through rbgtopo_place_groups_lw_ranked (§3.12) when the placer has
+        `places_lw_ranked`, and its alternates are keyed by pod name and stay inside each replica's co-location
+        domain; a placer without it gives no hint for such a group.
         False (default): those groups are placed as before, one pod per replica."""
         if not 0 <= alternates <= 8:
             raise ValueError(f"alternates must be in [0, 8], got {alternates}")
@@ -351,7 +354,7 @@ class B200TopoPodGroupManager:
             if not reason and self.is_leader_worker(r):
                 if committed:
                     reason = "leader-worker replicas: committed batches place one pod per replica"
-                elif self.alternates:
+                elif self.alternates and not getattr(self.placer, "places_lw_ranked", False):
                     reason = "leader-worker replicas: no ranked alternates for them"
                 else:
                     reason = self.role_pods(r)[1]
@@ -440,8 +443,13 @@ class B200TopoPodGroupManager:
             blob, runs = self.groups_blob([rbgs[i] for i in lw])
             pods = [self.role_pods(g.rbg)[0] for g in runs]
             role_pods = [pods[k][ri] for k, g in enumerate(runs) for ri in g.order]
-            assign, status, domain = self.placer.place_groups_lw(blob, role_pods)
-            for i, p in zip(lw, self._placements(runs, assign, status, domain, None, pods)):
+            alt_node = None
+            if self.alternates > 0:
+                assign, status, domain, _, alt_node, _ = self.placer.place_groups_lw_ranked(blob, role_pods,
+                                                                                           self.alternates)
+            else:
+                assign, status, domain = self.placer.place_groups_lw(blob, role_pods)
+            for i, p in zip(lw, self._placements(runs, assign, status, domain, alt_node, pods)):
                 done[i] = p
         return self._merge(all_rbgs, done, skipped)
 
