@@ -89,6 +89,14 @@ static int32_t rbgtopo_go_place_groups_lw(rbgtopo_ctx* ctx, const int32_t* group
   rbgtopo_go_err(ctx, rc, err);
   return rc;
 }
+static int32_t rbgtopo_go_place_groups_lw_committed(rbgtopo_ctx* ctx, const int32_t* groups, int64_t words,
+                                                    const int32_t* role_pods, int64_t role_pods_words, int32_t* assign,
+                                                    int32_t* status, int32_t* domain, int32_t* rounds, char* err) {
+  int32_t rc = rbgtopo_place_groups_lw_committed(ctx, groups, words, role_pods, role_pods_words, assign, status, domain,
+                                                 rounds);
+  rbgtopo_go_err(ctx, rc, err);
+  return rc;
+}
 static int32_t rbgtopo_go_place_groups_lw_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t words,
                                                  const int32_t* role_pods, int64_t role_pods_words, int32_t n_alt,
                                                  int32_t* assign, int32_t* status, int32_t* domain, float* score,
@@ -273,6 +281,23 @@ func (p *placer) placeGroupsLW(blob, rolePods []int32, nPods int) (assign, statu
 		return nil, nil, nil, err
 	}
 	return assign[:nPods], status[:nGroups], domain[:nGroups], nil
+}
+
+// placeGroupsLWCommitted: placeGroupsLW as a committed batch (DESIGN.md §3.13): the groups in blob order, each seeing
+// the pods and exclusive domains the groups before it took; rounds = wave-loop rounds the library ran.
+func (p *placer) placeGroupsLWCommitted(blob, rolePods []int32, nPods int) (assign, status, domain []int32, rounds int32, err error) {
+	nGroups := int(blob[2])
+	assign = make([]int32, max(nPods, 1))
+	status = make([]int32, max(nGroups, 1))
+	domain = make([]int32, max(nGroups, 1))
+	var r C.int32_t
+	var buf [C.RBGTOPO_GO_ERRLEN]C.char
+	rc := C.rbgtopo_go_place_groups_lw_committed(p.ctx, p32(blob), C.int64_t(len(blob)), p32(rolePods),
+		C.int64_t(len(rolePods)), p32(assign), p32(status), p32(domain), &r, &buf[0])
+	if err = mkErr(rc, &buf); err != nil {
+		return nil, nil, nil, 0, err
+	}
+	return assign[:nPods], status[:nGroups], domain[:nGroups], int32(r), nil
 }
 
 // placeGroupsLWRanked: placeGroupsLW plus, per pod, up to nAlt next-best nodes that still have room once its group is

@@ -390,6 +390,21 @@ int32_t rbgtopo_place_groups_lw_ranked(rbgtopo_ctx* ctx, const int32_t* groups, 
                                        int32_t* assign, int32_t* status, int32_t* domain, float* score,
                                        int32_t* alt_node, float* alt_score);
 
+/* Committed leader-worker batch (DESIGN.md §3.13): rbgtopo_place_groups_lw's inputs, validation, exactness bound,
+ * error codes and outputs, with the groups placed in blob order as rbgtopo_place_groups_committed places them.
+ * Group g is placed exactly as a one-group rbgtopo_place_groups_lw call would place it, except that
+ *   - every pod an earlier group placed consumes (node, demand) for g (feasibility only: base, order and scores
+ *     stay the snapshot's); a gang-failed group consumes nothing;
+ *   - an earlier exclusive group with status != 2 that reports domain D makes D owned by its gid (the last such
+ *     group wins); in occupancy mode node n of D shows owner_0[n] (+) gid instead.
+ * Over the batch no node receives more than free[n].  With S = 1 and C = -1 everywhere the results are
+ * bit-identical to rbgtopo_place_groups_committed's.  *rounds (may be NULL) = wave-loop rounds run: at most
+ * n_groups, 1 for one group.  Limits (RBGTOPO_ELIMIT): a group whose own exclusive level is >= 1, a ctx with
+ * world > 1, more nodes than the room bitmap of rbgtopo_place_groups_lw holds.  No alternates. */
+int32_t rbgtopo_place_groups_lw_committed(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                          const int32_t* role_pods, int64_t role_pods_words, int32_t* assign,
+                                          int32_t* status, int32_t* domain, int32_t* rounds);
+
 /* rbgtopo_place_groups pipeline, staged: the groups are compiled into a
  * device-resident multi-wave plan (one step blob, wave-major, expanded on the
  * device), so rbgtopo_run_staged runs ONE score launch for the dense rows of every

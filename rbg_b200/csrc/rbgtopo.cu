@@ -874,13 +874,19 @@ int launch_emit_plan(rbgtopo_ctx* c, Batch* b, cudaStream_t s, long long n_rows,
   return RBGTOPO_OK;
 }
 
-int launch_score(rbgtopo_ctx* c, Batch* b, cudaStream_t s) {
+// claim_off != nullptr (step batches of rbgtopo_place_groups_lw_committed only): k_score_emit_claims with the owner
+// claims of earlier groups per step (score.cuh).
+int launch_score(rbgtopo_ctx* c, Batch* b, cudaStream_t s, const int* claim_off = nullptr,
+                 const int2* claim_rec = nullptr) {
   const BatchMeta& m = b->m;
   if (m.n_steps == 0) return RBGTOPO_OK;
   if (!b->wave_begin.empty()) return launch_emit_plan(c, b, s, m.total_p);  // multi-wave plan: background rows from the row table
   const int items = (int)emit_items(m.n_steps, c->lc);
   const int grid = items / kEmitBlockSteps;  // one CTA per (block of steps, chunk of nodes)
-  k_score_emit<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items);  // step batch: rows + sparse corrections
+  if (claim_off)
+    k_score_emit_claims<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items, claim_off, claim_rec, c->topo.occ);
+  else
+    k_score_emit<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items);  // step batch: rows + sparse corrections
   return RBGTOPO_OK;
 }
 
@@ -3943,7 +3949,8 @@ struct LwRun {  // one group while its pod waves are placed
   int ord0[RBGTOPO_MAX_GROUP_ROLES] = {0};      // first pod of every role inside the group's range
   int unplaced[RBGTOPO_MAX_GROUP_ROLES] = {0};  // pods
   std::vector<int32_t> anchors;     // (node, role, count)*
-  std::map<int, int> consumed;      // node -> amount
+  std::map<int, int> consumed;      // node -> amount (committed: earlier groups' claims included)
+  std::vector<int32_t> owner_claims;  // committed, exclusive group: (node, claim gid)* of claimed domains, by node
   int w[RBGTOPO_MAX_STEP_ROLES][3];
   int P = 0;
   bool done() const { return failed || cur_role >= q; }
@@ -4066,43 +4073,80 @@ size_t lw_role_rows(const int32_t* roles, int q, const int32_t* grp) {
   return n;
 }
 
+// What a group of a committed leader-worker batch takes from the groups after it (§3.13): (node, demand) of its placed
+// pods, aggregated by node, and the exclusive domain it reports (-1 = none).  A gang-failed group takes nothing.
+struct LwClaims {
+  std::vector<std::pair<int, int>> cap;
+  int dom = -1, gid = -1;
+  bool operator==(const LwClaims& o) const { return cap == o.cap && dom == o.dom && gid == o.gid; }
+};
+
 // rk != nullptr: the ranked form (§3.12).  The matrix is overwritten by every wave, so each wave's rows are copied
 // out before the next wave scores (one copy per wave); once the placements are final one k_alternates launch ranks
 // the rows of every (wave, role) that placed a pod.
+// rounds != nullptr: the committed form (§3.13).  A round runs the wave loop for groups [lo, ng); group g sees the
+// claims of groups < g as the previous round left them (final below lo).  c = the lowest group whose claims changed:
+// groups <= c saw their final input, the next round starts at c + 1, and a round that changes nothing ends the call.
 int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
-                    int32_t* assign, int32_t* status, int32_t* domain, const RankReq* rk = nullptr) {
+                    int32_t* assign, int32_t* status, int32_t* domain, const RankReq* rk = nullptr,
+                    int32_t* rounds = nullptr) {
   long long total_pods = 0;
   int rc = lw_validate(c, gb, words, rp, rp_words, &total_pods);
   if (rc) return rc;
   const Topology& T = c->topo;
+  const int ng = gb[2];
+  if (rounds)
+    for (int g = 0; g < ng; ++g)
+      if (group_rec(gb, g)[10] > 0)
+        return fail(RBGTOPO_ELIMIT, "committed leader-worker batch: group %d is exclusive at level %d; only level 0 is "
+                                    "committed (levels >= 1: rbgtopo_place_groups_committed)", g, group_rec(gb, g)[10]);
   const size_t smem = (size_t)((T.n + 31) / 32) * 4;
   if (smem > kFastSmemMax) return fail(RBGTOPO_ELIMIT, "leader-worker placement: %d nodes exceed the room bitmap", T.n);
-  const int ng = gb[2];
   std::vector<LwRun> runs(ng);
-  std::vector<AltRow> kept;  // rk: the (wave, role) rows that placed a pod, in b->lw_kept
-  size_t kept_cap = 0, kept_used = 0;
-  long long pod_acc = 0;
-  for (int g = 0, r0 = 0; g < ng; ++g) {
+  std::vector<int> rp0(ng + 1, 0);
+  std::vector<long long> pod0(ng + 1, 0);
+  for (int g = 0; g < ng; ++g) {
+    const int32_t* rec = group_rec(gb, g);
+    rp0[g + 1] = rp0[g] + rec[3];
+    long long pods = 0;
+    for (int i = 0; i < rec[3]; ++i) pods += (long long)gb[rec[4] + 4 * i + 1] * rp[2LL * (rp0[g] + i)];
+    pod0[g + 1] = pod0[g] + pods;
+  }
+  auto init_run = [&](int g) {
     LwRun& r = runs[g];
+    r = LwRun();
     r.rec = group_rec(gb, g);
     r.q = r.rec[3];
     r.roles = gb + r.rec[4];
     r.pair = gb + r.rec[5];
-    r.rp = rp + 2LL * r0;
-    r0 += r.q;
+    r.rp = rp + 2LL * rp0[g];
     r.fixed_domain = r.rec[2];
-    r.pod0 = pod_acc;
+    r.pod0 = pod0[g];
     for (int i = 0, acc = 0; i < r.q; ++i) {
       r.ord0[i] = acc;
       r.unplaced[i] = r.roles[4 * i + 1] * r.rp[2 * i];
       acc += r.unplaced[i];
     }
-    for (int i = 0; i < r.q; ++i) pod_acc += r.unplaced[i];
     r.anchors.assign(gb + r.rec[7], gb + r.rec[7] + 3LL * r.rec[6]);
     while (r.cur_role < r.q && r.roles[4 * r.cur_role + 1] == 0) ++r.cur_role;
-    if (rk) kept_cap += lw_role_rows(r.roles, r.q, r.rp);
+    for (long long k = pod0[g]; k < pod0[g + 1]; ++k) assign[k] = -1;
+  };
+  std::vector<AltRow> kept;  // rk: the (wave, role) rows that placed a pod, in b->lw_kept
+  size_t kept_cap = 0, kept_used = 0;
+  for (int g = 0; g < ng; ++g) {
+    init_run(g);
+    if (rk) kept_cap += lw_role_rows(runs[g].roles, runs[g].q, runs[g].rp);
   }
-  for (long long k = 0; k < total_pods; ++k) assign[k] = -1;
+  std::vector<LwClaims> claims(rounds ? ng : 0);  // committed: every group's claims as the latest round left them
+  std::vector<int> dom_ptr, dom_nodes;             // committed: the nodes of every level-0 domain
+  if (rounds) {
+    dom_ptr.assign((size_t)T.n_domains + 1, 0);
+    for (int n = 0; n < T.n; ++n) ++dom_ptr[T.h_domain[n] + 1];
+    for (int d = 0; d < T.n_domains; ++d) dom_ptr[d + 1] += dom_ptr[d];
+    dom_nodes.resize(T.n);
+    std::vector<int> fill(dom_ptr.begin(), dom_ptr.end() - 1);
+    for (int n = 0; n < T.n; ++n) dom_nodes[fill[T.h_domain[n]]++] = n;
+  }
   LwLevels lv{};
   for (int L = 0; L <= installed_levels(c); ++L) lv.nd[L] = level_domains(T, L);
 
@@ -4120,150 +4164,185 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
   rbgtopo_timing total{};
   std::vector<int32_t> blob, w_assign, w_status, w_domain, side;
   std::vector<int> active;
-  while (true) {
-    active.clear();
-    for (int g = 0; g < ng; ++g)
-      if (!runs[g].done()) active.push_back(g);
-    if (active.empty()) break;
-    // ---- this wave's step blob: role counts in pods, need over unplaced pods
-    const int ns = (int)active.size();
-    blob.assign((size_t)RBGTOPO_HDR_WORDS + (size_t)ns * RBGTOPO_STEP_WORDS, 0);
-    side.assign((size_t)ns * MAXP, 0);
-    int racc = 0, rowacc = 0, dmax = 0;
-    for (int i = 0; i < ns; ++i) {
-      LwRun& r = runs[active[i]];
-      r.P = lw_wave(r.roles, r.q, r.rp, r.cur_role, r.cur_taken, r.w);
-      int32_t st[RBGTOPO_STEP_WORDS] = {0};
-      st[0] = r.rec[0];
-      st[1] = r.rec[1] & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG);
-      st[2] = (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) ? r.fixed_domain : -1;
-      st[3] = r.P;
-      while (blob.size() & 3) blob.push_back(0);  // role records are read as 16-byte vectors
-      st[4] = (int32_t)blob.size();
-      int n = 0;
-      for (int p = 0; p < r.P; ++p) {
-        const int ri = r.w[p][0], S = r.rp[2 * ri], C = r.rp[2 * ri + 1];
-        int need = 0;
-        for (int q = 0; q < r.q; ++q)
-          if (r.pair[ri * r.q + q] > 0) need += r.unplaced[q];
-        blob.push_back(r.w[p][2] * S);
-        blob.push_back(r.roles[4 * ri + 2]);
-        blob.push_back(std::min(need, RBGTOPO_NEED_CAP));
-        blob.push_back(r.roles[4 * ri + 3] & RBGTOPO_ROLE_EXCLUSIVE);
-        side[(size_t)i * MAXP + p] = lw_pack_role(S, C);
-        if (C >= 0) dmax = std::max(dmax, lv.nd[C]);
-        n += r.w[p][2] * S;
-      }
-      st[5] = r.q;
-      st[6] = (int32_t)blob.size();
-      for (int p = 0; p < r.P; ++p) blob.insert(blob.end(), r.pair + r.w[p][0] * r.q, r.pair + (r.w[p][0] + 1) * r.q);
-      st[7] = (int32_t)(r.anchors.size() / 3);
-      st[8] = (int32_t)blob.size();
-      blob.insert(blob.end(), r.anchors.begin(), r.anchors.end());
-      st[9] = (int32_t)r.consumed.size();
-      st[10] = (int32_t)blob.size();
-      for (const auto& kv : r.consumed) { blob.push_back(kv.first); blob.push_back(kv.second); }  // by node, one per node
-      st[11] = n;
-      st[12] = racc;
-      st[13] = rowacc;
-      st[14] = r.rec[10];  // exclusive level
-      racc += n;
-      rowacc += r.P;
-      memcpy(blob.data() + RBGTOPO_HDR_WORDS + (size_t)i * RBGTOPO_STEP_WORDS, st, sizeof st);
-    }
-    blob[0] = RBGTOPO_BLOB_MAGIC;
-    blob[1] = RBGTOPO_ABI_VERSION;
-    blob[2] = ns;
-    blob[3] = (int32_t)blob.size();
-    blob[4] = racc;
-    blob[5] = rowacc;
-    w_assign.resize(racc);
-    w_status.resize(ns);
-    w_domain.resize(ns);
-    rc = stage_into(c, b, blob.data(), (int64_t)blob.size());
-    if (rc) break;
-    rc = [&]() -> int {
-      // grid: every step resident at once if the device holds them, the level-C scratch bounded by kLwScratchBytes
-      int per_sm = 0;
-      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_lw_assign, LW_THREADS, smem));
-      long long grid = std::min<long long>(ns, (long long)std::max(1, per_sm) * c->sm_count);
-      if (dmax > 0) grid = std::min<long long>(grid, std::max<long long>(1, kLwScratchBytes / (12LL * dmax)));
-      CK(b->lw.reserve(side.size()));
-      CK(b->h_lw.reserve(side.size()));
-      CK(b->lw_best.reserve((size_t)grid * dmax + 1));
-      CK(b->lw_cap.reserve((size_t)grid * dmax + 1));
-      memcpy(b->h_lw.p, side.data(), side.size() * 4);
-      CK(cudaMemcpyAsync(b->lw.p, b->h_lw.p, side.size() * 4, cudaMemcpyHostToDevice, s));
-      CK(cudaStreamWaitEvent(s, c->base_ready, 0));  // a pending snapshot refresh
-      CK(cudaStreamWaitEvent(s, c->topo_ready, 0));
-      int r2 = launch_score(c, b, s);
-      if (r2) return r2;
-      k_lw_assign<<<(unsigned)grid, LW_THREADS, smem, s>>>(topo_dev(c), batch_dev(c, b), b->lw.p, b->lw_best.p,
-                                                           b->lw_cap.p, dmax, lv);
-      CK(cudaGetLastError());
-      b->pend_launches += 2;
-      b->ran = true;
-      return RBGTOPO_OK;
-    }();
-    if (!rc) rc = fetch_batch(c, b, w_assign.data(), w_status.data(), w_domain.data());
-    const size_t slot0 = kept_used;  // this wave's rows in b->lw_kept, in matrix order
-    if (!rc && rk) {
-      const size_t stride = (size_t)c->slab_stride;
-      cudaError_t e = slot0 + rowacc <= kept_cap ? cudaMemcpyAsync(b->lw_kept.p + slot0 * stride, b->matrix.p,
-                                                                    (size_t)rowacc * stride * 4, cudaMemcpyDeviceToDevice, s)
-                                                 : cudaErrorInvalidValue;
-      if (e != cudaSuccess) rc = fail(RBGTOPO_ECUDA, "keeping the dense rows of a wave: %s", cudaGetErrorString(e));
-      kept_used += (size_t)rowacc;
-    }
-    if (rc) break;
-    {
-      std::lock_guard<std::mutex> g(c->stat_mu);
-      c->launches += 2;
-      total.h2d_ms += c->last.h2d_ms; total.d2h_ms += c->last.d2h_ms;
-      total.total_ms += c->last.total_ms; total.launches += c->last.launches;
-      total.scores += c->last.scores; total.algo_bytes += c->last.algo_bytes;
-      total.h2d_words += c->last.h2d_words;
-    }
-    // ---- absorb the placements: every pod placed is an anchor (node, role, 1) and consumes (node, demand)
-    int off = 0;
-    for (int i = 0; i < ns; ++i) {
-      LwRun& r = runs[active[i]];
-      bool any = false;
-      for (int p = 0; p < r.P; ++p) {
-        const int ri = r.w[p][0], S = r.rp[2 * ri];
-        const long long first = r.pod0 + r.ord0[ri] + (long long)r.w[p][1] * S;
-        bool placed = false;
-        for (int k = 0; k < r.w[p][2] * S; ++k, ++off) {
-          const int node = w_assign[off];
-          assign[first + k] = node;
-          if (node < 0) continue;
-          any = placed = true;
-          r.anchors.push_back(node); r.anchors.push_back(ri); r.anchors.push_back(1);
-          r.consumed[node] += r.roles[4 * ri + 2];
-          r.unplaced[ri] -= 1;
+  std::vector<std::pair<int, int>> oc;
+  int lo = 0, n_rounds = 0;  // committed: the round's first group, rounds run
+  for (bool more = true; more;) {
+    more = false;
+    if (rounds) {  // every group of the round starts from the claims of the groups before it
+      std::map<int, int> cap, own;  // node -> capacity taken; level-0 domain -> gid of its last reporter
+      for (int g = 0; g < ng; ++g) {
+        if (g >= lo) {
+          LwRun& r = runs[g];
+          if (n_rounds > 0) init_run(g);
+          r.consumed = cap;
+          if (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) {
+            oc.clear();
+            for (const auto& [d, gid] : own)
+              for (int k = dom_ptr[d]; k < dom_ptr[d + 1]; ++k) oc.emplace_back(dom_nodes[k], gid);
+            std::sort(oc.begin(), oc.end());
+            for (const auto& [n, gid] : oc) { r.owner_claims.push_back(n); r.owner_claims.push_back(gid); }
+          }
         }
-        if (rk && placed) {
-          const int row = blob[RBGTOPO_HDR_WORDS + (size_t)i * RBGTOPO_STEP_WORDS + 13] + p;  // in this wave's matrix
-          kept.push_back(AltRow{(int)slot0 + row, active[i], ri, (int)first, r.w[p][2] * S});
-        }
+        for (const auto& [n, a] : claims[g].cap) cap[n] += a;
+        if (claims[g].dom >= 0) own[claims[g].dom] = claims[g].gid;
       }
-      if ((r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) && w_domain[i] >= 0 && any) r.fixed_domain = w_domain[i];
-      r.status = std::max(r.status, w_status[i]);
-      if ((r.rec[1] & RBGTOPO_STEP_GANG) && w_status[i] != RBGTOPO_PLACED_ALL) r.failed = true;
-      r.cur_role = r.w[r.P - 1][0];
-      r.cur_taken = r.w[r.P - 1][1] + r.w[r.P - 1][2];
-      if (r.cur_taken >= r.roles[4 * r.cur_role + 1]) { ++r.cur_role; r.cur_taken = 0; }
-      while (r.cur_role < r.q && r.roles[4 * r.cur_role + 1] == 0) ++r.cur_role;
     }
-  }
-  if (!rc) {
-    for (int g = 0; g < ng; ++g) {
+    while (true) {
+      active.clear();
+      for (int g = lo; g < ng; ++g)
+        if (!runs[g].done()) active.push_back(g);
+      if (active.empty()) break;
+      // ---- this wave's step blob: role counts in pods, need over unplaced pods
+      const int ns = (int)active.size();
+      blob.assign((size_t)RBGTOPO_HDR_WORDS + (size_t)ns * RBGTOPO_STEP_WORDS, 0);
+      side.assign((size_t)ns * MAXP, 0);
+      int racc = 0, rowacc = 0, dmax = 0;
+      for (int i = 0; i < ns; ++i) {
+        LwRun& r = runs[active[i]];
+        r.P = lw_wave(r.roles, r.q, r.rp, r.cur_role, r.cur_taken, r.w);
+        int32_t st[RBGTOPO_STEP_WORDS] = {0};
+        st[0] = r.rec[0];
+        st[1] = r.rec[1] & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG);
+        st[2] = (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) ? r.fixed_domain : -1;
+        st[3] = r.P;
+        while (blob.size() & 3) blob.push_back(0);  // role records are read as 16-byte vectors
+        st[4] = (int32_t)blob.size();
+        int n = 0;
+        for (int p = 0; p < r.P; ++p) {
+          const int ri = r.w[p][0], S = r.rp[2 * ri], C = r.rp[2 * ri + 1];
+          int need = 0;
+          for (int q = 0; q < r.q; ++q)
+            if (r.pair[ri * r.q + q] > 0) need += r.unplaced[q];
+          blob.push_back(r.w[p][2] * S);
+          blob.push_back(r.roles[4 * ri + 2]);
+          blob.push_back(std::min(need, RBGTOPO_NEED_CAP));
+          blob.push_back(r.roles[4 * ri + 3] & RBGTOPO_ROLE_EXCLUSIVE);
+          side[(size_t)i * MAXP + p] = lw_pack_role(S, C);
+          if (C >= 0) dmax = std::max(dmax, lv.nd[C]);
+          n += r.w[p][2] * S;
+        }
+        st[5] = r.q;
+        st[6] = (int32_t)blob.size();
+        for (int p = 0; p < r.P; ++p) blob.insert(blob.end(), r.pair + r.w[p][0] * r.q, r.pair + (r.w[p][0] + 1) * r.q);
+        st[7] = (int32_t)(r.anchors.size() / 3);
+        st[8] = (int32_t)blob.size();
+        blob.insert(blob.end(), r.anchors.begin(), r.anchors.end());
+        st[9] = (int32_t)r.consumed.size();
+        st[10] = (int32_t)blob.size();
+        // by node, one per node.  Only a committed round whose group is re-run later can see claims summing past
+        // free[n] (stale claims of earlier groups), so clamping them to RBGTOPO_MAX_FREE changes no kept result
+        for (const auto& kv : r.consumed) { blob.push_back(kv.first); blob.push_back(std::min(kv.second, RBGTOPO_MAX_FREE)); }
+        st[11] = n;
+        st[12] = racc;
+        st[13] = rowacc;
+        st[14] = r.rec[10];  // exclusive level
+        racc += n;
+        rowacc += r.P;
+        memcpy(blob.data() + RBGTOPO_HDR_WORDS + (size_t)i * RBGTOPO_STEP_WORDS, st, sizeof st);
+      }
+      blob[0] = RBGTOPO_BLOB_MAGIC;
+      blob[1] = RBGTOPO_ABI_VERSION;
+      blob[2] = ns;
+      blob[3] = (int32_t)blob.size();
+      blob[4] = racc;
+      blob[5] = rowacc;
+      // committed: per step the offsets of its owner claims, then the (node, gid) records, 8-byte aligned
+      size_t claim_at = 0, rec_at = 0;
+      if (rounds) {
+        claim_at = side.size();
+        int acc = 0;
+        side.push_back(0);
+        for (int i = 0; i < ns; ++i) side.push_back(acc += (int)runs[active[i]].owner_claims.size() / 2);
+        if (side.size() & 1) side.push_back(0);
+        rec_at = side.size();
+        for (int i = 0; i < ns; ++i) side.insert(side.end(), runs[active[i]].owner_claims.begin(), runs[active[i]].owner_claims.end());
+      }
+      w_assign.resize(racc);
+      w_status.resize(ns);
+      w_domain.resize(ns);
+      rc = stage_into(c, b, blob.data(), (int64_t)blob.size());
+      if (rc) break;
+      rc = [&]() -> int {
+        // grid: every step resident at once if the device holds them, the level-C scratch bounded by kLwScratchBytes
+        int per_sm = 0;
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_lw_assign, LW_THREADS, smem));
+        long long grid = std::min<long long>(ns, (long long)std::max(1, per_sm) * c->sm_count);
+        if (dmax > 0) grid = std::min<long long>(grid, std::max<long long>(1, kLwScratchBytes / (12LL * dmax)));
+        CK(b->lw.reserve(side.size()));
+        CK(b->h_lw.reserve(side.size()));
+        CK(b->lw_best.reserve((size_t)grid * dmax + 1));
+        CK(b->lw_cap.reserve((size_t)grid * dmax + 1));
+        memcpy(b->h_lw.p, side.data(), side.size() * 4);
+        CK(cudaMemcpyAsync(b->lw.p, b->h_lw.p, side.size() * 4, cudaMemcpyHostToDevice, s));
+        CK(cudaStreamWaitEvent(s, c->base_ready, 0));  // a pending snapshot refresh
+        CK(cudaStreamWaitEvent(s, c->topo_ready, 0));
+        int r2 = rounds ? launch_score(c, b, s, b->lw.p + claim_at, reinterpret_cast<const int2*>(b->lw.p + rec_at))
+                        : launch_score(c, b, s);
+        if (r2) return r2;
+        k_lw_assign<<<(unsigned)grid, LW_THREADS, smem, s>>>(topo_dev(c), batch_dev(c, b), b->lw.p, b->lw_best.p,
+                                                             b->lw_cap.p, dmax, lv);
+        CK(cudaGetLastError());
+        b->pend_launches += 2;
+        b->ran = true;
+        return RBGTOPO_OK;
+      }();
+      if (!rc) rc = fetch_batch(c, b, w_assign.data(), w_status.data(), w_domain.data());
+      const size_t slot0 = kept_used;  // this wave's rows in b->lw_kept, in matrix order
+      if (!rc && rk) {
+        const size_t stride = (size_t)c->slab_stride;
+        cudaError_t e = slot0 + rowacc <= kept_cap ? cudaMemcpyAsync(b->lw_kept.p + slot0 * stride, b->matrix.p,
+                                                                      (size_t)rowacc * stride * 4, cudaMemcpyDeviceToDevice, s)
+                                                   : cudaErrorInvalidValue;
+        if (e != cudaSuccess) rc = fail(RBGTOPO_ECUDA, "keeping the dense rows of a wave: %s", cudaGetErrorString(e));
+        kept_used += (size_t)rowacc;
+      }
+      if (rc) break;
+      {
+        std::lock_guard<std::mutex> g(c->stat_mu);
+        c->launches += 2;
+        total.h2d_ms += c->last.h2d_ms; total.d2h_ms += c->last.d2h_ms;
+        total.total_ms += c->last.total_ms; total.launches += c->last.launches;
+        total.scores += c->last.scores; total.algo_bytes += c->last.algo_bytes;
+        total.h2d_words += c->last.h2d_words;
+      }
+      // ---- absorb the placements: every pod placed is an anchor (node, role, 1) and consumes (node, demand)
+      int off = 0;
+      for (int i = 0; i < ns; ++i) {
+        LwRun& r = runs[active[i]];
+        bool any = false;
+        for (int p = 0; p < r.P; ++p) {
+          const int ri = r.w[p][0], S = r.rp[2 * ri];
+          const long long first = r.pod0 + r.ord0[ri] + (long long)r.w[p][1] * S;
+          bool placed = false;
+          for (int k = 0; k < r.w[p][2] * S; ++k, ++off) {
+            const int node = w_assign[off];
+            assign[first + k] = node;
+            if (node < 0) continue;
+            any = placed = true;
+            r.anchors.push_back(node); r.anchors.push_back(ri); r.anchors.push_back(1);
+            r.consumed[node] += r.roles[4 * ri + 2];
+            r.unplaced[ri] -= 1;
+          }
+          if (rk && placed) {
+            const int row = blob[RBGTOPO_HDR_WORDS + (size_t)i * RBGTOPO_STEP_WORDS + 13] + p;  // in this wave's matrix
+            kept.push_back(AltRow{(int)slot0 + row, active[i], ri, (int)first, r.w[p][2] * S});
+          }
+        }
+        if ((r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) && w_domain[i] >= 0 && any) r.fixed_domain = w_domain[i];
+        r.status = std::max(r.status, w_status[i]);
+        if ((r.rec[1] & RBGTOPO_STEP_GANG) && w_status[i] != RBGTOPO_PLACED_ALL) r.failed = true;
+        r.cur_role = r.w[r.P - 1][0];
+        r.cur_taken = r.w[r.P - 1][1] + r.w[r.P - 1][2];
+        if (r.cur_taken >= r.roles[4 * r.cur_role + 1]) { ++r.cur_role; r.cur_taken = 0; }
+        while (r.cur_role < r.q && r.roles[4 * r.cur_role + 1] == 0) ++r.cur_role;
+      }
+    }
+    if (rc) break;
+    for (int g = lo; g < ng; ++g) {
       const LwRun& r = runs[g];
       const bool excl = (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) != 0;
       if (r.failed) {  // gang: nothing of the group is placed
-        long long pods = 0;
-        for (int i = 0; i < r.q; ++i) pods += (long long)r.roles[4 * i + 1] * r.rp[2 * i];
-        for (long long k = 0; k < pods; ++k) assign[r.pod0 + k] = -1;
+        for (long long k = pod0[g]; k < pod0[g + 1]; ++k) assign[k] = -1;
         if (status) status[g] = RBGTOPO_GANG_FAILED;
         if (domain) domain[g] = -1;
       } else {
@@ -4271,6 +4350,34 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
         if (domain) domain[g] = excl ? r.fixed_domain : -1;
       }
     }
+    if (rounds) {
+      ++n_rounds;
+      int cmin = -1;  // the lowest group whose claims differ from what the groups after it saw
+      for (int g = lo; g < ng; ++g) {
+        const LwRun& r = runs[g];
+        LwClaims nc;
+        if (!r.failed) {
+          std::map<int, int> cap;
+          for (int i = 0; i < r.q; ++i)
+            for (long long k = 0; k < (long long)r.roles[4 * i + 1] * r.rp[2 * i]; ++k)
+              if (const int node = assign[r.pod0 + r.ord0[i] + k]; node >= 0) cap[node] += r.roles[4 * i + 2];
+          nc.cap.assign(cap.begin(), cap.end());
+          if ((r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) && r.fixed_domain >= 0) {
+            nc.dom = r.fixed_domain;
+            nc.gid = r.rec[0];
+          }
+        }
+        if (cmin < 0 && !(nc == claims[g])) cmin = g;
+        claims[g] = std::move(nc);
+      }
+      if (cmin >= 0 && cmin + 1 < ng) {
+        lo = cmin + 1;
+        more = true;
+      }
+    }
+  }
+  if (rounds) *rounds = n_rounds;
+  if (!rc) {
     harvest_base_ms(c);
     std::lock_guard<std::mutex> g(c->stat_mu);
     total.base_ms = c->topo.base_ms;
@@ -4351,6 +4458,22 @@ int32_t rbgtopo_place_groups_lw_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_
   if (!domain) { own_domain.resize((size_t)ng + 1); domain = own_domain.data(); }
   const RankReq rk{n_alt, score, alt_node, alt_score};
   return place_groups_lw(c, gb, words, role_pods, role_pods_words, assign, status, domain, &rk);
+}
+
+int32_t rbgtopo_place_groups_lw_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* role_pods,
+                                          int64_t role_pods_words, int32_t* assign, int32_t* status, int32_t* domain,
+                                          int32_t* rounds) {
+  if (rounds) *rounds = 0;
+  if (!c || !gb || !assign || !role_pods) return fail(RBGTOPO_EINVAL, "null argument");
+  if (c->cfg.world > 1)
+    return fail(RBGTOPO_ELIMIT, "committed leader-worker placement needs world == 1: a rank holds only its slab of every dense row");
+  std::shared_lock<std::shared_mutex> lk(c->topo_mu);  // one snapshot for every round
+  if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
+  CK(cudaSetDevice(c->cfg.device));
+  int32_t r = 0;
+  const int rc = place_groups_lw(c, gb, words, role_pods, role_pods_words, assign, status, domain, nullptr, &r);
+  if (rounds) *rounds = r;
+  return rc;
 }
 
 int32_t rbgtopo_plan_describe(const int32_t* gb, int64_t words, int32_t n_nodes, int32_t n_domains,

@@ -39,8 +39,15 @@ __device__ __forceinline__ void red_add_f32(float* p, float v) {
 // tail fix-up and header decode per store); here they are amortised over the block's steps.
 constexpr int EMIT_MAX_BLOCK = 16;  // upper bound of b.bsteps
 
-__global__ void __launch_bounds__(SCORE_THREADS, 6)
-k_score_emit(TopoDev t, BatchDev b, int items) {
+// CLAIMS (k_score_emit_claims, rbgtopo_place_groups_lw_committed, DESIGN.md §3.13): exclusive domains earlier groups of a
+// committed batch reported.  Per step, claim_rec[claim_off[step] .. claim_off[step + 1]) = {node, claim gid} for every
+// node of a claimed level-0 domain.  The effective owner is the claim gid (map mode) or owner_merge(node_owner[n], gid)
+// (occupancy, `occ`); participating rows of exclusive steps are rewritten to need·base[n] or -inf there, BEFORE the
+// consumed and anchor passes (-inf absorbs their adds, and an unblocked node must exist before them).  The step's
+// consumed records are then sorted by node with one record per node, so a record is its node's whole amount.
+template <bool CLAIMS>
+__device__ __forceinline__ void score_emit(TopoDev t, BatchDev b, int items, const int* __restrict__ claim_off,
+                                           const int2* __restrict__ claim_rec, bool occ) {
   const int T = b.chunk, lc = b.lc;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int groups = T >> 2;
@@ -130,6 +137,25 @@ k_score_emit(TopoDev t, BatchDev b, int items) {
         }
       }
 
+      if constexpr (CLAIMS) {
+        const int c0 = __ldg(claim_off + step), c1 = __ldg(claim_off + step + 1);
+        if (excl_step && c1 > c0) {
+          __syncthreads();  // the background stores precede the rewrite
+          for (int i = c0 + tid; i < c1; i += SCORE_THREADS) {
+            const int2 cl = __ldg(claim_rec + i);
+            const int m = cl.x;
+            if (m < n0 || m >= n1) continue;
+            const int ow = occ ? owner_merge(__ldg(t.node_owner + m), cl.y) : cl.y;
+            const int a = (ow == -1 || ow == gid) ? __ldg(t.free_ + m) : -1;
+            const float bm = __ldg(t.base + m);
+            for (int p = 0; p < P; ++p)
+              if (roles[p].w & RBGTOPO_ROLE_EXCLUSIVE)
+                mrow0[(size_t)p * stride + (m - n0)] = a >= roles[p].y ? (float)roles[p].z * bm : -INFINITY;
+          }
+          __syncthreads();  // ... and the consumed and anchor passes follow it
+        }
+      }
+
       // ---- 2. sparse corrections.  Few records: every warp scans them all and
       // applies the ones inside its own segments (ordering by __syncwarp alone).
       // Many records: one block barrier, then the records are spread over warps.
@@ -144,8 +170,12 @@ k_score_emit(TopoDev t, BatchDev b, int items) {
           const int g = (m - n0) >> 2;
           if (m >= n0 && m < n1 && (!own || ((g & (SCORE_THREADS - 1)) >> 5) == warp)) {
             int amt = 0;
-            for (int k = 0; k < h2.y; ++k)
-              if (__ldg(con + 2 * k) == m) amt += __ldg(con + 2 * k + 1);  // duplicates add up
+            if constexpr (CLAIMS) {
+              amt = __ldg(con + 2 * c + 1);  // one record per node
+            } else {
+              for (int k = 0; k < h2.y; ++k)
+                if (__ldg(con + 2 * k) == m) amt += __ldg(con + 2 * k + 1);  // duplicates add up
+            }
             const int avail = __ldg(t.free_ + m) - amt;
             for (int p = 0; p < P; ++p)
               if (avail < roles[p].y) mrow0[(size_t)p * stride + (m - n0)] = -INFINITY;
@@ -177,6 +207,18 @@ k_score_emit(TopoDev t, BatchDev b, int items) {
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(SCORE_THREADS, 6)
+k_score_emit(TopoDev t, BatchDev b, int items) {
+  score_emit<false>(t, b, items, nullptr, nullptr, false);
+}
+
+// Only rbgtopo_place_groups_lw_committed launches this variant.
+__global__ void __launch_bounds__(SCORE_THREADS, 6)
+k_score_emit_claims(TopoDev t, BatchDev b, int items, const int* __restrict__ claim_off,
+                    const int2* __restrict__ claim_rec, bool occ) {
+  score_emit<true>(t, b, items, claim_off, claim_rec, occ);
 }
 
 }  // namespace rbgtopo

@@ -61,6 +61,7 @@ class TopoPlacer:
         self.places_levels = bool(level_placement)
         self.places_committed_levels = bool(committed_levels)
         self.places_lw_ranked = True   # place_groups_lw_ranked: alternates for leader-worker pods (DESIGN.md §3.12)
+        self.places_lw_committed = True  # place_groups_lw_committed: committed leader-worker batches (§3.13)
         h = C.c_void_p()
         self._h = None
         self._check(self.lib.rbgtopo_create(C.byref(cfg), C.byref(h)))
@@ -208,6 +209,20 @@ class TopoPlacer:
         self._check(self.lib.rbgtopo_place_groups_lw(self._h, _p(gb), len(gb), _p(rp), len(rp), _p(assign),
                                                      _p(status), _p(domain)))
         return assign[:pods], status[:ng], domain[:ng]
+
+    def place_groups_lw_committed(self, groups_blob: np.ndarray, role_pods):
+        """place_groups_lw as a committed batch (DESIGN.md §3.13): in blob order, each group sees the pods and the
+        exclusive domains the groups before it took.  Returns (assign per pod, status, domain, wave-loop rounds run)."""
+        gb = _i32(groups_blob)
+        rp = _i32(np.asarray(role_pods, dtype=np.int64).reshape(-1))
+        ng, pods = int(gb[2]), self._lw_pods(gb, rp)
+        assign = np.empty(max(pods, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        rounds = C.c_int32()
+        self._check(self.lib.rbgtopo_place_groups_lw_committed(self._h, _p(gb), len(gb), _p(rp), len(rp), _p(assign),
+                                                               _p(status), _p(domain), C.byref(rounds)))
+        return assign[:pods], status[:ng], domain[:ng], rounds.value
 
     def place_groups_lw_ranked(self, groups_blob: np.ndarray, role_pods, n_alt: int):
         """place_groups_lw plus ranked alternates per pod (DESIGN.md §3.12): returns (assign, status, domain,

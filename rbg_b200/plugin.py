@@ -314,7 +314,10 @@ class B200TopoPodGroupManager:
         name, "{rbg}-{role}-{ordinal}-{k}" (k = 0 the leader); standalone roles keep "{rbg}-{role}-{ordinal}".  A
         role annotation COLOCATE_KEY names the topology key whose one domain must hold all pods of a replica; it
         resolves against exclusive_keys like an exclusive key (None: the level-0 label).  An unknown key, a level
-        the snapshot does not hold or a committed batch leave such a group without a hint and log why.  With
+        the snapshot does not hold leave such a group without a hint and log why.  A committed batch with such a
+        group and no group at an exclusive level >= 1 goes through ONE rbgtopo_place_groups_lw_committed call (§3.13)
+        when the placer has `places_lw_committed`: standalone groups take (1, -1) for every role and keep their RoleID
+        keys; otherwise (levels >= 1, or a placer without it) such a group gets no hint and a logged reason.  With
         alternates, such a group is placed through rbgtopo_place_groups_lw_ranked (§3.12) when the placer has
         `places_lw_ranked`, and its alternates are keyed by pod name and stay inside each replica's co-location
         domain; a placer without it gives no hint for such a group.
@@ -346,13 +349,21 @@ class B200TopoPodGroupManager:
             return lv, f"exclusive key {key!r} is not the level-0 label: committed batches place level 0 only"
         return lv, ""
 
+    def lw_committed(self, rbgs: Sequence[RoleBasedGroup], committed: bool) -> bool:
+        """A committed batch placed by one rbgtopo_place_groups_lw_committed call: it has a leader-worker group, no
+        group at an exclusive level >= 1, and the placer places such batches."""
+        return (committed and getattr(self.placer, "places_lw_committed", False)
+                and any(self.is_leader_worker(r) for r in rbgs)
+                and not any(self.exclusive_level(r, True)[0] > 0 for r in rbgs))
+
     def _split_no_hint(self, rbgs: Sequence[RoleBasedGroup], committed: bool = False):
         """The groups that get a hint, and a no-hint Placement per group that does not (logged, hint dropped)."""
         keep, skipped = [], {}
+        lw_commit = self.lw_committed(rbgs, committed)
         for i, r in enumerate(rbgs):
             _, reason = self.exclusive_level(r, committed)
             if not reason and self.is_leader_worker(r):
-                if committed:
+                if committed and not lw_commit:
                     reason = "leader-worker replicas: committed batches place one pod per replica"
                 elif self.alternates and not getattr(self.placer, "places_lw_ranked", False):
                     reason = "leader-worker replicas: no ranked alternates for them"
@@ -422,9 +433,17 @@ class B200TopoPodGroupManager:
         domains the groups before it took, so the hints of one call never contradict each other (the controller
         passes the groups ordered by namespaced name)."""
         all_rbgs = rbgs
+        lw_commit = self.lw_committed(rbgs, committed)
         rbgs, skipped = self._split_no_hint(rbgs, committed)
         if not rbgs:
             return self._merge(all_rbgs, [], skipped)
+        if lw_commit:   # one call in the given order: every group sees what the groups before it took
+            blob, runs = self.groups_blob(rbgs)
+            pods = [self.role_pods(g.rbg)[0] if self.is_leader_worker(g.rbg) else [(1, -1)] * len(g.rbg.roles)
+                    for g in runs]
+            role_pods = [pods[k][ri] for k, g in enumerate(runs) for ri in g.order]
+            assign, status, domain, _ = self.placer.place_groups_lw_committed(blob, role_pods)
+            return self._merge(all_rbgs, self._placements(runs, assign, status, domain, None, pods), skipped)
         lw = [i for i, r in enumerate(rbgs) if self.is_leader_worker(r)]
         plain = [i for i, r in enumerate(rbgs) if not self.is_leader_worker(r)]
         done: List[Optional[Placement]] = [None] * len(rbgs)   # by position in rbgs
