@@ -342,6 +342,33 @@ int32_t rbgtopo_place_groups_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int
                                     int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain,
                                     float* score, int32_t* alt_node, float* alt_score);
 
+/* Ranked alternates of a committed batch (DESIGN.md §3.14).  rbgtopo_place_groups_committed — same GROUPS blob,
+ * validation, error codes and levels rule, bit-identical assign / status / domain / *rounds — plus, per pending
+ * replica r (in assign order), score[r] and alt_node[r * n_alt + i] / alt_score[r * n_alt + i], i < n_alt, as by
+ * rbgtopo_place_groups_ranked, with room and owners counted after the WHOLE batch instead of after r's group:
+ *   - the row of r is the one its group's final placement was decided on in the committed wave loop (need over the
+ *     replicas still unplaced, the group's earlier waves as anchors); scores are the snapshot's;
+ *   - a candidate n has a finite score, is not assign[r], and free[n] - used_B[n] >= demand, where used_B sums the
+ *     demand of every replica this call placed on n, in all groups (a gang-failed group places nothing);
+ *   - for a participating role of an exclusive group g it also lies in domain[g] (a domain of g's level L_g) and the
+ *     owner a group of gid_g placed after the whole batch would see there is -1 or gid_g (§3.8's rule with every
+ *     group's claims, later groups' included; g's own claims never block g).
+ * So moving one replica to one of its alternates over-commits no node and meets no exclusive claim of another gid in
+ * this batch.  A one-group batch gives all six outputs of rbgtopo_place_groups_ranked.  Unfilled slots: node -1,
+ * score -inf; an unplaced replica and every replica of a gang-failed group get score -inf and no alternates.
+ * n_alt in [0, RBGTOPO_MAX_ALTERNATES], else RBGTOPO_EINVAL; status / domain / rounds may be NULL; alt_node /
+ * alt_score may be NULL when n_alt == 0.
+ * Exactness (§3.4) is checked before the first round against every wave the ranking can score, as
+ * rbgtopo_place_groups_lw checks it with one pod per replica: a non-gang group can reach a wave after unplaced
+ * replicas, so such a group can be refused with RBGTOPO_EINEXACT a little below the bound
+ * rbgtopo_place_groups_committed applies; nothing is written then, and the call never fails once it has placed.
+ * Documented limits (RBGTOPO_ELIMIT): a ctx with world > 1 (a rank holds only its slab of every dense row), more
+ * nodes than a shared-memory room bitmap of 200 KB holds (1 638 400), and a group table that does not fit
+ * k_plan_group, as for rbgtopo_place_groups_committed.  Leader-worker committed batches have no ranked form. */
+int32_t rbgtopo_place_groups_committed_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                              int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain,
+                                              int32_t* rounds, float* score, int32_t* alt_node, float* alt_score);
+
 /* Leader-worker replicas (DESIGN.md §3.11).  The GROUPS blob of rbgtopo_place_groups — same validation and
  * error codes — where a replica of a role can be several pods (a leaderWorkerPattern of size S: one leader and
  * S - 1 workers), optionally all inside one domain of a co-location level.

@@ -12,8 +12,13 @@
 // shared-memory bit per node whatever the group's size: the CTA first marks the nodes where free[n] - used_g[n] < demand from the group's aggregated placements (node, amount).
 // S[n] != -inf already implies free[n] >= demand (§3.3), so free[] is read only for those nodes.
 // Bandwidth-bound: 4 bytes per node and job (+ 4 for each domain condition).
+//
+// k_alternates_commit ranks the rows of a committed batch (rbgtopo_place_groups_committed_ranked, §3.14): `used` is
+// then the whole batch's placements, and a node of a participating job must also pass the owner test every group of the
+// batch has left on it (commit_owner with cm.g = n_groups), read only where the room bit is read.
 #pragma once
 #include "kernels.cuh"
+#include "plan_group.cuh"
 
 namespace rbgtopo {
 
@@ -54,10 +59,12 @@ __device__ __forceinline__ void alt_insert(unsigned long long (&top)[ALT_LIST], 
 // out: per compact replica 1 + 2 * n_alt words — score, n_alt nodes, n_alt scores (fp32 bits).
 // COLOC: some job has a co-location condition.  The <false> form is the ranked placement of one-pod replicas with the
 // registers it had before the condition existed (40; the condition costs 5 more, one CTA per SM less).
-template <bool COLOC>
-__global__ void __launch_bounds__(ALT_THREADS)
-k_alternates(TopoDev t, const float* __restrict__ rows, const AltJob* __restrict__ jobs, const int2* __restrict__ used,
-             const int* __restrict__ own, int n_alt, int* __restrict__ out) {
+// COMMIT (never with COLOC): gids[job] = the job's group gid; LV: the batch has a group at a level >= 1 (commit_owner<LV>).
+template <bool COLOC, bool COMMIT, bool LV>
+__device__ __forceinline__ void alternates_body(TopoDev t, const float* __restrict__ rows,
+                                                const AltJob* __restrict__ jobs, const int2* __restrict__ used,
+                                                const int* __restrict__ own, int n_alt, int* __restrict__ out,
+                                                const CommitDev& cm0, const int* __restrict__ gids) {
   extern __shared__ unsigned int sFull[];
   __shared__ unsigned long long sWarp[ALT_WARPS * ALT_LIST];
   __shared__ unsigned long long sTop[ALT_LIST];
@@ -99,6 +106,13 @@ k_alternates(TopoDev t, const float* __restrict__ rows, const AltJob* __restrict
       const unsigned long long k = make_key(s[j], m);
       if (k <= top[ALT_LIST - 1]) continue;
       if ((sFull[m >> 5] >> (m & 31)) & 1u) continue;
+      if constexpr (COMMIT)
+        if (need_dom) {  // d[j] = dom_{L_g}(m): the owner every group of the batch left on m
+          CommitDev cm = cm0;
+          cm.level = J.level;
+          const int o = commit_owner<LV>(cm, m, d[j], __ldg(at_level(t, J.level).node_owner + m));
+          if (!(o == -1 || o == __ldg(gids + blockIdx.x))) continue;
+        }
       alt_insert(top, k);
     }
   }
@@ -153,6 +167,22 @@ k_alternates(TopoDev t, const float* __restrict__ rows, const AltJob* __restrict
       o[1 + n_alt + k] = __float_as_int(-INFINITY);
     }
   }
+}
+
+template <bool COLOC>
+__global__ void __launch_bounds__(ALT_THREADS)
+k_alternates(TopoDev t, const float* __restrict__ rows, const AltJob* __restrict__ jobs, const int2* __restrict__ used,
+             const int* __restrict__ own, int n_alt, int* __restrict__ out) {
+  alternates_body<COLOC, false, false>(t, rows, jobs, used, own, n_alt, out, CommitDev{}, nullptr);
+}
+
+// cm: the final claims of the committed batch's rounds, cm.g = n_groups (every group's claims count).
+template <bool LV>
+__global__ void __launch_bounds__(ALT_THREADS)
+k_alternates_commit(TopoDev t, const float* __restrict__ rows, const AltJob* __restrict__ jobs,
+                    const int2* __restrict__ used, const int* __restrict__ own, int n_alt, int* __restrict__ out,
+                    CommitDev cm, const int* __restrict__ gids) {
+  alternates_body<false, true, LV>(t, rows, jobs, used, own, n_alt, out, cm, gids);
 }
 
 }  // namespace rbgtopo

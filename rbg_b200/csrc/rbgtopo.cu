@@ -1415,6 +1415,8 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
   }
   for (auto* f : {k_alternates<false>, k_alternates<true>})
     CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
+  for (auto* f : {k_alternates_commit<false>, k_alternates_commit<true>})
+    CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_lw_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_plan_group<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
 #ifdef RBGTOPO_PHASE_CLOCKS
@@ -1834,7 +1836,7 @@ struct KeptRows {
 };
 int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vector<AltRow>& list, const int32_t* gb,
                    const int32_t* rp, const int32_t* assign, const int32_t* status, const int32_t* domain,
-                   const RankReq& rk);
+                   const RankReq& rk, const CommitDev* cm = nullptr, bool cm_levels = false);
 void alt_clear(const RankReq& rk, int64_t first, int64_t count);
 }  // namespace
 
@@ -2147,9 +2149,12 @@ size_t group_role_rows(const int32_t* gb, int g) {
 // rp: the (S, C) table of place_groups_lw (§3.12), whose `list` entries and assign indices count pods, or nullptr (one
 // pod per replica, no co-location).  used_g sums the demand of every placed pod of the group.  A role with C >= 0
 // makes one job per co-location domain D_r its row's placed replicas chose; its unplaced replicas make none.
+// cm != nullptr: the rows of a committed batch (§3.14, rp == nullptr): every job's room is counted after the whole
+// batch (one list `used` of every group's placements), and participating jobs test the owner the batch left on a node
+// (k_alternates_commit<cm_levels>, cm->g = n_groups).
 int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vector<AltRow>& list, const int32_t* gb,
                    const int32_t* rp, const int32_t* assign, const int32_t* status, const int32_t* domain,
-                   const RankReq& rk) {
+                   const RankReq& rk, const CommitDev* cm, bool cm_levels) {
   const int F = rk.n_alt;
   const int ng = gb[2];
   std::vector<int> r0((size_t)ng + 1, 0);        // first role of every group in rp
@@ -2164,14 +2169,30 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
   std::vector<AltJob> jobs;
   std::vector<int2> used, tmp;
   std::vector<int> own, idx, doms;  // own / idx: node and assign index of every compact replica
+  std::vector<int> gids;            // cm: the gid of every job
   std::map<int, int2> placed;  // group -> (first, count) of its aggregated placements in `used`
   bool coloc = false;
+  if (cm) {  // (node, amount) per node the whole batch took
+    for (int g = 0; g < ng; ++g) {
+      if (status[g] == RBGTOPO_GANG_FAILED) continue;
+      const int32_t* rec = group_rec(gb, g);
+      int64_t i = pod0[g];
+      for (int q = 0; q < rec[3]; ++q)
+        for (int k = 0; k < gb[rec[4] + 4 * q + 1]; ++k, ++i)
+          if (assign[i] >= 0) tmp.push_back(make_int2(assign[i], gb[rec[4] + 4 * q + 2]));
+    }
+    std::sort(tmp.begin(), tmp.end(), [](int2 a, int2 b2) { return a.x < b2.x; });
+    for (const int2& u : tmp) {
+      if (!used.empty() && used.back().x == u.x) used.back().y += u.y;
+      else used.push_back(u);
+    }
+  }
   for (const AltRow& r : list) {
     if (status[r.group] == RBGTOPO_GANG_FAILED) continue;
     const int32_t* rec = group_rec(gb, r.group);
     const int32_t* roles = gb + rec[4];
     const int32_t* grp = rp ? rp + 2 * r0[r.group] : nullptr;
-    auto it = placed.find(r.group);
+    auto it = cm ? placed.emplace(r.group, make_int2(0, (int)used.size())).first : placed.find(r.group);
     if (it == placed.end()) {  // (node, amount) per node the group's pods of this call took
       tmp.clear();
       int64_t i = pod0[r.group];
@@ -2204,6 +2225,7 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
       add(r.rep0, r.nrep);
       j.nrep = (int)own.size() - j.rep0;
       jobs.push_back(j);
+      if (cm) gids.push_back(rec[0]);
       continue;
     }
     // D_r = dom_C of the replica's nodes (all S pods lie in it), in the order of first appearance
@@ -2227,7 +2249,7 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
   if (smem > kFastSmemMax) return fail(RBGTOPO_ELIMIT, "ranked placement: %d nodes exceed the room bitmap", c->topo.n);
   static_assert(sizeof(AltJob) % 4 == 0, "jobs are staged as words");
   const size_t w_jobs = jobs.size() * (sizeof(AltJob) / 4), w_used = used.size() * 2, w_own = own.size();
-  const size_t w_in = w_jobs + w_used + w_own, w_out = own.size() * (size_t)(1 + 2 * F);
+  const size_t w_in = w_jobs + w_used + w_own + gids.size(), w_out = own.size() * (size_t)(1 + 2 * F);
   cudaStream_t s = stream_of(c, b);
   CK(b->alt.reserve(w_in + w_out));
   CK(b->h_alt.reserve(w_in + w_out));
@@ -2235,11 +2257,17 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
   memcpy(h, jobs.data(), w_jobs * 4);
   memcpy(h + w_jobs, used.data(), w_used * 4);
   memcpy(h + w_jobs + w_used, own.data(), w_own * 4);
+  memcpy(h + w_jobs + w_used + w_own, gids.data(), gids.size() * 4);
   int* d = b->alt.p;
   CK(cudaMemcpyAsync(d, h, w_in * 4, cudaMemcpyHostToDevice, s));
-  (coloc ? k_alternates<true> : k_alternates<false>)<<<(unsigned)jobs.size(), ALT_THREADS, smem, s>>>(
-      topo_dev(c), rows, reinterpret_cast<const AltJob*>(d), reinterpret_cast<const int2*>(d + w_jobs),
-      d + w_jobs + w_used, F, d + w_in);
+  if (cm)
+    (cm_levels ? k_alternates_commit<true> : k_alternates_commit<false>)<<<(unsigned)jobs.size(), ALT_THREADS, smem, s>>>(
+        topo_dev(c), rows, reinterpret_cast<const AltJob*>(d), reinterpret_cast<const int2*>(d + w_jobs),
+        d + w_jobs + w_used, F, d + w_in, *cm, d + w_jobs + w_used + w_own);
+  else
+    (coloc ? k_alternates<true> : k_alternates<false>)<<<(unsigned)jobs.size(), ALT_THREADS, smem, s>>>(
+        topo_dev(c), rows, reinterpret_cast<const AltJob*>(d), reinterpret_cast<const int2*>(d + w_jobs),
+        d + w_jobs + w_used, F, d + w_in);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(h + w_in, d + w_in, w_out * 4, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
@@ -3623,8 +3651,119 @@ int place_groups_direct(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_
 // read-back.  Groups up to that lowest group are final, the next round re-runs the groups above it: it only grows, so
 // there are at most n_groups rounds, and a batch whose groups read nothing an earlier group took needs one.  The host
 // validates the blob exactly as the direct path of rbgtopo_place_groups does (same codes).
+int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
+                long long* total_pods);
+
+// Ranked alternates of a committed batch (DESIGN.md §3.14), once its rounds have converged: the dense row of every
+// (group, wave) that placed a replica is scored again as a step batch — the snapshot's scores, `need` over the
+// replicas still unplaced at that wave, the group's earlier waves as anchors — without consumed records and without
+// the exclusive flag: room and owner are tested by k_alternates_commit after the whole batch, against the final claims
+// in `cm`.  A batch whose rows exceed kReplayRows is scored and ranked in chunks of steps.  status / domain not null.
+constexpr long long kReplayBytes = 1LL << 30;
+int rank_committed(rbgtopo_ctx* c, Batch* b, const int32_t* gb, const int32_t* assign, const int32_t* status,
+                   const int32_t* domain, const CommitDev& cm, bool lv, const RankReq& rk, int* launches) {
+  const int ng = gb[2];
+  alt_clear(rk, 0, gb[4]);
+  cudaStream_t s = stream_of(c, b);
+  CK(cudaStreamWaitEvent(s, c->base_ready, 0));  // the rows read base and free of the snapshot the rounds saw
+  const int max_rows = (int)std::max<long long>(RBGTOPO_MAX_STEP_ROLES, kReplayBytes / 4 / c->slab_stride);
+  std::vector<int32_t> tab, data, anchors;  // the chunk's step table, and its sections (offsets from the table's end)
+  std::vector<AltRow> list;
+  int ns = 0, racc = 0, rowacc = 0, rc = RBGTOPO_OK;
+  auto flush = [&]() -> int {
+    if (ns == 0) return RBGTOPO_OK;
+    const int32_t base = RBGTOPO_HDR_WORDS + ns * RBGTOPO_STEP_WORDS;  // a multiple of 4: role records stay aligned
+    std::vector<int32_t> blob((size_t)base, 0);
+    for (int i = 0; i < ns; ++i) {
+      int32_t* st = tab.data() + (size_t)i * RBGTOPO_STEP_WORDS;
+      for (int k : {4, 6, 8, 10}) st[k] += base;
+    }
+    memcpy(blob.data() + RBGTOPO_HDR_WORDS, tab.data(), tab.size() * 4);
+    blob.insert(blob.end(), data.begin(), data.end());
+    blob[0] = RBGTOPO_BLOB_MAGIC;
+    blob[1] = RBGTOPO_ABI_VERSION;
+    blob[2] = ns;
+    blob[3] = (int32_t)blob.size();
+    blob[4] = racc;
+    blob[5] = rowacc;
+    int r2 = stage_into(c, b, blob.data(), (int64_t)blob.size());
+    if (!r2) r2 = launch_score(c, b, s);
+    if (!r2) r2 = run_alternates(c, b, b->matrix.p, list, gb, nullptr, assign, status, domain, rk, &cm, lv);
+    *launches += 2;
+    tab.clear(); data.clear(); list.clear();
+    ns = racc = rowacc = 0;
+    return r2;
+  };
+  for (int g = 0; g < ng && !rc; ++g) {
+    if (status[g] == RBGTOPO_GANG_FAILED) continue;
+    const int32_t* rec = group_rec(gb, g);
+    const int q = rec[3];
+    const int32_t* roles = gb + rec[4];
+    const int32_t* pair = gb + rec[5];
+    int ord0[RBGTOPO_MAX_GROUP_ROLES], unplaced[RBGTOPO_MAX_GROUP_ROLES];
+    for (int k = 0, acc = 0; k < q; ++k) { ord0[k] = acc; acc += roles[4 * k + 1]; unplaced[k] = roles[4 * k + 1]; }
+    anchors.assign(gb + rec[7], gb + rec[7] + 3LL * rec[6]);
+    walk_waves(roles, q, [&](int, const PlanWave& w) {
+      if (rc) return;
+      bool any = false;
+      for (int p = 0; p < w.n; ++p)
+        for (int k = 0; k < w.count[p]; ++k) any |= assign[rec[8] + ord0[w.role[p]] + w.first[p] + k] >= 0;
+      if (any) {
+        if (rowacc + w.n > max_rows) rc = flush();
+        if (rc) return;
+        int32_t st[RBGTOPO_STEP_WORDS] = {0};
+        st[0] = rec[0];
+        st[2] = -1;
+        st[3] = w.n;
+        while (data.size() & 3) data.push_back(0);
+        st[4] = (int32_t)data.size();
+        int n = 0;
+        for (int p = 0; p < w.n; ++p) {
+          const int ri = w.role[p];
+          int need = 0;
+          for (int k = 0; k < q; ++k)
+            if (pair[ri * q + k] > 0) need += unplaced[k];
+          data.push_back(w.count[p]);
+          data.push_back(roles[4 * ri + 2]);
+          data.push_back(std::min(need, RBGTOPO_NEED_CAP));
+          data.push_back(0);
+          n += w.count[p];
+          const int rep0 = rec[8] + ord0[ri] + w.first[p];
+          bool placed = false;
+          for (int k = 0; k < w.count[p]; ++k) placed |= assign[rep0 + k] >= 0;
+          if (placed) list.push_back(AltRow{rowacc + p, g, ri, rep0, w.count[p]});
+        }
+        st[5] = q;
+        st[6] = (int32_t)data.size();
+        for (int p = 0; p < w.n; ++p) data.insert(data.end(), pair + w.role[p] * q, pair + (w.role[p] + 1) * q);
+        st[7] = (int32_t)(anchors.size() / 3);
+        st[8] = (int32_t)data.size();
+        data.insert(data.end(), anchors.begin(), anchors.end());
+        st[10] = (int32_t)data.size();
+        st[11] = n;
+        st[12] = racc;
+        st[13] = rowacc;
+        tab.insert(tab.end(), st, st + RBGTOPO_STEP_WORDS);
+        ++ns;
+        racc += n;
+        rowacc += w.n;
+      }
+      for (int p = 0; p < w.n; ++p)  // the wave's placements: anchors of the later waves
+        for (int k = 0; k < w.count[p]; ++k) {
+          const int node = assign[rec[8] + ord0[w.role[p]] + w.first[p] + k];
+          if (node < 0) continue;
+          anchors.push_back(node); anchors.push_back(w.role[p]); anchors.push_back(1);
+          unplaced[w.role[p]] -= 1;
+        }
+    });
+  }
+  if (!rc) rc = flush();
+  return rc;
+}
+
+// rk != nullptr: the ranked form (§3.14): the same rounds, then rank_committed before the batch's buffers are released.
 int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign, int32_t* status,
-                           int32_t* domain, int32_t* rounds_out) {
+                           int32_t* domain, int32_t* rounds_out, const RankReq* rk = nullptr) {
   *rounds_out = 0;
   if (words < RBGTOPO_HDR_WORDS || gb[0] != RBGTOPO_GROUPS_MAGIC || gb[1] != RBGTOPO_ABI_VERSION || gb[3] != words)
     return fail(RBGTOPO_EINVAL, "bad groups blob header");
@@ -3656,6 +3795,17 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
   if (G.max_cap > 0x3FFFFFFFLL || G.smem > kFastSmemMax)
     return fail(RBGTOPO_ELIMIT, "a group's table of patched nodes (%lld entries, %zu B of shared memory) does not fit "
                                 "k_plan_group: a committed batch has no per-wave fallback", G.max_cap, G.smem);
+  if (rk) {  // before the first round: the ranking must not fail once the batch is placed
+    if ((size_t)((T.n + 31) / 32) * 4 > kFastSmemMax)
+      return fail(RBGTOPO_ELIMIT, "ranked placement: %d nodes exceed the room bitmap", T.n);
+    // the §3.4 bound over every wave the ranking can score: lw_validate's with one pod per replica (§3.11 rule 7)
+    long long qsum = 0, pods = 0;
+    for (int g = 0; g < ng; ++g) qsum += gb[RBGTOPO_HDR_WORDS + (int64_t)g * RBGTOPO_GROUP_WORDS + 3];
+    std::vector<int32_t> unit(2 * (size_t)qsum);
+    for (size_t i = 0; i < unit.size(); i += 2) { unit[i] = 1; unit[i + 1] = -1; }
+    rc = lw_validate(c, gb, words, unit.data(), (int64_t)unit.size(), &pods);
+    if (rc) return rc;
+  }
   run.clear();  // groups with pending replicas, ascending: a round runs a suffix of them
   for (int g = 0; g < ng; ++g)
     if (facts[g].nw > 0) run.push_back(g);
@@ -3678,6 +3828,7 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
   const bool timed = c->kernel_timing.load(std::memory_order_relaxed);
   std::vector<float> round_ms;
   int rounds = 0;
+  CommitDev cm{};  // the claims lists; after the last round they hold the final claims (the ranking reads them)
   rc = [&]() -> int {
     if (n0 == 0) return RBGTOPO_OK;
     const size_t run_off = ((size_t)words + 3) & ~(size_t)3;  // staging: GROUPS blob | pad | run[n0]
@@ -3704,7 +3855,6 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
     CK(cudaMemsetAsync(b->out.p, 0xFF, out_n * 4, s));
     CK(cudaMemsetAsync(ci + o_prev, 0xFF, out_n * 4, s));
     CK(cudaMemsetAsync(ci, 0xFF, (size_t)(N + ND + NP) * 4, s));
-    CommitDev cm{};
     cm.head = ci;
     cm.claim = b->cm_claim.p;
     cm.dhead = ci + o_dhead;
@@ -3789,11 +3939,24 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
     if (status) status[g] = st;
     if (domain) domain[g] = dm;
   }
+  int rank_launches = 0;
+  if (rk && n0 > 0) {
+    cm.g = ng;
+    rc = rank_committed(c, b, gb, assign, status, domain, cm, lv, *rk, &rank_launches);
+    if (rc) {
+      cudaStreamSynchronize(s);
+      release_batch(c, b);
+      return rc;
+    }
+  } else if (rk) {
+    alt_clear(*rk, 0, total_r);
+  }
   release_batch(c, b);
   *rounds_out = rounds;
   {
     rbgtopo_timing tm{};
-    tm.launches = 3 * rounds + (n0 > 0 ? 1 : 0);  // kernels: the first claims build, then plan + diff + claims per round
+    // kernels: the first claims build, then plan + diff + claims per round; ranked: score + k_alternates per chunk
+    tm.launches = 3 * rounds + (n0 > 0 ? 1 : 0) + rank_launches;
     tm.h2d_words = (int32_t)std::min<long long>((long long)words + n0, INT32_MAX);
     std::lock_guard<std::mutex> g(c->stat_mu);
     c->last = tm;
@@ -4425,6 +4588,29 @@ int32_t rbgtopo_place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_
   CK(cudaSetDevice(c->cfg.device));
   int32_t r = 0;
   const int rc = place_groups_committed(c, gb, words, assign, status, domain, &r);
+  if (rounds) *rounds = r;
+  return rc;
+}
+
+int32_t rbgtopo_place_groups_committed_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t n_alt,
+                                              int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds,
+                                              float* score, int32_t* alt_node, float* alt_score) {
+  if (rounds) *rounds = 0;
+  if (!c || !gb || !assign || !score || (n_alt > 0 && (!alt_node || !alt_score))) return fail(RBGTOPO_EINVAL, "null argument");
+  if (n_alt < 0 || n_alt > RBGTOPO_MAX_ALTERNATES)
+    return fail(RBGTOPO_EINVAL, "n_alt %d outside [0, %d]", n_alt, RBGTOPO_MAX_ALTERNATES);
+  if (c->cfg.world > 1)
+    return fail(RBGTOPO_ELIMIT, "ranked placement needs world == 1: a rank holds only its slab of every dense row");
+  std::shared_lock<std::shared_mutex> lk(c->topo_mu);  // one snapshot for the rounds and the ranking
+  if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
+  CK(cudaSetDevice(c->cfg.device));
+  const int64_t ng = words >= RBGTOPO_HDR_WORDS ? std::max<int64_t>(0, std::min<int64_t>(gb[2], words / RBGTOPO_GROUP_WORDS)) : 0;
+  std::vector<int32_t> own_status, own_domain;  // status / domain may be NULL: the ranking still needs them
+  if (!status) { own_status.resize((size_t)ng + 1); status = own_status.data(); }
+  if (!domain) { own_domain.resize((size_t)ng + 1); domain = own_domain.data(); }
+  const RankReq rk{n_alt, score, alt_node, alt_score};
+  int32_t r = 0;
+  const int rc = place_groups_committed(c, gb, words, assign, status, domain, &r, &rk);
   if (rounds) *rounds = r;
   return rc;
 }

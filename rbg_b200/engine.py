@@ -62,6 +62,7 @@ class TopoPlacer:
         self.places_committed_levels = bool(committed_levels)
         self.places_lw_ranked = True   # place_groups_lw_ranked: alternates for leader-worker pods (DESIGN.md §3.12)
         self.places_lw_committed = True  # place_groups_lw_committed: committed leader-worker batches (§3.13)
+        self.places_committed_ranked = True  # place_groups_committed_ranked: alternates of committed batches (§3.14)
         h = C.c_void_p()
         self._h = None
         self._check(self.lib.rbgtopo_create(C.byref(cfg), C.byref(h)))
@@ -159,6 +160,26 @@ class TopoPlacer:
         self._check(self.lib.rbgtopo_place_groups_committed(self._h, _p(gb), len(gb), _p(assign), _p(status),
                                                             _p(domain), C.byref(rounds)))
         return assign[:tp], status[:ng], domain[:ng], rounds.value
+
+    def place_groups_committed_ranked(self, groups_blob: np.ndarray, n_alt: int):
+        """place_groups_committed plus ranked alternates (DESIGN.md §3.14): returns (assign, status, domain, rounds,
+        score[R], alt_node[R, n_alt], alt_score[R, n_alt]).  assign / status / domain / rounds are those of
+        place_groups_committed; alt_node[r] holds the next-best nodes of replica r's row that still have room once the
+        WHOLE batch is placed and, for a participating role, that no exclusive claim of another gid in the batch
+        forbids (-1 / -inf where there are fewer), nothing for unplaced and gang-failed replicas."""
+        gb = _i32(groups_blob)
+        ng, tp = int(gb[2]), int(gb[4])
+        assign = np.empty(max(tp, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        rounds = C.c_int32()
+        score = np.empty(max(tp, 1), dtype=np.float32)
+        alt_node = np.empty((max(tp, 1), max(n_alt, 0)), dtype=np.int32)
+        alt_score = np.empty((max(tp, 1), max(n_alt, 0)), dtype=np.float32)
+        self._check(self.lib.rbgtopo_place_groups_committed_ranked(
+            self._h, _p(gb), len(gb), int(n_alt), _p(assign), _p(status), _p(domain), C.byref(rounds),
+            _p(score, _lib.f32p), _p(alt_node) if n_alt > 0 else None, _p(alt_score, _lib.f32p) if n_alt > 0 else None))
+        return (assign[:tp], status[:ng], domain[:ng], rounds.value, score[:tp], alt_node[:tp], alt_score[:tp])
 
     def place_groups_ranked(self, groups_blob: np.ndarray, n_alt: int):
         """place_groups plus ranked alternates (DESIGN.md §3.10): returns (assign, status, domain, score[R],

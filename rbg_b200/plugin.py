@@ -308,7 +308,11 @@ class B200TopoPodGroupManager:
         (no_hint[(ns, name)]): a hint into a domain of the wrong key is worse than none.
         alternates: next-best nodes per replica carried beside the hint (DESIGN.md §3.10, at most 8).  0 keeps the
         single-node hint; with n > 0 the snapshot call is rbgtopo_place_groups_ranked, which places identically and
-        also ranks, per replica, the nodes that still have room once its group is placed.
+        also ranks, per replica, the nodes that still have room once its group is placed.  A committed batch of
+        one-pod replicas goes through rbgtopo_place_groups_committed_ranked (§3.14) when the placer has
+        `places_committed_ranked`: same hints as rbgtopo_place_groups_committed, and alternates that still have
+        room, and meet no exclusive claim of another gid, once the whole batch is placed.  A placer without it gives
+        committed hints without alternates.  Committed leader-worker batches carry no alternates.
         leader_worker: a group with a role of lws_size > 1 is placed through rbgtopo_place_groups_lw (DESIGN.md
         §3.11): every replica of such a role is lws_size pods, placed all or nothing, and the hints are keyed by pod
         name, "{rbg}-{role}-{ordinal}-{k}" (k = 0 the leader); standalone roles keep "{rbg}-{role}-{ordinal}".  A
@@ -431,7 +435,9 @@ class B200TopoPodGroupManager:
         """committed=False: every group against the same snapshot (DESIGN.md §3.7), like concurrent reconciles.
         committed=True: a committed batch (§3.8) in the order given — each group sees the capacity and exclusive
         domains the groups before it took, so the hints of one call never contradict each other (the controller
-        passes the groups ordered by namespaced name)."""
+        passes the groups ordered by namespaced name).  With alternates, a committed batch of one-pod replicas gets
+        them from place_groups_committed_ranked (§3.14) when the placer has `places_committed_ranked`: room and
+        exclusive claims counted after the whole batch.  Committed leader-worker batches carry no alternates."""
         all_rbgs = rbgs
         lw_commit = self.lw_committed(rbgs, committed)
         rbgs, skipped = self._split_no_hint(rbgs, committed)
@@ -450,7 +456,10 @@ class B200TopoPodGroupManager:
         if plain:
             blob, runs = self.groups_blob([rbgs[i] for i in plain])
             alt_node = None
-            if committed:
+            if committed and self.alternates > 0 and getattr(self.placer, "places_committed_ranked", False):
+                assign, status, domain, _, _, alt_node, _ = self.placer.place_groups_committed_ranked(
+                    blob, self.alternates)
+            elif committed:
                 assign, status, domain, _ = self.placer.place_groups_committed(blob)
             elif self.alternates > 0:
                 assign, status, domain, _, alt_node, _ = self.placer.place_groups_ranked(blob, self.alternates)
