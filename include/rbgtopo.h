@@ -335,8 +335,10 @@ int32_t rbgtopo_place_groups_committed(rbgtopo_ctx* ctx, const int32_t* groups, 
  * included).  Unfilled slots: node -1, score -inf; an unplaced replica and every replica of a
  * gang-failed group get score -inf and no alternates.  n_alt in [0, RBGTOPO_MAX_ALTERNATES], else
  * RBGTOPO_EINVAL; alt_node / alt_score may be NULL when n_alt == 0.
- * Documented limit: a ctx with world > 1 holds only its slab of every dense row, so the call returns
- * RBGTOPO_ELIMIT there.  An RBGTOPO_SPLIT_MIN_GROUPS split does not apply to this call. */
+ * Documented limits (RBGTOPO_ELIMIT): a ctx with world > 1 (a rank holds only its slab of every dense
+ * row), and more nodes than a shared-memory room bitmap of 200 KB holds (1 638 400).  Both are checked
+ * before anything is placed: nothing is written then, and the call never fails once it has placed.
+ * An RBGTOPO_SPLIT_MIN_GROUPS split does not apply to this call. */
 #define RBGTOPO_MAX_ALTERNATES 8
 int32_t rbgtopo_place_groups_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
                                     int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain,

@@ -1855,6 +1855,8 @@ static int32_t place_groups_slow(rbgtopo_ctx* c, const int32_t* gb, int64_t word
     return fail(RBGTOPO_EINVAL, "group table exceeds blob");
   std::shared_lock<std::shared_mutex> lk(c->topo_mu);
   if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
+  if (kept && (size_t)((c->topo.n + 31) / 32) * 4 > kFastSmemMax)  // the snapshot may have changed since the direct pass
+    return fail(RBGTOPO_ELIMIT, "ranked placement: %d nodes exceed the room bitmap", c->topo.n);
   CK(cudaSetDevice(c->cfg.device));
   auto in = [&](long long off, long long cnt) { return off >= 0 && cnt >= 0 && off + cnt <= words; };
   std::vector<GroupRun> runs(ng);
@@ -3978,6 +3980,8 @@ int32_t place_groups_impl(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int3
   {
     std::shared_lock<std::shared_mutex> lk(c->topo_mu);
     if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
+    if (rk && (size_t)((c->topo.n + 31) / 32) * 4 > kFastSmemMax)  // before placing: the ranking must not fail afterwards
+      return fail(RBGTOPO_ELIMIT, "ranked placement: %d nodes exceed the room bitmap", c->topo.n);
     CK(cudaSetDevice(c->cfg.device));
     static const bool prof = getenv("RBGTOPO_PROFILE_HOST") != nullptr;
     auto now = [] { return std::chrono::steady_clock::now(); };

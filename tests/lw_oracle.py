@@ -5,10 +5,13 @@ oracle's own BLOB format (oracle/wave_loop.build_blob: role counts in pods, need
 placed pod, consumed capacity per node) scored by the CPU oracle (oracle/placer.py); its dense rows are all this file
 takes from it.  Rule 3 is then restated literally: candidates with room, D* as §3.5 decides it, the level-C domains
 enumerated with their pod capacity, the best one that holds the replica, the pods one after the other, and a replica
-whose pods do not all fit reverted before the next one.
+whose pods do not all fit reverted before the next one.  That enumeration costs O(N) per domain; `fast_domains()`
+swaps in a one-pass form of the same choice (domain_fast) for fleets with one domain per node.
 """
 from __future__ import annotations
 
+import contextlib
+import functools
 from typing import List, Optional, Sequence
 
 import numpy as np
@@ -96,8 +99,40 @@ class LwGroup:
                     consumed=sorted(self.consumed.items()))
 
 
-def place_wave(G: LwGroup, w: int, rows: np.ndarray, topo, excl_domain: np.ndarray, level_domain) -> tuple:
-    """Rule 3 for group G's wave w; rows[p] = the dense row of the wave's role p.  Returns (pods, status, D*)."""
+def domain_literal(cand: np.ndarray, avail: np.ndarray, demand: int, S: int, dom: np.ndarray, row: np.ndarray) -> int:
+    """D_r as rule 3 states it: enumerate the level-C domains of the candidates, count the pods each can hold, keep the
+    best one that holds S (its best candidate by key); -1 if none.  O(N) per domain."""
+    chosen, chosen_best = -1, -1
+    for d in np.unique(dom[cand]):
+        members = cand & (dom == d)
+        cap = int((avail[members] // demand).sum()) if demand > 0 else S
+        if cap < S:
+            continue
+        b = best_node(members, row)
+        if better(b, chosen_best, row):
+            chosen, chosen_best = int(d), b
+    return chosen
+
+
+def domain_fast(cand: np.ndarray, avail: np.ndarray, demand: int, S: int, dom: np.ndarray, row: np.ndarray) -> int:
+    """domain_literal in one pass: per-domain pod capacity by bincount (S per candidate when demand = 0), then the best
+    candidate among the domains that hold S.  O(N) per replica, so one domain per node stays cheap."""
+    idx = np.flatnonzero(cand)
+    if len(idx) == 0:
+        return -1
+    d = dom[idx]
+    per = avail[idx] // demand if demand > 0 else np.full(len(idx), S, dtype=np.int64)
+    cap = np.bincount(d, weights=per.astype(np.float64))   # sums below 2^53: exact
+    keep = np.zeros(len(row), dtype=bool)
+    keep[idx[cap[d] >= S]] = True
+    b = best_node(keep, row)
+    return int(dom[b]) if b >= 0 else -1
+
+
+def place_wave(G: LwGroup, w: int, rows: np.ndarray, topo, excl_domain: np.ndarray, level_domain,
+               choose=domain_literal) -> tuple:
+    """Rule 3 for group G's wave w; rows[p] = the dense row of the wave's role p.  Returns (pods, status, D*).
+    choose: how D_r is found (domain_literal or domain_fast; they agree)."""
     n = topo.n
     avail = topo.free.astype(np.int64).copy()
     for node, amt in G.consumed.items():
@@ -122,18 +157,9 @@ def place_wave(G: LwGroup, w: int, rows: np.ndarray, topo, excl_domain: np.ndarr
         for _ in range(reps):
             inside = np.ones(n, dtype=bool)
             ok = True
-            if C >= 0:   # enumerate the level-C domains, count the pods each can hold, keep the best that holds S
+            if C >= 0:   # the best level-C domain that holds the replica
                 dom = np.asarray(level_domain[C])
-                cand = scored & (avail >= demand)
-                chosen, chosen_best = -1, -1
-                for d in np.unique(dom[cand]):
-                    members = cand & (dom == d)
-                    cap = int((avail[members] // demand).sum()) if demand > 0 else S
-                    if cap < S:
-                        continue
-                    b = best_node(members, row)
-                    if better(b, chosen_best, row):
-                        chosen, chosen_best = int(d), b
+                chosen = choose(scored & (avail >= demand), avail, demand, S, dom, row)
                 if chosen < 0:
                     ok = False
                 else:
@@ -156,6 +182,22 @@ def place_wave(G: LwGroup, w: int, rows: np.ndarray, topo, excl_domain: np.ndarr
     if gang and unplaced:
         return [-1] * len(pods), 2, dstar
     return pods, 1 if unplaced else 0, dstar
+
+
+_place_wave = place_wave   # the function itself, whatever the name place_wave is bound to
+
+
+@contextlib.contextmanager
+def fast_domains():
+    """Inside the block place_wave finds D_r with domain_fast.  run_lw, lw_committed_oracle and lw_alternates_oracle
+    all call place_wave through this module, so all three oracles then scale to one domain per node."""
+    global place_wave
+    saved = place_wave
+    place_wave = functools.partial(_place_wave, choose=domain_fast)
+    try:
+        yield
+    finally:
+        place_wave = saved
 
 
 def run_lw(topo, gblob, role_pods, level_domain=None, excl_domain=None, groups: Optional[Sequence[int]] = None):
