@@ -338,6 +338,10 @@ int32_t rbgtopo_place_groups_committed(rbgtopo_ctx* ctx, const int32_t* groups, 
  * Documented limits (RBGTOPO_ELIMIT): a ctx with world > 1 (a rank holds only its slab of every dense
  * row), and more nodes than a shared-memory room bitmap of 200 KB holds (1 638 400).  Both are checked
  * before anything is placed: nothing is written then, and the call never fails once it has placed.
+ * Exactness (§3.4) is checked before anything is placed too, with the bound rbgtopo_place_groups_lw
+ * applies with one pod per replica: a non-gang group the host-driven loop re-runs reaches waves after
+ * unplaced replicas, so such a group can be refused with RBGTOPO_EINEXACT a little below the bound
+ * rbgtopo_place_groups applies, with nothing written.
  * An RBGTOPO_SPLIT_MIN_GROUPS split does not apply to this call. */
 #define RBGTOPO_MAX_ALTERNATES 8
 int32_t rbgtopo_place_groups_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,

@@ -3973,6 +3973,25 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
 }  // namespace
 
 namespace {
+// The exactness bound of a ranked placement (§3.10): lw_validate's with one pod per replica, which takes every mix of
+// unplaced earlier replicas a re-run group's later waves can see.  Only its RBGTOPO_EINEXACT is returned: a malformed
+// blob gets the code the placement itself gives it.
+int ranked_exact(rbgtopo_ctx* c, const int32_t* gb, int64_t words) {
+  if (words < RBGTOPO_HDR_WORDS || gb[0] != RBGTOPO_GROUPS_MAGIC || gb[3] != words) return RBGTOPO_OK;
+  const int ng = gb[2];
+  if (ng < 0 || (int64_t)RBGTOPO_HDR_WORDS + (int64_t)ng * RBGTOPO_GROUP_WORDS > words) return RBGTOPO_OK;
+  long long qsum = 0, pods = 0;
+  for (int g = 0; g < ng; ++g) {
+    const int q = gb[RBGTOPO_HDR_WORDS + (int64_t)g * RBGTOPO_GROUP_WORDS + 3];
+    if (q < 0 || q > RBGTOPO_MAX_GROUP_ROLES) return RBGTOPO_OK;
+    qsum += q;
+  }
+  std::vector<int32_t> unit(2 * (size_t)qsum);
+  for (size_t i = 0; i < unit.size(); i += 2) { unit[i] = 1; unit[i + 1] = -1; }
+  const int rc = lw_validate(c, gb, words, unit.data(), (int64_t)unit.size(), &pods);
+  return rc == RBGTOPO_EINEXACT ? rc : RBGTOPO_OK;
+}
+
 // rbgtopo_place_groups, and its ranked form when rk != nullptr (status and domain are then not null)
 int32_t place_groups_impl(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign, int32_t* status,
                           int32_t* domain, const RankReq* rk) {
@@ -3982,6 +4001,10 @@ int32_t place_groups_impl(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int3
     if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
     if (rk && (size_t)((c->topo.n + 31) / 32) * 4 > kFastSmemMax)  // before placing: the ranking must not fail afterwards
       return fail(RBGTOPO_ELIMIT, "ranked placement: %d nodes exceed the room bitmap", c->topo.n);
+    if (rk) {  // before placing: a group the host loop re-runs must not meet the §3.4 bound in a later wave (§3.10)
+      const int rc0 = ranked_exact(c, gb, words);
+      if (rc0) return rc0;
+    }
     CK(cudaSetDevice(c->cfg.device));
     static const bool prof = getenv("RBGTOPO_PROFILE_HOST") != nullptr;
     auto now = [] { return std::chrono::steady_clock::now(); };

@@ -65,7 +65,8 @@ def run_fleet_committed_levels(topo, groups: Sequence[wave_loop.OGroup], group_l
     last = [np.full(int(n_domains[L]), FREE, np.int32) for L in range(dom.shape[0])]
     pods: List = []
     claimed: Dict[int, int] = {}
-    other = max([g.gid for g in groups] + [0]) + 1
+    gids = {g.gid for g in groups}
+    other = min(set(range(len(gids) + 1)) - gids)   # a gid of no group that fits int32 (gids reach 2^31 - 1)
     states: List = []
     for g, L in zip(groups[:limit], group_levels):
         ow = np.array(owner, dtype=np.int32, copy=True)
