@@ -205,7 +205,9 @@ __global__ void k_prep(int n, const int* __restrict__ free_, const int* __restri
 // [L * ls, L * ls + n) of `dom` / `owner` (ls = level_stride(n): the dense-matrix kernels load owners as int4);
 // the per-level domain tables are tab[doff[L] + d] (present) and tab[total_d + doff[L] + d] (keyed).  Owner
 // values merge with  -1 (+) x = x,  x (+) x = x,  anything else -2  (blocked for every group).
-// phase 0: clear the tables; 1: scatter the records (node, gid, level); 2: one gather per node.
+// phase 0: clear the tables; 1: scatter the records (node, gid, level); 2: one gather per node.  The loop indices
+// are 64-bit: 2 * total_d reaches 2^31 - 32 at the domain ceiling (0x3FFFFFF0), where an int index plus one grid
+// stride would overflow.
 __device__ __forceinline__ int owner_merge(int a, int b) { return a == -1 ? b : (b == -1 || a == b) ? a : -2; }
 __device__ __forceinline__ void owner_merge_at(int* p, int g) {
   const int old = atomicCAS(p, -1, g);
@@ -215,23 +217,23 @@ __global__ void k_level_owner(int phase, int n, int n_lv, const int* __restrict_
                               int total_d, int* __restrict__ tab, const int* __restrict__ occ, int n_occ,
                               int* __restrict__ owner) {
   const int ls = level_stride(n);
-  const int stride = gridDim.x * blockDim.x;
-  const int i0 = blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (phase == 0) {
-    for (int i = i0; i < 2 * total_d; i += stride) tab[i] = -1;
+    for (long long i = i0; i < 2LL * total_d; i += stride) tab[i] = -1;
   } else if (phase == 1) {
-    for (int r = i0; r < n_occ; r += stride) {
+    for (long long r = i0; r < n_occ; r += stride) {
       const int node = occ[3 * r], gid = occ[3 * r + 1], lv = occ[3 * r + 2];
       for (int L = 0; L < n_lv; ++L) {
-        const int d = doff[L] + dom[(size_t)L * ls + node];
+        const long long d = (long long)doff[L] + dom[(size_t)L * ls + node];
         owner_merge_at(tab + d, gid);                       // present: records count at every level
         if (L == lv) owner_merge_at(tab + total_d + d, gid);  // keyed: only at the record's own level
       }
     }
   } else {
-    for (int v = i0; v < n; v += stride) {
+    for (long long v = i0; v < n; v += stride) {
       int k = -1;
-      for (int L = 0; L < n_lv; ++L) k = owner_merge(k, tab[total_d + doff[L] + dom[(size_t)L * ls + v]]);
+      for (int L = 0; L < n_lv; ++L) k = owner_merge(k, tab[(long long)total_d + doff[L] + dom[(size_t)L * ls + v]]);
       for (int L = 0; L < n_lv; ++L) owner[(size_t)L * ls + v] = owner_merge(tab[doff[L] + dom[(size_t)L * ls + v]], k);
     }
   }

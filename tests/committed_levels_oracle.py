@@ -66,7 +66,7 @@ def run_fleet_committed_levels(topo, groups: Sequence[wave_loop.OGroup], group_l
     pods: List = []
     claimed: Dict[int, int] = {}
     gids = {g.gid for g in groups}
-    other = min(set(range(len(gids) + 1)) - gids)   # a gid of no group that fits int32 (gids reach 2^31 - 1)
+    other = levels_oracle.unused_gid(gids)          # a gid of no group that fits int32 (gids reach 2^31 - 1)
     states: List = []
     for g, L in zip(groups[:limit], group_levels):
         ow = np.array(owner, dtype=np.int32, copy=True)

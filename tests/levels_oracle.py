@@ -1,6 +1,8 @@
 """Oracle of exclusive topology at several levels (DESIGN.md §3.9; test infrastructure).
 
 derive_level_owner   the owner vector of every level from the pod records, as §3.9 defines it (numpy);
+derive_level_owner_fast  the same, vectorised (a million nodes x eight levels); the literal form stays the reference;
+unused_gid           the smallest non-negative gid no group uses (the "other" owner of a level view);
 constraining_gids    a restatement node by node: the set of exclusive groups whose pods constrain a labeled pod there;
 owner_from_terms     the brute-force checker: the terms oracle.refpinned.exclusive_affinity_terms returns (the pinned
                      restatement of setExclusiveAffinities), evaluated with label-selector semantics on both sides of
@@ -50,6 +52,47 @@ def derive_level_owner(level_domain: np.ndarray, occ) -> np.ndarray:
         for L in range(n_lv):
             out[L, v] = merge(present[L].get(int(dom[L, v]), FREE), k)
     return out
+
+
+def merge_arrays(a: np.ndarray, b: np.ndarray) -> np.ndarray:
+    """merge element by element."""
+    return np.where(a == FREE, b, np.where((b == FREE) | (a == b), a, BLOCKED)).astype(np.int32)
+
+
+def domain_owner_fast(dom: np.ndarray, nodes: np.ndarray, gids: np.ndarray) -> np.ndarray:
+    """Per node v: the merge of the gids of the records (nodes[i], gids[i]) whose node shares v's domain — the one gid
+    of a domain with one distinct gid, -2 with two or more, -1 with none.  Domains are renumbered densely first, so a
+    partition with ~2^30 mostly empty domains costs O(n)."""
+    ids, cd = np.unique(np.asarray(dom, dtype=np.int64), return_inverse=True)
+    own = np.full(len(ids), FREE, dtype=np.int32)
+    if len(nodes):
+        pairs = np.unique(cd[nodes].astype(np.int64) << 32 | np.asarray(gids, dtype=np.int64))
+        pd, pg = (pairs >> 32).astype(np.int64), (pairs & 0xFFFFFFFF).astype(np.int32)
+        own[pd] = pg
+        own[np.bincount(pd, minlength=len(ids)) >= 2] = BLOCKED
+    return own[cd]
+
+
+def derive_level_owner_fast(level_domain: np.ndarray, occ) -> np.ndarray:
+    """derive_level_owner in vectorised numpy, for a million nodes x eight levels: per level, the distinct
+    (domain, gid) pairs of the records (all of them for present_L, those of level L for keyed_L), then one gather per
+    node."""
+    dom = np.asarray(level_domain)
+    n_lv, n = dom.shape
+    occ = np.asarray(occ, dtype=np.int64).reshape(-1, 3)
+    node, gid, lv = occ[:, 0], occ[:, 1], occ[:, 2]
+    present = [domain_owner_fast(dom[L], node, gid) for L in range(n_lv)]
+    k = np.full(n, FREE, dtype=np.int32)
+    for L in range(n_lv):
+        m = lv == L
+        k = merge_arrays(k, domain_owner_fast(dom[L], node[m], gid[m]))
+    return np.stack([merge_arrays(present[L], k) for L in range(n_lv)]) if n_lv else np.empty((0, n), np.int32)
+
+
+def unused_gid(gids) -> int:
+    """The smallest non-negative gid no group uses: an "other" owner that fits int32 even next to gid 2^31 - 1."""
+    used = {int(g) for g in gids}
+    return min(set(range(len(used) + 1)) - used)
 
 
 def constraining_gids(level_domain: np.ndarray, occ, level: int, node: int) -> set:

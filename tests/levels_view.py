@@ -37,7 +37,7 @@ def expected_fleet(topo, level_domain, owner, n_domains, gblob):
     """Per group (assign in group order, status, domain) of the wave loop on the group's level view, plus the views."""
     ng = int(gblob[2])
     gids = [int(gblob[8 + 12 * g]) for g in range(ng)]
-    other = max(gids) + 1
+    other = lo.unused_gid(gids)
     out, views = [], []
     for g in range(ng):
         L = int(gblob[8 + 12 * g + 10])
