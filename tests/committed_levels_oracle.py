@@ -57,10 +57,13 @@ def level_owner(level_domain: np.ndarray, owner: np.ndarray, n_domains, level: i
 
 def run_fleet_committed_levels(topo, groups: Sequence[wave_loop.OGroup], group_levels: Sequence[int],
                                level_domain: np.ndarray, owner: np.ndarray, n_domains, nthreads: int = 1,
-                               limit: Optional[int] = None, fast: bool = False) -> List[wave_loop.GroupState]:
+                               limit: Optional[int] = None, fast: bool = False, terms: Sequence[str] = ("K", "P"),
+                               reporter: str = "last") -> List[wave_loop.GroupState]:
     """States in the given order.  level_domain [n_levels + 1][n] (row 0 = the snapshot's domain), owner =
     levels_oracle.derive_level_owner(level_domain, occ), n_domains per level.  `limit`: place only the first `limit`
-    groups."""
+    groups.  `terms` and `reporter` exist for the preconditions of tests/commit_levels_limits_cases.py: the owner
+    without the domain term K or the pod term P, or with the first earlier reporter of a domain instead of the last."""
+    assert set(terms) <= {"K", "P"} and reporter in ("last", "first")
     dom = np.asarray(level_domain)
     last = [np.full(int(n_domains[L]), FREE, np.int32) for L in range(dom.shape[0])]
     pods: List = []
@@ -82,9 +85,10 @@ def run_fleet_committed_levels(topo, groups: Sequence[wave_loop.OGroup], group_l
             claimed[node] = claimed.get(node, 0) + amt
         res = s.result()
         if g.exclusive and res["status"] != 2:
-            if res["domain"] >= 0:
+            if res["domain"] >= 0 and "K" in terms and (reporter == "last" or last[L][res["domain"]] == FREE):
                 last[L][res["domain"]] = g.gid
-            pods += [(g.gid, L, m) for m in participating_pods(s)]
+            if "P" in terms:
+                pods += [(g.gid, L, m) for m in participating_pods(s)]
         states.append(s)
     return states
 
