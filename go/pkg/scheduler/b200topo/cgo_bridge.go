@@ -106,6 +106,16 @@ static int32_t rbgtopo_go_place_groups_lw_committed(rbgtopo_ctx* ctx, const int3
   rbgtopo_go_err(ctx, rc, err);
   return rc;
 }
+static int32_t rbgtopo_go_place_groups_lw_committed_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t words,
+                                                           const int32_t* role_pods, int64_t role_pods_words,
+                                                           int32_t n_alt, int32_t* assign, int32_t* status,
+                                                           int32_t* domain, int32_t* rounds, float* score,
+                                                           int32_t* alt_node, float* alt_score, char* err) {
+  int32_t rc = rbgtopo_place_groups_lw_committed_ranked(ctx, groups, words, role_pods, role_pods_words, n_alt, assign,
+                                                        status, domain, rounds, score, alt_node, alt_score);
+  rbgtopo_go_err(ctx, rc, err);
+  return rc;
+}
 static int32_t rbgtopo_go_place_groups_lw_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t words,
                                                  const int32_t* role_pods, int64_t role_pods_words, int32_t n_alt,
                                                  int32_t* assign, int32_t* status, int32_t* domain, float* score,
@@ -351,4 +361,27 @@ func (p *placer) placeGroupsLWRanked(blob, rolePods []int32, nPods, nAlt int) (a
 		return nil, nil, nil, nil, err
 	}
 	return assign[:nPods], status[:nGroups], domain[:nGroups], altNode[:nPods*nAlt], nil
+}
+
+// placeGroupsLWCommittedRanked: placeGroupsLWCommitted plus, per pod, up to nAlt next-best nodes that still have room
+// once the whole batch is placed, that meet no exclusive claim of another gid in the batch for a participating role,
+// and that keep a co-located replica inside its domain (DESIGN.md §3.15); altNode[p*nAlt+i] = -1 where there are
+// fewer.  assign / status / domain / rounds are placeGroupsLWCommitted's.
+func (p *placer) placeGroupsLWCommittedRanked(blob, rolePods []int32, nPods, nAlt int) (assign, status, domain, altNode []int32, rounds int32, err error) {
+	nGroups := int(blob[2])
+	assign = make([]int32, max(nPods, 1))
+	status = make([]int32, max(nGroups, 1))
+	domain = make([]int32, max(nGroups, 1))
+	score := make([]float32, max(nPods, 1))
+	altNode = make([]int32, max(nPods*nAlt, 1))
+	altScore := make([]float32, max(nPods*nAlt, 1))
+	var r C.int32_t
+	var buf [C.RBGTOPO_GO_ERRLEN]C.char
+	rc := C.rbgtopo_go_place_groups_lw_committed_ranked(p.ctx, p32(blob), C.int64_t(len(blob)), p32(rolePods),
+		C.int64_t(len(rolePods)), C.int32_t(nAlt), p32(assign), p32(status), p32(domain), &r,
+		(*C.float)(unsafe.Pointer(&score[0])), p32(altNode), (*C.float)(unsafe.Pointer(&altScore[0])), &buf[0])
+	if err = mkErr(rc, &buf); err != nil {
+		return nil, nil, nil, nil, 0, err
+	}
+	return assign[:nPods], status[:nGroups], domain[:nGroups], altNode[:nPods*nAlt], int32(r), nil
 }

@@ -370,7 +370,8 @@ int32_t rbgtopo_place_groups_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int
  * rbgtopo_place_groups_committed applies; nothing is written then, and the call never fails once it has placed.
  * Documented limits (RBGTOPO_ELIMIT): a ctx with world > 1 (a rank holds only its slab of every dense row), more
  * nodes than a shared-memory room bitmap of 200 KB holds (1 638 400), and a group table that does not fit
- * k_plan_group, as for rbgtopo_place_groups_committed.  Leader-worker committed batches have no ranked form. */
+ * k_plan_group, as for rbgtopo_place_groups_committed.  The ranked form of a committed leader-worker batch is
+ * rbgtopo_place_groups_lw_committed_ranked. */
 int32_t rbgtopo_place_groups_committed_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
                                               int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain,
                                               int32_t* rounds, float* score, int32_t* alt_node, float* alt_score);
@@ -433,10 +434,36 @@ int32_t rbgtopo_place_groups_lw_ranked(rbgtopo_ctx* ctx, const int32_t* groups, 
  * Over the batch no node receives more than free[n].  With S = 1 and C = -1 everywhere the results are
  * bit-identical to rbgtopo_place_groups_committed's.  *rounds (may be NULL) = wave-loop rounds run: at most
  * n_groups, 1 for one group.  Limits (RBGTOPO_ELIMIT): a group whose own exclusive level is >= 1, a ctx with
- * world > 1, more nodes than the room bitmap of rbgtopo_place_groups_lw holds.  No alternates. */
+ * world > 1, more nodes than the room bitmap of rbgtopo_place_groups_lw holds.  Alternates:
+ * rbgtopo_place_groups_lw_committed_ranked. */
 int32_t rbgtopo_place_groups_lw_committed(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
                                           const int32_t* role_pods, int64_t role_pods_words, int32_t* assign,
                                           int32_t* status, int32_t* domain, int32_t* rounds);
+
+/* Ranked alternates of a committed leader-worker batch (DESIGN.md §3.15).  rbgtopo_place_groups_lw_committed — same
+ * GROUPS blob and (S, C) table, validation, exactness bound, error codes and limits (a group exclusive at a level
+ * >= 1 is RBGTOPO_ELIMIT), bit-identical assign / status / domain / *rounds — plus, per pod p (in assign order),
+ * score[p] and alt_node[p * n_alt + i] / alt_score[p * n_alt + i], i < n_alt, as by
+ * rbgtopo_place_groups_lw_ranked, with room and owners counted after the WHOLE batch:
+ *   - the row of p is the one of its replica's (wave, role) in its group's final run of the committed wave loop
+ *     (need over the pods still unplaced, the group's earlier pods as anchors (node, role, 1)); scores are the
+ *     snapshot's;
+ *   - a candidate n has a finite score, is not assign[p], and free[n] - used_B[n] >= demand, where used_B sums the
+ *     demand of every pod this call placed on n, in all groups (a gang-failed group places nothing);
+ *   - for a participating role of an exclusive group g it also lies in domain[g] and the level-0 owner the whole
+ *     batch leaves there (§3.13's rule with every group's claims, later groups' included) is -1 or gid_g;
+ *   - for a role with C >= 0 it lies in the level-C domain of the pod's replica (dom_C(n) = dom_C(assign[p])).
+ * So moving one pod to one of its alternates over-commits no node, meets no exclusive claim of another gid in this
+ * batch and keeps its replica co-located.  A one-group batch gives all six outputs of rbgtopo_place_groups_lw_ranked;
+ * with S = 1 and C = -1 everywhere, every output but *rounds is bit-identical to
+ * rbgtopo_place_groups_committed_ranked's.  Unfilled slots: node -1, score -inf; an unplaced pod and every pod of a
+ * gang-failed group get score -inf and no alternates.  n_alt in [0, RBGTOPO_MAX_ALTERNATES], else RBGTOPO_EINVAL;
+ * status / domain / rounds may be NULL; alt_node / alt_score may be NULL when n_alt == 0.  The call accepts exactly
+ * the blobs rbgtopo_place_groups_lw_committed accepts, and never fails once it has placed. */
+int32_t rbgtopo_place_groups_lw_committed_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                                 const int32_t* role_pods, int64_t role_pods_words, int32_t n_alt,
+                                                 int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds,
+                                                 float* score, int32_t* alt_node, float* alt_score);
 
 /* rbgtopo_place_groups pipeline, staged: the groups are compiled into a
  * device-resident multi-wave plan (one step blob, wave-major, expanded on the

@@ -53,6 +53,8 @@ SIGNATURES = {
     "rbgtopo_place_groups_lw": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, C.c_int64, i32p, i32p, i32p]),
     "rbgtopo_place_groups_lw_committed": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, C.c_int64, i32p, i32p, i32p,
                                                       i32p]),
+    "rbgtopo_place_groups_lw_committed_ranked": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, C.c_int64, C.c_int32,
+                                                             i32p, i32p, i32p, i32p, f32p, i32p, f32p]),
     "rbgtopo_place_groups_lw_ranked": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, C.c_int64, C.c_int32, i32p, i32p,
                                                    i32p, f32p, i32p, f32p]),
     "rbgtopo_stage_groups": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p]),

@@ -1834,9 +1834,17 @@ struct KeptRows {
   size_t cap = 0;
   std::vector<AltRow> list;
 };
+// The level-0 owner claims of a committed leader-worker batch (§3.15), built on the host from its final claims in the
+// layout commit_owner<false> reads: dhead[d] = a group that reported domain d (-1 = none), dclaim[g] = {gid of group g,
+// next group that reported the same domain}.
+struct HostClaims {
+  std::vector<int32_t> dhead;
+  std::vector<int2> dclaim;
+};
 int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vector<AltRow>& list, const int32_t* gb,
                    const int32_t* rp, const int32_t* assign, const int32_t* status, const int32_t* domain,
-                   const RankReq& rk, const CommitDev* cm = nullptr, bool cm_levels = false);
+                   const RankReq& rk, const CommitDev* cm = nullptr, bool cm_levels = false,
+                   const HostClaims* hc = nullptr);
 void alt_clear(const RankReq& rk, int64_t first, int64_t count);
 }  // namespace
 
@@ -2151,12 +2159,13 @@ size_t group_role_rows(const int32_t* gb, int g) {
 // rp: the (S, C) table of place_groups_lw (§3.12), whose `list` entries and assign indices count pods, or nullptr (one
 // pod per replica, no co-location).  used_g sums the demand of every placed pod of the group.  A role with C >= 0
 // makes one job per co-location domain D_r its row's placed replicas chose; its unplaced replicas make none.
-// cm != nullptr: the rows of a committed batch (§3.14, rp == nullptr): every job's room is counted after the whole
+// cm != nullptr: the rows of a committed batch (§3.14, and §3.15 with rp): every job's room is counted after the whole
 // batch (one list `used` of every group's placements), and participating jobs test the owner the batch left on a node
-// (k_alternates_commit<cm_levels>, cm->g = n_groups).
+// (k_alternates_commit<cm_levels>, cm->g = n_groups; k_alternates_commit_coloc when a job has a co-location domain).
+// hc != nullptr: cm's dhead / dclaim are hc's lists, uploaded with the jobs.
 int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vector<AltRow>& list, const int32_t* gb,
                    const int32_t* rp, const int32_t* assign, const int32_t* status, const int32_t* domain,
-                   const RankReq& rk, const CommitDev* cm, bool cm_levels) {
+                   const RankReq& rk, const CommitDev* cm, bool cm_levels, const HostClaims* hc) {
   const int F = rk.n_alt;
   const int ng = gb[2];
   std::vector<int> r0((size_t)ng + 1, 0);        // first role of every group in rp
@@ -2180,7 +2189,7 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
       const int32_t* rec = group_rec(gb, g);
       int64_t i = pod0[g];
       for (int q = 0; q < rec[3]; ++q)
-        for (int k = 0; k < gb[rec[4] + 4 * q + 1]; ++k, ++i)
+        for (int64_t k = 0; k < (int64_t)gb[rec[4] + 4 * q + 1] * (rp ? rp[2 * (r0[g] + q)] : 1); ++k, ++i)
           if (assign[i] >= 0) tmp.push_back(make_int2(assign[i], gb[rec[4] + 4 * q + 2]));
     }
     std::sort(tmp.begin(), tmp.end(), [](int2 a, int2 b2) { return a.x < b2.x; });
@@ -2243,6 +2252,7 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
         if (assign[p] >= 0 && dc[assign[p]] == d) add(p, S);
       j.nrep = (int)own.size() - j.rep0;
       jobs.push_back(j);
+      if (cm) gids.push_back(rec[0]);
       coloc = true;
     }
   }
@@ -2251,7 +2261,10 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
   if (smem > kFastSmemMax) return fail(RBGTOPO_ELIMIT, "ranked placement: %d nodes exceed the room bitmap", c->topo.n);
   static_assert(sizeof(AltJob) % 4 == 0, "jobs are staged as words");
   const size_t w_jobs = jobs.size() * (sizeof(AltJob) / 4), w_used = used.size() * 2, w_own = own.size();
-  const size_t w_in = w_jobs + w_used + w_own + gids.size(), w_out = own.size() * (size_t)(1 + 2 * F);
+  // hc: dhead, then dclaim 8-byte aligned, after the gids
+  const size_t o_dhead = w_jobs + w_used + w_own + gids.size();
+  const size_t o_dclaim = hc ? (o_dhead + hc->dhead.size() + 1) & ~(size_t)1 : o_dhead;
+  const size_t w_in = hc ? o_dclaim + 2 * hc->dclaim.size() : o_dhead, w_out = own.size() * (size_t)(1 + 2 * F);
   cudaStream_t s = stream_of(c, b);
   CK(b->alt.reserve(w_in + w_out));
   CK(b->h_alt.reserve(w_in + w_out));
@@ -2260,12 +2273,25 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
   memcpy(h + w_jobs, used.data(), w_used * 4);
   memcpy(h + w_jobs + w_used, own.data(), w_own * 4);
   memcpy(h + w_jobs + w_used + w_own, gids.data(), gids.size() * 4);
+  if (hc) {
+    memcpy(h + o_dhead, hc->dhead.data(), hc->dhead.size() * 4);
+    memcpy(h + o_dclaim, hc->dclaim.data(), hc->dclaim.size() * 8);
+  }
   int* d = b->alt.p;
   CK(cudaMemcpyAsync(d, h, w_in * 4, cudaMemcpyHostToDevice, s));
-  if (cm)
+  CommitDev cmd = cm ? *cm : CommitDev{};
+  if (hc) {
+    cmd.dhead = d + o_dhead;
+    cmd.dclaim = reinterpret_cast<const int2*>(d + o_dclaim);
+  }
+  if (cm && coloc)
+    k_alternates_commit_coloc<<<(unsigned)jobs.size(), ALT_THREADS, smem, s>>>(
+        topo_dev(c), rows, reinterpret_cast<const AltJob*>(d), reinterpret_cast<const int2*>(d + w_jobs),
+        d + w_jobs + w_used, F, d + w_in, cmd, d + w_jobs + w_used + w_own);
+  else if (cm)
     (cm_levels ? k_alternates_commit<true> : k_alternates_commit<false>)<<<(unsigned)jobs.size(), ALT_THREADS, smem, s>>>(
         topo_dev(c), rows, reinterpret_cast<const AltJob*>(d), reinterpret_cast<const int2*>(d + w_jobs),
-        d + w_jobs + w_used, F, d + w_in, *cm, d + w_jobs + w_used + w_own);
+        d + w_jobs + w_used, F, d + w_in, cmd, d + w_jobs + w_used + w_own);
   else
     (coloc ? k_alternates<true> : k_alternates<false>)<<<(unsigned)jobs.size(), ALT_THREADS, smem, s>>>(
         topo_dev(c), rows, reinterpret_cast<const AltJob*>(d), reinterpret_cast<const int2*>(d + w_jobs),
@@ -3660,12 +3686,22 @@ int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t*
 // (group, wave) that placed a replica is scored again as a step batch — the snapshot's scores, `need` over the
 // replicas still unplaced at that wave, the group's earlier waves as anchors — without consumed records and without
 // the exclusive flag: room and owner are tested by k_alternates_commit after the whole batch, against the final claims
-// in `cm`.  A batch whose rows exceed kReplayRows is scored and ranked in chunks of steps.  status / domain not null.
+// in `cm`.  A batch whose rows exceed kReplayBytes is scored and ranked in chunks of steps.  status / domain not null.
+// rp != nullptr: a committed leader-worker batch (§3.15): the (S, C) table of place_groups_lw, pod waves (lw_wave),
+// role counts, `need`, anchors and rows in pods; hc: its owner claims (HostClaims).
+int lw_wave(const int32_t* roles, int q, const int32_t* rp, int cr, int taken, int (*w)[3]);
 constexpr long long kReplayBytes = 1LL << 30;
-int rank_committed(rbgtopo_ctx* c, Batch* b, const int32_t* gb, const int32_t* assign, const int32_t* status,
-                   const int32_t* domain, const CommitDev& cm, bool lv, const RankReq& rk, int* launches) {
+int rank_committed(rbgtopo_ctx* c, Batch* b, const int32_t* gb, const int32_t* rp, const int32_t* assign,
+                   const int32_t* status, const int32_t* domain, const CommitDev& cm, bool lv, const RankReq& rk,
+                   int* launches, const HostClaims* hc = nullptr) {
   const int ng = gb[2];
-  alt_clear(rk, 0, gb[4]);
+  std::vector<int64_t> pod0((size_t)ng + 1, 0);  // first pod of every group in assign
+  for (int g = 0, r0 = 0; g < ng; ++g) {
+    const int32_t* rec = group_rec(gb, g);
+    pod0[g + 1] = pod0[g];
+    for (int q = 0; q < rec[3]; ++q, ++r0) pod0[g + 1] += (int64_t)gb[rec[4] + 4 * q + 1] * (rp ? rp[2 * r0] : 1);
+  }
+  alt_clear(rk, 0, rp ? pod0[ng] : gb[4]);
   cudaStream_t s = stream_of(c, b);
   CK(cudaStreamWaitEvent(s, c->base_ready, 0));  // the rows read base and free of the snapshot the rounds saw
   const int max_rows = (int)std::max<long long>(RBGTOPO_MAX_STEP_ROLES, kReplayBytes / 4 / c->slab_stride);
@@ -3690,54 +3726,62 @@ int rank_committed(rbgtopo_ctx* c, Batch* b, const int32_t* gb, const int32_t* a
     blob[5] = rowacc;
     int r2 = stage_into(c, b, blob.data(), (int64_t)blob.size());
     if (!r2) r2 = launch_score(c, b, s);
-    if (!r2) r2 = run_alternates(c, b, b->matrix.p, list, gb, nullptr, assign, status, domain, rk, &cm, lv);
+    if (!r2) r2 = run_alternates(c, b, b->matrix.p, list, gb, rp, assign, status, domain, rk, &cm, lv, hc);
     *launches += 2;
     tab.clear(); data.clear(); list.clear();
     ns = racc = rowacc = 0;
     return r2;
   };
-  for (int g = 0; g < ng && !rc; ++g) {
+  for (int g = 0, r0 = 0; g < ng && !rc; r0 += group_rec(gb, g)[3], ++g) {
     if (status[g] == RBGTOPO_GANG_FAILED) continue;
     const int32_t* rec = group_rec(gb, g);
     const int q = rec[3];
     const int32_t* roles = gb + rec[4];
     const int32_t* pair = gb + rec[5];
-    int ord0[RBGTOPO_MAX_GROUP_ROLES], unplaced[RBGTOPO_MAX_GROUP_ROLES];
-    for (int k = 0, acc = 0; k < q; ++k) { ord0[k] = acc; acc += roles[4 * k + 1]; unplaced[k] = roles[4 * k + 1]; }
+    const int32_t* grp = rp ? rp + 2LL * r0 : nullptr;
+    int S[RBGTOPO_MAX_GROUP_ROLES], ord0[RBGTOPO_MAX_GROUP_ROLES], unplaced[RBGTOPO_MAX_GROUP_ROLES];  // in pods
+    for (int k = 0, acc = 0; k < q; ++k) {
+      S[k] = grp ? grp[2 * k] : 1;
+      ord0[k] = acc;
+      unplaced[k] = roles[4 * k + 1] * S[k];
+      acc += unplaced[k];
+    }
     anchors.assign(gb + rec[7], gb + rec[7] + 3LL * rec[6]);
-    walk_waves(roles, q, [&](int, const PlanWave& w) {
+    // one wave: (role, first replica, replicas) per role row; pods of role ri from pod0[g] + ord0[ri] + first * S[ri]
+    auto wave = [&](int n_rows, const int (*w)[3]) {
       if (rc) return;
+      auto first = [&](int p) { return pod0[g] + ord0[w[p][0]] + (int64_t)w[p][1] * S[w[p][0]]; };
       bool any = false;
-      for (int p = 0; p < w.n; ++p)
-        for (int k = 0; k < w.count[p]; ++k) any |= assign[rec[8] + ord0[w.role[p]] + w.first[p] + k] >= 0;
+      for (int p = 0; p < n_rows; ++p)
+        for (int k = 0; k < w[p][2] * S[w[p][0]]; ++k) any |= assign[first(p) + k] >= 0;
       if (any) {
-        if (rowacc + w.n > max_rows) rc = flush();
+        if (rowacc + n_rows > max_rows) rc = flush();
         if (rc) return;
         int32_t st[RBGTOPO_STEP_WORDS] = {0};
         st[0] = rec[0];
         st[2] = -1;
-        st[3] = w.n;
+        st[3] = n_rows;
         while (data.size() & 3) data.push_back(0);
         st[4] = (int32_t)data.size();
         int n = 0;
-        for (int p = 0; p < w.n; ++p) {
-          const int ri = w.role[p];
+        for (int p = 0; p < n_rows; ++p) {
+          const int ri = w[p][0], pods = w[p][2] * S[ri];
           int need = 0;
           for (int k = 0; k < q; ++k)
             if (pair[ri * q + k] > 0) need += unplaced[k];
-          data.push_back(w.count[p]);
+          data.push_back(pods);
           data.push_back(roles[4 * ri + 2]);
           data.push_back(std::min(need, RBGTOPO_NEED_CAP));
           data.push_back(0);
-          n += w.count[p];
-          const int rep0 = rec[8] + ord0[ri] + w.first[p];
+          n += pods;
+          const int64_t rep0 = first(p);
           bool placed = false;
-          for (int k = 0; k < w.count[p]; ++k) placed |= assign[rep0 + k] >= 0;
-          if (placed) list.push_back(AltRow{rowacc + p, g, ri, rep0, w.count[p]});
+          for (int k = 0; k < pods; ++k) placed |= assign[rep0 + k] >= 0;
+          if (placed) list.push_back(AltRow{rowacc + p, g, ri, (int)rep0, pods});
         }
         st[5] = q;
         st[6] = (int32_t)data.size();
-        for (int p = 0; p < w.n; ++p) data.insert(data.end(), pair + w.role[p] * q, pair + (w.role[p] + 1) * q);
+        for (int p = 0; p < n_rows; ++p) data.insert(data.end(), pair + w[p][0] * q, pair + (w[p][0] + 1) * q);
         st[7] = (int32_t)(anchors.size() / 3);
         st[8] = (int32_t)data.size();
         data.insert(data.end(), anchors.begin(), anchors.end());
@@ -3748,16 +3792,29 @@ int rank_committed(rbgtopo_ctx* c, Batch* b, const int32_t* gb, const int32_t* a
         tab.insert(tab.end(), st, st + RBGTOPO_STEP_WORDS);
         ++ns;
         racc += n;
-        rowacc += w.n;
+        rowacc += n_rows;
       }
-      for (int p = 0; p < w.n; ++p)  // the wave's placements: anchors of the later waves
-        for (int k = 0; k < w.count[p]; ++k) {
-          const int node = assign[rec[8] + ord0[w.role[p]] + w.first[p] + k];
+      for (int p = 0; p < n_rows; ++p)  // the wave's placements: anchors of the later waves
+        for (int k = 0; k < w[p][2] * S[w[p][0]]; ++k) {
+          const int node = assign[first(p) + k];
           if (node < 0) continue;
-          anchors.push_back(node); anchors.push_back(w.role[p]); anchors.push_back(1);
-          unplaced[w.role[p]] -= 1;
+          anchors.push_back(node); anchors.push_back(w[p][0]); anchors.push_back(1);
+          unplaced[w[p][0]] -= 1;
         }
-    });
+    };
+    int w[RBGTOPO_MAX_STEP_ROLES][3];
+    if (grp) {  // pod waves, as place_groups_lw staged them
+      for (int cr = 0, taken = 0, P; (P = lw_wave(roles, q, grp, cr, taken, w)) > 0;) {
+        wave(P, w);
+        cr = w[P - 1][0];
+        taken = w[P - 1][1] + w[P - 1][2];
+      }
+    } else {
+      walk_waves(roles, q, [&](int, const PlanWave& pw) {
+        for (int p = 0; p < pw.n; ++p) { w[p][0] = pw.role[p]; w[p][1] = pw.first[p]; w[p][2] = pw.count[p]; }
+        wave(pw.n, w);
+      });
+    }
   }
   if (!rc) rc = flush();
   return rc;
@@ -3944,7 +4001,7 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
   int rank_launches = 0;
   if (rk && n0 > 0) {
     cm.g = ng;
-    rc = rank_committed(c, b, gb, assign, status, domain, cm, lv, *rk, &rank_launches);
+    rc = rank_committed(c, b, gb, nullptr, assign, status, domain, cm, lv, *rk, &rank_launches);
     if (rc) {
       cudaStreamSynchronize(s);
       release_batch(c, b);
@@ -4277,6 +4334,8 @@ struct LwClaims {
 // rounds != nullptr: the committed form (§3.13).  A round runs the wave loop for groups [lo, ng); group g sees the
 // claims of groups < g as the previous round left them (final below lo).  c = the lowest group whose claims changed:
 // groups <= c saw their final input, the next round starts at c + 1, and a round that changes nothing ends the call.
+// Both: the committed ranked form (§3.15).  The rounds keep no rows (a re-run would keep its rows again); once they
+// converge, rank_committed replays the rows of every group's final run and ranks them after the whole batch.
 int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
                     int32_t* assign, int32_t* status, int32_t* domain, const RankReq* rk = nullptr,
                     int32_t* rounds = nullptr) {
@@ -4321,11 +4380,12 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
     while (r.cur_role < r.q && r.roles[4 * r.cur_role + 1] == 0) ++r.cur_role;
     for (long long k = pod0[g]; k < pod0[g + 1]; ++k) assign[k] = -1;
   };
-  std::vector<AltRow> kept;  // rk: the (wave, role) rows that placed a pod, in b->lw_kept
+  const bool keep = rk && !rounds;
+  std::vector<AltRow> kept;  // keep: the (wave, role) rows that placed a pod, in b->lw_kept
   size_t kept_cap = 0, kept_used = 0;
   for (int g = 0; g < ng; ++g) {
     init_run(g);
-    if (rk) kept_cap += lw_role_rows(runs[g].roles, runs[g].q, runs[g].rp);
+    if (keep) kept_cap += lw_role_rows(runs[g].roles, runs[g].q, runs[g].rp);
   }
   std::vector<LwClaims> claims(rounds ? ng : 0);  // committed: every group's claims as the latest round left them
   std::vector<int> dom_ptr, dom_nodes;             // committed: the nodes of every level-0 domain
@@ -4344,7 +4404,7 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
   rc = acquire_batch(c, &b);
   if (rc) return rc;
   cudaStream_t s = stream_of(c, b);
-  if (rk) {
+  if (keep) {
     cudaError_t e = b->lw_kept.reserve(std::max<size_t>(1, kept_cap) * (size_t)c->slab_stride);
     if (e != cudaSuccess) {
       release_batch(c, b);
@@ -4478,7 +4538,7 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
       }();
       if (!rc) rc = fetch_batch(c, b, w_assign.data(), w_status.data(), w_domain.data());
       const size_t slot0 = kept_used;  // this wave's rows in b->lw_kept, in matrix order
-      if (!rc && rk) {
+      if (!rc && keep) {
         const size_t stride = (size_t)c->slab_stride;
         cudaError_t e = slot0 + rowacc <= kept_cap ? cudaMemcpyAsync(b->lw_kept.p + slot0 * stride, b->matrix.p,
                                                                       (size_t)rowacc * stride * 4, cudaMemcpyDeviceToDevice, s)
@@ -4513,7 +4573,7 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
             r.consumed[node] += r.roles[4 * ri + 2];
             r.unplaced[ri] -= 1;
           }
-          if (rk && placed) {
+          if (keep && placed) {
             const int row = blob[RBGTOPO_HDR_WORDS + (size_t)i * RBGTOPO_STEP_WORDS + 13] + p;  // in this wave's matrix
             kept.push_back(AltRow{(int)slot0 + row, active[i], ri, (int)first, r.w[p][2] * S});
           }
@@ -4567,6 +4627,24 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
     }
   }
   if (rounds) *rounds = n_rounds;
+  if (!rc && rk && rounds) {  // the claims are final now: level-0 owner lists for commit_owner<false>, then the replay
+    HostClaims hc;
+    hc.dhead.assign((size_t)T.n_domains, -1);
+    hc.dclaim.assign((size_t)std::max(ng, 1), make_int2(-1, -1));
+    for (int g = 0; g < ng; ++g)
+      if (claims[g].dom >= 0) {
+        hc.dclaim[g] = make_int2(claims[g].gid, hc.dhead[claims[g].dom]);
+        hc.dhead[claims[g].dom] = g;
+      }
+    CommitDev cm{};
+    cm.g = ng;
+    cm.occ = T.occ;
+    int rank_launches = 0;
+    rc = rank_committed(c, b, gb, rp, assign, status, domain, cm, false, *rk, &rank_launches, &hc);
+    total.launches += rank_launches;
+    std::lock_guard<std::mutex> g(c->stat_mu);
+    c->launches += rank_launches;
+  }
   if (!rc) {
     harvest_base_ms(c);
     std::lock_guard<std::mutex> g(c->stat_mu);
@@ -4575,7 +4653,7 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
   } else {
     cudaStreamSynchronize(s);
   }
-  if (!rc && rk) {  // the placements are final now: rank the kept rows
+  if (!rc && keep) {  // the placements are final now: rank the kept rows
     alt_clear(*rk, 0, total_pods);
     rc = run_alternates(c, b, b->lw_kept.p, kept, gb, rp, assign, status, domain, *rk);
     if (rc) cudaStreamSynchronize(s);
@@ -4685,6 +4763,31 @@ int32_t rbgtopo_place_groups_lw_committed(rbgtopo_ctx* c, const int32_t* gb, int
   CK(cudaSetDevice(c->cfg.device));
   int32_t r = 0;
   const int rc = place_groups_lw(c, gb, words, role_pods, role_pods_words, assign, status, domain, nullptr, &r);
+  if (rounds) *rounds = r;
+  return rc;
+}
+
+int32_t rbgtopo_place_groups_lw_committed_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words,
+                                                 const int32_t* role_pods, int64_t role_pods_words, int32_t n_alt,
+                                                 int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds,
+                                                 float* score, int32_t* alt_node, float* alt_score) {
+  if (rounds) *rounds = 0;
+  if (!c || !gb || !assign || !role_pods || !score || (n_alt > 0 && (!alt_node || !alt_score)))
+    return fail(RBGTOPO_EINVAL, "null argument");
+  if (n_alt < 0 || n_alt > RBGTOPO_MAX_ALTERNATES)
+    return fail(RBGTOPO_EINVAL, "n_alt %d outside [0, %d]", n_alt, RBGTOPO_MAX_ALTERNATES);
+  if (c->cfg.world > 1)
+    return fail(RBGTOPO_ELIMIT, "committed leader-worker placement needs world == 1: a rank holds only its slab of every dense row");
+  std::shared_lock<std::shared_mutex> lk(c->topo_mu);  // one snapshot for the rounds and the ranking
+  if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
+  CK(cudaSetDevice(c->cfg.device));
+  const int64_t ng = words >= RBGTOPO_HDR_WORDS ? std::max<int64_t>(0, std::min<int64_t>(gb[2], words / RBGTOPO_GROUP_WORDS)) : 0;
+  std::vector<int32_t> own_status, own_domain;  // status / domain may be NULL: the ranking still needs them
+  if (!status) { own_status.resize((size_t)ng + 1); status = own_status.data(); }
+  if (!domain) { own_domain.resize((size_t)ng + 1); domain = own_domain.data(); }
+  const RankReq rk{n_alt, score, alt_node, alt_score};
+  int32_t r = 0;
+  const int rc = place_groups_lw(c, gb, words, role_pods, role_pods_words, assign, status, domain, &rk, &r);
   if (rounds) *rounds = r;
   return rc;
 }

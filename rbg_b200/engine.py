@@ -63,6 +63,7 @@ class TopoPlacer:
         self.places_lw_ranked = True   # place_groups_lw_ranked: alternates for leader-worker pods (DESIGN.md §3.12)
         self.places_lw_committed = True  # place_groups_lw_committed: committed leader-worker batches (§3.13)
         self.places_committed_ranked = True  # place_groups_committed_ranked: alternates of committed batches (§3.14)
+        self.places_lw_committed_ranked = True  # place_groups_lw_committed_ranked: alternates of committed LW batches (§3.15)
         h = C.c_void_p()
         self._h = None
         self._check(self.lib.rbgtopo_create(C.byref(cfg), C.byref(h)))
@@ -244,6 +245,29 @@ class TopoPlacer:
         self._check(self.lib.rbgtopo_place_groups_lw_committed(self._h, _p(gb), len(gb), _p(rp), len(rp), _p(assign),
                                                                _p(status), _p(domain), C.byref(rounds)))
         return assign[:pods], status[:ng], domain[:ng], rounds.value
+
+    def place_groups_lw_committed_ranked(self, groups_blob: np.ndarray, role_pods, n_alt: int):
+        """place_groups_lw_committed plus ranked alternates per pod (DESIGN.md §3.15): returns (assign, status, domain,
+        rounds, score[P], alt_node[P, n_alt], alt_score[P, n_alt]).  assign / status / domain / rounds are those of
+        place_groups_lw_committed; alt_node[p] holds the next-best nodes of pod p's row that still have room once the
+        WHOLE batch is placed, that no exclusive claim of another gid in the batch forbids for a participating role,
+        and that keep the replica in its co-location domain (-1 / -inf where there are fewer), nothing for unplaced
+        pods and gang-failed groups."""
+        gb = _i32(groups_blob)
+        rp = _i32(np.asarray(role_pods, dtype=np.int64).reshape(-1))
+        ng, pods = int(gb[2]), self._lw_pods(gb, rp)
+        assign = np.empty(max(pods, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        rounds = C.c_int32()
+        score = np.empty(max(pods, 1), dtype=np.float32)
+        alt_node = np.empty((max(pods, 1), max(n_alt, 0)), dtype=np.int32)
+        alt_score = np.empty((max(pods, 1), max(n_alt, 0)), dtype=np.float32)
+        self._check(self.lib.rbgtopo_place_groups_lw_committed_ranked(
+            self._h, _p(gb), len(gb), _p(rp), len(rp), int(n_alt), _p(assign), _p(status), _p(domain), C.byref(rounds),
+            _p(score, _lib.f32p), _p(alt_node) if n_alt > 0 else None, _p(alt_score, _lib.f32p) if n_alt > 0 else None))
+        return (assign[:pods], status[:ng], domain[:ng], rounds.value, score[:pods], alt_node[:pods],
+                alt_score[:pods])
 
     def place_groups_lw_ranked(self, groups_blob: np.ndarray, role_pods, n_alt: int):
         """place_groups_lw plus ranked alternates per pod (DESIGN.md §3.12): returns (assign, status, domain,

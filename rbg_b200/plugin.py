@@ -312,7 +312,10 @@ class B200TopoPodGroupManager:
         one-pod replicas goes through rbgtopo_place_groups_committed_ranked (§3.14) when the placer has
         `places_committed_ranked`: same hints as rbgtopo_place_groups_committed, and alternates that still have
         room, and meet no exclusive claim of another gid, once the whole batch is placed.  A placer without it gives
-        committed hints without alternates.  Committed leader-worker batches carry no alternates.
+        committed hints without alternates.  A committed batch placed through rbgtopo_place_groups_lw_committed
+        (below) gets alternates from rbgtopo_place_groups_lw_committed_ranked (§3.15) when the placer has
+        `places_lw_committed_ranked`, for its one-pod and its multi-pod groups alike; a placer without it gives that
+        batch's hints without alternates.
         leader_worker: a group with a role of lws_size > 1 is placed through rbgtopo_place_groups_lw (DESIGN.md
         §3.11): every replica of such a role is lws_size pods, placed all or nothing, and the hints are keyed by pod
         name, "{rbg}-{role}-{ordinal}-{k}" (k = 0 the leader); standalone roles keep "{rbg}-{role}-{ordinal}".  A
@@ -437,7 +440,8 @@ class B200TopoPodGroupManager:
         domains the groups before it took, so the hints of one call never contradict each other (the controller
         passes the groups ordered by namespaced name).  With alternates, a committed batch of one-pod replicas gets
         them from place_groups_committed_ranked (§3.14) when the placer has `places_committed_ranked`: room and
-        exclusive claims counted after the whole batch.  Committed leader-worker batches carry no alternates."""
+        exclusive claims counted after the whole batch.  A committed batch with leader-worker groups gets them from
+        place_groups_lw_committed_ranked (§3.15) when the placer has `places_lw_committed_ranked`."""
         all_rbgs = rbgs
         lw_commit = self.lw_committed(rbgs, committed)
         rbgs, skipped = self._split_no_hint(rbgs, committed)
@@ -448,8 +452,13 @@ class B200TopoPodGroupManager:
             pods = [self.role_pods(g.rbg)[0] if self.is_leader_worker(g.rbg) else [(1, -1)] * len(g.rbg.roles)
                     for g in runs]
             role_pods = [pods[k][ri] for k, g in enumerate(runs) for ri in g.order]
-            assign, status, domain, _ = self.placer.place_groups_lw_committed(blob, role_pods)
-            return self._merge(all_rbgs, self._placements(runs, assign, status, domain, None, pods), skipped)
+            alt_node = None
+            if self.alternates > 0 and getattr(self.placer, "places_lw_committed_ranked", False):
+                assign, status, domain, _, _, alt_node, _ = self.placer.place_groups_lw_committed_ranked(
+                    blob, role_pods, self.alternates)
+            else:
+                assign, status, domain, _ = self.placer.place_groups_lw_committed(blob, role_pods)
+            return self._merge(all_rbgs, self._placements(runs, assign, status, domain, alt_node, pods), skipped)
         lw = [i for i, r in enumerate(rbgs) if self.is_leader_worker(r)]
         plain = [i for i, r in enumerate(rbgs) if not self.is_leader_worker(r)]
         done: List[Optional[Placement]] = [None] * len(rbgs)   # by position in rbgs
