@@ -44,7 +44,7 @@ def jobs_and_bytes(gblob, rp, assign, status, dom0):
         S = [int(rp[r0 + i][0]) for i in range(q)]
         C = [int(rp[r0 + i][1]) for i in range(q)]
         first = np.concatenate([[0], np.cumsum([roles[i, 1] * S[i] for i in range(q)])]).astype(int) + pod0
-        waves, cur, npod = [], [], 0   # (role, first replica, replicas), as lw_wave splits them
+        waves, cur, npod = [], [], 0   # (role, first replica, replicas), as next_wave splits them
         for ri in range(q):
             if cur and roles[ri, 0] != roles[cur[-1][0], 0]:
                 waves.append(cur)

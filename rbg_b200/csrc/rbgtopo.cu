@@ -236,7 +236,9 @@ struct Batch {
   DevBuf<int> lw, lw_cap;
   PinBuf<int> h_lw;
   DevBuf<unsigned long long> lw_best;
-  DevBuf<float> lw_kept;  // its ranked form: the dense rows of every (wave, role), kept across calls like the matrix
+  // ranked host-driven wave loops (place_groups_slow, place_groups_lw): the dense rows of every (wave, role), kept
+  // across calls like the matrix
+  DevBuf<float> kept;
   ~Batch() {
     if (stream) cudaStreamDestroy(stream);
     if (stream2) cudaStreamDestroy(stream2);
@@ -1799,22 +1801,230 @@ int32_t rbgtopo_score_assign(rbgtopo_ctx* c, const int32_t* blob, int64_t words,
 
 // ---- whole groups: level/wave loop on the host side of the ABI -------------
 namespace {
-struct GroupRun {
+const int32_t* group_rec(const int32_t* gb, int g) { return gb + RBGTOPO_HDR_WORDS + (int64_t)g * RBGTOPO_GROUP_WORDS; }
+
+// The GROUPS blob header and its group table: every group record lies inside the blob.
+bool groups_blob_ok(const int32_t* gb, int64_t words) {
+  return words >= RBGTOPO_HDR_WORDS && gb[0] == RBGTOPO_GROUPS_MAGIC && gb[1] == RBGTOPO_ABI_VERSION && gb[3] == words &&
+         gb[2] >= 0 && (int64_t)RBGTOPO_HDR_WORDS + (int64_t)gb[2] * RBGTOPO_GROUP_WORDS <= words;
+}
+// The same checks, reported.
+int check_groups_blob(const int32_t* gb, int64_t words) {
+  if (words < RBGTOPO_HDR_WORDS || gb[0] != RBGTOPO_GROUPS_MAGIC || gb[1] != RBGTOPO_ABI_VERSION || gb[3] != words)
+    return fail(RBGTOPO_EINVAL, "bad groups blob header");
+  if (gb[2] < 0 || (int64_t)RBGTOPO_HDR_WORDS + (int64_t)gb[2] * RBGTOPO_GROUP_WORDS > words)
+    return fail(RBGTOPO_EINVAL, "group table exceeds blob");
+  return RBGTOPO_OK;
+}
+
+// Per group of a GROUPS blob: its first role in a role_pods table (r0) and its first pod in assign (pod0); index
+// n_groups holds the totals.  rp: the (S, C) table of place_groups_lw (§3.11), or nullptr (one pod per replica).
+struct GroupOffsets {
+  std::vector<int> r0;
+  std::vector<int64_t> pod0;
+  GroupOffsets(const int32_t* gb, const int32_t* rp) : r0((size_t)gb[2] + 1, 0), pod0((size_t)gb[2] + 1, 0) {
+    for (int g = 0; g < gb[2]; ++g) {
+      const int32_t* rec = group_rec(gb, g);
+      r0[g + 1] = r0[g] + rec[3];
+      pod0[g + 1] = pod0[g];
+      for (int i = 0; i < rec[3]; ++i) pod0[g + 1] += (int64_t)gb[rec[4] + 4 * i + 1] * (rp ? rp[2 * (r0[g] + i)] : 1);
+    }
+  }
+  const int32_t* grp(const int32_t* rp, int g) const { return rp ? rp + 2LL * r0[g] : nullptr; }  // group g's (S, C)
+};
+
+// One wave of a group: (role, first replica, replicas) per role row.  <= RBGTOPO_MAX_STEP_ROLES entries, no heap.
+struct PlanWave {
+  int n = 0;
+  int role[RBGTOPO_MAX_STEP_ROLES], first[RBGTOPO_MAX_STEP_ROLES], count[RBGTOPO_MAX_STEP_ROLES];
+  void push(int r, int f, int c) { role[n] = r; first[n] = f; count[n] = c; ++n; }
+  int size() const { return n; }
+};
+struct WaveCursor {  // a group's next replica: replica `taken` of role `role`; role == q once every replica is in a wave
+  int role = 0, taken = 0;
+  void settle(const int32_t* roles, int q) {
+    while (role < q && roles[4 * role + 1] - taken <= 0) { ++role; taken = 0; }
+  }
+};
+
+// The wave rule of the host loops, the plan paths and plugin.py: a wave is the next replicas of the roles of one level,
+// in role order, at most RBGTOPO_MAX_STEP_ROLES role rows and RBGTOPO_MAX_STEP_REPLICAS pods, a replica's S pods never
+// split.  rp: the group's (S, C) per role (§3.11), nullptr = one pod per replica.  Fills w, moves cur past it and
+// returns its role rows (0: no replica left).
+inline int next_wave(const int32_t* roles, int q, const int32_t* rp, WaveCursor& cur, PlanWave& w) {
+  w.n = 0;
+  cur.settle(roles, q);
+  if (cur.role >= q) return 0;
+  const int level = roles[4 * cur.role];
+  int n = 0;
+  while (cur.role < q && roles[4 * cur.role] == level && w.n < RBGTOPO_MAX_STEP_ROLES) {
+    const int left = roles[4 * cur.role + 1] - cur.taken;
+    if (left <= 0) { ++cur.role; cur.taken = 0; continue; }
+    const int S = rp ? rp[2 * cur.role] : 1;
+    const int take = std::min(left, (RBGTOPO_MAX_STEP_REPLICAS - n) / S);
+    if (take == 0) break;
+    w.push(cur.role, cur.taken, take);
+    n += take * S;
+    cur.taken += take;
+    if (cur.taken == roles[4 * cur.role + 1]) { ++cur.role; cur.taken = 0; }
+  }
+  cur.settle(roles, q);
+  return w.n;
+}
+
+// Static wave structure of a group: calls f(index, wave) per wave, returns the count.
+extern "C++" {
+template <class F>
+inline int walk_waves(const int32_t* roles, int q, const int32_t* rp, F&& f) {
+  WaveCursor cur;
+  PlanWave w;
+  int nw = 0;
+  while (next_wave(roles, q, rp, cur, w) > 0) f(nw++, w);
+  return nw;
+}
+}  // extern "C++"
+int gen_waves(const int32_t* roles, int q, PlanWave* out) {  // out == nullptr: count only
+  return walk_waves(roles, q, nullptr, [out](int i, const PlanWave& w) { if (out) out[i] = w; });
+}
+
+// One group while a host-driven loop places its waves (or rank_committed replays them).  Counts are in pods: S pods per
+// replica from rp (place_groups_lw), one without it.
+struct HostRun {
   const int32_t* rec = nullptr;
   const int32_t* roles = nullptr;  // q x (level, pending, demand, role_flags)
   const int32_t* pair = nullptr;   // q x q
-  int q = 0;
-  int cur_role = 0, cur_taken = 0;  // wave cursor
-  int fixed_domain = -1;
-  int status = 0;
+  const int32_t* rp = nullptr;     // (S, C) per role, or nullptr
+  int q = 0, fixed_domain = -1, status = RBGTOPO_PLACED_ALL;
   bool failed = false;
-  std::vector<int> unplaced;        // per role
-  std::vector<int32_t> anchors;     // (node, role, count)*
-  std::vector<int32_t> consumed;    // (node, amount)*
-  // current wave
-  std::vector<int> w_role, w_first, w_count;
-  bool done() const { return failed || cur_role >= q; }
+  int64_t pod0 = 0, pods = 0;                   // the group's pods in assign
+  int ord0[RBGTOPO_MAX_GROUP_ROLES] = {0};      // first pod of every role inside the group's range
+  int unplaced[RBGTOPO_MAX_GROUP_ROLES] = {0};  // pods
+  WaveCursor cur;
+  PlanWave w;                         // the wave in flight
+  std::vector<int32_t> anchors;       // (node, role, count)*
+  std::vector<int32_t> consumed;      // place_groups_slow: (node, amount)*, one per placed replica
+  std::map<int, int> taken;           // place_groups_lw: node -> amount (committed: earlier groups' claims included)
+  std::vector<int32_t> owner_claims;  // committed, exclusive group: (node, claim gid)* of claimed domains, by node
+  HostRun() = default;
+  HostRun(const int32_t* gb, int g, const int32_t* grp, int64_t first_pod)
+      : rec(group_rec(gb, g)), roles(gb + rec[4]), pair(gb + rec[5]), rp(grp), q(rec[3]), fixed_domain(rec[2]),
+        pod0(first_pod) {
+    for (int i = 0; i < q; ++i) {
+      ord0[i] = (int)pods;
+      unplaced[i] = roles[4 * i + 1] * S(i);
+      pods += unplaced[i];
+    }
+    anchors.assign(gb + rec[7], gb + rec[7] + 3LL * rec[6]);
+    cur.settle(roles, q);
+  }
+  int S(int ri) const { return rp ? rp[2 * ri] : 1; }
+  bool done() const { return failed || cur.role >= q; }
+  // The group's results once its waves are placed: a failed gang places nothing.
+  void results(int g, int32_t* assign, int32_t* status_out, int32_t* domain_out) const {
+    if (failed) {
+      for (int64_t k = pod0; k < pod0 + pods; ++k) assign[k] = -1;
+      if (status_out) status_out[g] = RBGTOPO_GANG_FAILED;
+      if (domain_out) domain_out[g] = -1;
+    } else {
+      if (status_out) status_out[g] = status;
+      if (domain_out) domain_out[g] = (rec[1] & RBGTOPO_STEP_EXCLUSIVE) ? fixed_domain : -1;
+    }
+  }
 };
+
+// A step blob built on the host: the step records in `tab`, their sections in `data` with offsets from the table's
+// end until build() lays out the blob.
+struct StepBlob {
+  std::vector<int32_t> tab, data, blob;
+  int ns = 0, racc = 0, rowacc = 0;
+  // One step of wave w of group r: role counts in pods, `need` over r.unplaced, r.anchors; role flags keep the
+  // role-exclusive bit when role_excl; n_consumed (node, amount) records from `consumed`.
+  void add(const HostRun& r, const PlanWave& w, int32_t flags, int32_t dom, int32_t level, bool role_excl,
+           const int32_t* consumed, int n_consumed) {
+    int32_t st[RBGTOPO_STEP_WORDS] = {0};
+    st[0] = r.rec[0];
+    st[1] = flags;
+    st[2] = dom;
+    st[3] = w.n;
+    while (data.size() & 3) data.push_back(0);  // role records are read as 16-byte vectors
+    st[4] = (int32_t)data.size();
+    int n = 0;
+    for (int p = 0; p < w.n; ++p) {
+      const int ri = w.role[p], pods = w.count[p] * r.S(ri);
+      int need = 0;
+      for (int j = 0; j < r.q; ++j)
+        if (r.pair[ri * r.q + j] > 0) need += r.unplaced[j];
+      data.push_back(pods);
+      data.push_back(r.roles[4 * ri + 2]);
+      data.push_back(std::min(need, RBGTOPO_NEED_CAP));
+      data.push_back(role_excl ? r.roles[4 * ri + 3] & RBGTOPO_ROLE_EXCLUSIVE : 0);
+      n += pods;
+    }
+    st[5] = r.q;
+    st[6] = (int32_t)data.size();
+    for (int p = 0; p < w.n; ++p) data.insert(data.end(), r.pair + w.role[p] * r.q, r.pair + (w.role[p] + 1) * r.q);
+    st[7] = (int32_t)(r.anchors.size() / 3);
+    st[8] = (int32_t)data.size();
+    data.insert(data.end(), r.anchors.begin(), r.anchors.end());
+    st[9] = n_consumed;
+    st[10] = (int32_t)data.size();
+    data.insert(data.end(), consumed, consumed + 2 * (size_t)n_consumed);
+    st[11] = n;
+    st[12] = racc;
+    st[13] = rowacc;
+    st[14] = level;
+    tab.insert(tab.end(), st, st + RBGTOPO_STEP_WORDS);
+    ++ns;
+    racc += n;
+    rowacc += w.n;
+  }
+  // header | step records | sections
+  const std::vector<int32_t>& build() {
+    const int32_t base = RBGTOPO_HDR_WORDS + ns * RBGTOPO_STEP_WORDS;  // a multiple of 4: role records stay aligned
+    blob.assign((size_t)base, 0);
+    for (int i = 0; i < ns; ++i) {
+      int32_t* st = blob.data() + RBGTOPO_HDR_WORDS + (size_t)i * RBGTOPO_STEP_WORDS;
+      memcpy(st, tab.data() + (size_t)i * RBGTOPO_STEP_WORDS, RBGTOPO_STEP_WORDS * 4);
+      for (int k : {4, 6, 8, 10}) st[k] += base;
+    }
+    blob.insert(blob.end(), data.begin(), data.end());
+    blob[0] = RBGTOPO_BLOB_MAGIC;
+    blob[1] = RBGTOPO_ABI_VERSION;
+    blob[2] = ns;
+    blob[3] = (int32_t)blob.size();
+    blob[4] = racc;
+    blob[5] = rowacc;
+    return blob;
+  }
+  void clear() {
+    tab.clear();
+    data.clear();
+    ns = racc = rowacc = 0;
+  }
+};
+
+// (wave, role) rows of group g (grp: as next_wave's rp): what a ranked host-driven loop may keep for it.
+size_t group_role_rows(const int32_t* gb, int g, const int32_t* grp) {
+  const int32_t* rec = group_rec(gb, g);
+  size_t n = 0;
+  walk_waves(gb + rec[4], rec[3], grp, [&](int, const PlanWave& w) { n += (size_t)w.n; });
+  return n;
+}
+// The ranked host-driven loops: the matrix is overwritten by every wave, so the wave's `rows` dense rows go to
+// b->kept at row *used first (cap rows reserved by reserve_kept).  The ranking runs once the placements are final.
+int reserve_kept(rbgtopo_ctx* c, Batch* b, size_t cap) {
+  const cudaError_t e = b->kept.reserve(std::max<size_t>(1, cap) * (size_t)c->slab_stride);
+  return e == cudaSuccess ? RBGTOPO_OK : fail(RBGTOPO_ECUDA, "rows of a ranked placement: %s", cudaGetErrorString(e));
+}
+int keep_wave_rows(rbgtopo_ctx* c, Batch* b, int rows, size_t cap, size_t* used) {
+  const size_t stride = (size_t)c->slab_stride;
+  const cudaError_t e = *used + rows <= cap ? cudaMemcpyAsync(b->kept.p + *used * stride, b->matrix.p, (size_t)rows * stride * 4,
+                                                              cudaMemcpyDeviceToDevice, stream_of(c, b))
+                                            : cudaErrorInvalidValue;
+  if (e != cudaSuccess) return fail(RBGTOPO_ECUDA, "keeping the dense rows of a wave: %s", cudaGetErrorString(e));
+  *used += (size_t)rows;
+  return RBGTOPO_OK;
+}
 
 // ---- ranked placement (rbgtopo_place_groups_ranked, DESIGN.md §3.10)
 struct RankReq {  // the ranked outputs of one call, indexed like assign
@@ -1825,14 +2035,6 @@ struct RankReq {  // the ranked outputs of one call, indexed like assign
 };
 struct AltRow {  // one role row of one wave: where its dense row is, and its replicas [rep0, rep0 + nrep) in assign order
   int row, group, role, rep0, nrep;
-};
-// Rows of the host-driven loop: the wave's matrix is overwritten by the next wave, so the row of every (wave, role)
-// that placed a replica is copied out first.  The ranking runs once the groups' placements are final.
-struct KeptRows {
-  const RankReq* rk = nullptr;
-  DevBuf<float> rows;  // [cap][slab_stride]
-  size_t cap = 0;
-  std::vector<AltRow> list;
 };
 // The level-0 owner claims of a committed leader-worker batch (§3.15), built on the host from its final claims in the
 // layout commit_owner<false> reads: dhead[d] = a group that reported domain d (-1 = none), dclaim[g] = {gid of group g,
@@ -1851,136 +2053,81 @@ void alt_clear(const RankReq& rk, int64_t first, int64_t count);
 // The host-driven wave loop: one batched launch pair per wave, placements fed back
 // through the host.  Exact for every case; used for the groups the device-resident
 // plan cannot finish (`only` != null: just those groups) and as its reference.
+// rk != nullptr: the ranked form; each wave's rows are kept, and ranked once the placements are final.
 static int32_t place_groups_slow(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign,
                                  int32_t* status, int32_t* domain, const std::vector<char>* only,
-                                 KeptRows* kept = nullptr) {
-  if (!c || !gb) return fail(RBGTOPO_EINVAL, "null argument");
-  if (words < RBGTOPO_HDR_WORDS || gb[0] != RBGTOPO_GROUPS_MAGIC || gb[1] != RBGTOPO_ABI_VERSION ||
-      gb[3] != words)
-    return fail(RBGTOPO_EINVAL, "bad groups blob header");
+                                 const RankReq* rk = nullptr) {
+  if (const int hrc = check_groups_blob(gb, words)) return hrc;
   const int ng = gb[2];
-  if (ng < 0 || (int64_t)RBGTOPO_HDR_WORDS + (int64_t)ng * RBGTOPO_GROUP_WORDS > words)
-    return fail(RBGTOPO_EINVAL, "group table exceeds blob");
   std::shared_lock<std::shared_mutex> lk(c->topo_mu);
   if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
-  if (kept && (size_t)((c->topo.n + 31) / 32) * 4 > kFastSmemMax)  // the snapshot may have changed since the direct pass
+  if (rk && (size_t)((c->topo.n + 31) / 32) * 4 > kFastSmemMax)  // the snapshot may have changed since the direct pass
     return fail(RBGTOPO_ELIMIT, "ranked placement: %d nodes exceed the room bitmap", c->topo.n);
   CK(cudaSetDevice(c->cfg.device));
   auto in = [&](long long off, long long cnt) { return off >= 0 && cnt >= 0 && off + cnt <= words; };
-  std::vector<GroupRun> runs(ng);
+  std::vector<HostRun> runs(ng);
   long long pacc = 0;
   for (int g = 0; g < ng; ++g) {
-    const int32_t* rec = gb + RBGTOPO_HDR_WORDS + (int64_t)g * RBGTOPO_GROUP_WORDS;
-    GroupRun& r = runs[g];
-    r.rec = rec;
-    r.q = rec[3];
-    if (r.q < 1 || r.q > RBGTOPO_MAX_GROUP_ROLES) return fail(RBGTOPO_ELIMIT, "group %d: %d roles", g, r.q);
-    if (!in(rec[4], 4LL * r.q) || !in(rec[5], (long long)r.q * r.q) || !in(rec[7], 3LL * rec[6]))
+    const int32_t* rec = group_rec(gb, g);
+    const int q = rec[3];
+    if (q < 1 || q > RBGTOPO_MAX_GROUP_ROLES) return fail(RBGTOPO_ELIMIT, "group %d: %d roles", g, q);
+    if (!in(rec[4], 4LL * q) || !in(rec[5], (long long)q * q) || !in(rec[7], 3LL * rec[6]))
       return fail(RBGTOPO_EINVAL, "group %d: section out of bounds", g);
-    r.roles = gb + rec[4];
-    r.pair = gb + rec[5];
-    r.fixed_domain = rec[2];
-    r.unplaced.resize(r.q);
+    const int32_t* roles = gb + rec[4];
     long long pend = 0;
-    for (int i = 0; i < r.q; ++i) {
-      if (r.roles[4 * i + 1] < 0 || (i && r.roles[4 * i] < r.roles[4 * (i - 1)]))
+    for (int i = 0; i < q; ++i) {
+      if (roles[4 * i + 1] < 0 || (i && roles[4 * i] < roles[4 * (i - 1)]))
         return fail(RBGTOPO_EINVAL, "group %d role %d: pending < 0 or levels not ascending", g, i);
-      r.unplaced[i] = r.roles[4 * i + 1];
-      pend += r.roles[4 * i + 1];
+      pend += roles[4 * i + 1];
     }
     if (rec[8] != pacc || rec[9] != pend) return fail(RBGTOPO_EINVAL, "group %d: bad assign_off/n_pending", g);
     pacc += pend;
-    r.anchors.assign(gb + rec[7], gb + rec[7] + 3LL * rec[6]);
-    while (r.cur_role < r.q && r.roles[4 * r.cur_role + 1] == 0) ++r.cur_role;
+    runs[g] = HostRun(gb, g, nullptr, rec[8]);
   }
   if (gb[4] != pacc) return fail(RBGTOPO_EINVAL, "total pending mismatch");
+  size_t kept_cap = 0, kept_used = 0;  // rk: the role rows of the groups placed here
   for (int g = 0; g < ng; ++g) {
     if (only && !(*only)[g]) {
-      runs[g].cur_role = runs[g].q;  // not ours: done from the start, results untouched
+      runs[g].cur.role = runs[g].q;  // not ours: done from the start, results untouched
       continue;
     }
     for (int k = 0; k < runs[g].rec[9]; ++k) assign[runs[g].rec[8] + k] = -1;
+    if (rk) kept_cap += group_role_rows(gb, g, nullptr);
   }
 
   Batch* b = nullptr;
   int rc = acquire_batch(c, &b);
   if (rc) return rc;
+  if (rk) rc = reserve_kept(c, b, kept_cap);
   rbgtopo_timing total{};
-  std::vector<int32_t> blob, w_assign, w_status, w_domain;
+  StepBlob sb;
+  std::vector<int32_t> w_assign, w_status, w_domain;
   std::vector<int> active;
-  while (true) {
+  std::vector<AltRow> kept;  // rk: the (wave, role) rows that placed a replica, in b->kept
+  while (!rc) {
     active.clear();
     for (int g = 0; g < ng; ++g)
       if (!runs[g].done()) active.push_back(g);
     if (active.empty()) break;
     // ---- build this wave's step blob
-    const int ns = (int)active.size();
-    blob.assign((size_t)RBGTOPO_HDR_WORDS + (size_t)ns * RBGTOPO_STEP_WORDS, 0);
-    int racc = 0, rowacc = 0;
-    for (int i = 0; i < ns; ++i) {
-      GroupRun& r = runs[active[i]];
-      r.w_role.clear(); r.w_first.clear(); r.w_count.clear();
-      const int level = r.roles[4 * r.cur_role];
-      int cr = r.cur_role, taken = r.cur_taken, n = 0;
-      while (cr < r.q && r.roles[4 * cr] == level && n < RBGTOPO_MAX_STEP_REPLICAS &&
-             (int)r.w_role.size() < RBGTOPO_MAX_STEP_ROLES) {
-        const int left = r.roles[4 * cr + 1] - taken;
-        if (left <= 0) { ++cr; taken = 0; continue; }
-        const int take = std::min(left, RBGTOPO_MAX_STEP_REPLICAS - n);
-        r.w_role.push_back(cr); r.w_first.push_back(taken); r.w_count.push_back(take);
-        n += take;
-        taken += take;
-        if (taken == r.roles[4 * cr + 1]) { ++cr; taken = 0; }
-      }
-      const int P = (int)r.w_role.size();
-      int32_t st[RBGTOPO_STEP_WORDS] = {0};
-      st[0] = r.rec[0];
-      st[1] = r.rec[1] & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG);  // as build_plan / k_expand_plan
-      st[2] = (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) ? r.fixed_domain : -1;
-      st[3] = P;
-      while (blob.size() & 3) blob.push_back(0);  // role records are read as 16-byte vectors
-      st[4] = (int32_t)blob.size();
-      for (int p = 0; p < P; ++p) {
-        const int ri = r.w_role[p];
-        int need = 0;
-        for (int q = 0; q < r.q; ++q)
-          if (r.pair[ri * r.q + q] > 0) need += r.unplaced[q];
-        need = std::min(need, RBGTOPO_NEED_CAP);
-        blob.push_back(r.w_count[p]);
-        blob.push_back(r.roles[4 * ri + 2]);
-        blob.push_back(need);
-        blob.push_back(r.roles[4 * ri + 3] & RBGTOPO_ROLE_EXCLUSIVE);
-      }
-      st[5] = r.q;
-      st[6] = (int32_t)blob.size();
-      for (int p = 0; p < P; ++p)
-        blob.insert(blob.end(), r.pair + r.w_role[p] * r.q, r.pair + (r.w_role[p] + 1) * r.q);
-      st[7] = (int32_t)(r.anchors.size() / 3);
-      st[8] = (int32_t)blob.size();
-      blob.insert(blob.end(), r.anchors.begin(), r.anchors.end());
-      st[9] = (int32_t)(r.consumed.size() / 2);
-      st[10] = (int32_t)blob.size();
-      blob.insert(blob.end(), r.consumed.begin(), r.consumed.end());
-      st[11] = n;
-      st[12] = racc;
-      st[13] = rowacc;
-      st[14] = r.rec[10];  // exclusive level
-      racc += n;
-      rowacc += P;
-      memcpy(blob.data() + RBGTOPO_HDR_WORDS + (size_t)i * RBGTOPO_STEP_WORDS, st, sizeof st);
+    sb.clear();
+    for (int g : active) {
+      HostRun& r = runs[g];
+      next_wave(r.roles, r.q, nullptr, r.cur, r.w);
+      sb.add(r, r.w, r.rec[1] & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG),  // as build_plan / k_expand_plan
+             (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) ? r.fixed_domain : -1, r.rec[10], true, r.consumed.data(),
+             (int)(r.consumed.size() / 2));
     }
-    blob[0] = RBGTOPO_BLOB_MAGIC;
-    blob[1] = RBGTOPO_ABI_VERSION;
-    blob[2] = ns;
-    blob[3] = (int32_t)blob.size();
-    blob[4] = racc;
-    blob[5] = rowacc;
-    w_assign.resize(racc);
+    const std::vector<int32_t>& blob = sb.build();
+    const int ns = sb.ns;
+    w_assign.resize(sb.racc);
     w_status.resize(ns);
     w_domain.resize(ns);
+    const size_t slot0 = kept_used;  // this wave's rows in b->kept, in matrix order
     rc = stage_into(c, b, blob.data(), (int64_t)blob.size());
     if (!rc) rc = run_batch(c, b, 1);
     if (!rc) rc = fetch_batch(c, b, w_assign.data(), w_status.data(), w_domain.data());
+    if (!rc && rk) rc = keep_wave_rows(c, b, sb.rowacc, kept_cap, &kept_used);
     if (rc) break;
     {
       std::lock_guard<std::mutex> g(c->stat_mu);
@@ -1991,20 +2138,17 @@ static int32_t place_groups_slow(rbgtopo_ctx* c, const int32_t* gb, int64_t word
       total.h2d_words += c->last.h2d_words;
     }
     // ---- absorb the placements
-    int off = 0;
+    int off = 0, row = 0;  // row: the role's dense row in this wave's matrix
     for (int i = 0; i < ns; ++i) {
-      GroupRun& r = runs[active[i]];
-      const bool excl = (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) != 0;
+      HostRun& r = runs[active[i]];
       bool any = false;
-      for (size_t p = 0; p < r.w_role.size(); ++p) {
-        const int ri = r.w_role[p];
-        int ord0 = 0;  // index of this role's first replica inside the group's assign range
-        for (int k = 0; k < ri; ++k) ord0 += r.roles[4 * k + 1];
-        const int row = blob[RBGTOPO_HDR_WORDS + (size_t)i * RBGTOPO_STEP_WORDS + 13] + (int)p;  // the role's dense row in this wave's matrix
+      for (int p = 0; p < r.w.n; ++p, ++row) {
+        const int ri = r.w.role[p];
+        const int64_t first = r.pod0 + r.ord0[ri] + r.w.first[p];
         bool placed = false;
-        for (int k = 0; k < r.w_count[p]; ++k, ++off) {
+        for (int k = 0; k < r.w.count[p]; ++k, ++off) {
           const int node = w_assign[off];
-          assign[r.rec[8] + ord0 + r.w_first[p] + k] = node;
+          assign[first + k] = node;
           if (node >= 0) {
             any = true;
             placed = true;
@@ -2013,51 +2157,26 @@ static int32_t place_groups_slow(rbgtopo_ctx* c, const int32_t* gb, int64_t word
             r.unplaced[ri] -= 1;
           }
         }
-        if (kept && placed && !rc) {
-          const size_t stride = (size_t)c->slab_stride, slot = kept->list.size();
-          cudaError_t e = slot < kept->cap ? cudaMemcpyAsync(kept->rows.p + slot * stride, b->matrix.p + (size_t)row * stride,
-                                                             stride * 4, cudaMemcpyDeviceToDevice, stream_of(c, b))
-                                           : cudaErrorInvalidValue;
-          if (e != cudaSuccess) rc = fail(RBGTOPO_ECUDA, "keeping a dense row: %s", cudaGetErrorString(e));
-          kept->list.push_back(AltRow{(int)slot, active[i], ri, r.rec[8] + ord0 + r.w_first[p], r.w_count[p]});
-        }
+        if (rk && placed) kept.push_back(AltRow{(int)slot0 + row, active[i], ri, (int)first, r.w.count[p]});
       }
-      if (excl && w_domain[i] >= 0 && any) r.fixed_domain = w_domain[i];
+      if ((r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) && w_domain[i] >= 0 && any) r.fixed_domain = w_domain[i];
       r.status = std::max(r.status, w_status[i]);
       if ((r.rec[1] & RBGTOPO_STEP_GANG) && w_status[i] != RBGTOPO_PLACED_ALL) r.failed = true;
-      // advance the cursor past this wave
-      const int last = (int)r.w_role.size() - 1;
-      r.cur_role = r.w_role[last];
-      r.cur_taken = r.w_first[last] + r.w_count[last];
-      if (r.cur_taken >= r.roles[4 * r.cur_role + 1]) { ++r.cur_role; r.cur_taken = 0; }
-      while (r.cur_role < r.q && r.roles[4 * r.cur_role + 1] == 0) ++r.cur_role;
     }
-    if (rc) break;
   }
   if (!rc) {
-    for (int g = 0; g < ng; ++g) {
-      if (only && !(*only)[g]) continue;
-      const GroupRun& r = runs[g];
-      const bool excl = (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) != 0;
-      if (r.failed) {  // gang: nothing of the group is placed
-        for (int k = 0; k < r.rec[9]; ++k) assign[r.rec[8] + k] = -1;
-        if (status) status[g] = RBGTOPO_GANG_FAILED;
-        if (domain) domain[g] = -1;
-      } else {
-        if (status) status[g] = r.status;
-        if (domain) domain[g] = excl ? r.fixed_domain : -1;
-      }
-    }
+    for (int g = 0; g < ng; ++g)
+      if (!only || (*only)[g]) runs[g].results(g, assign, status, domain);
     std::lock_guard<std::mutex> g(c->stat_mu);
     total.base_ms = c->topo.base_ms;
     c->last = total;
   } else {
     cudaStreamSynchronize(stream_of(c, b));
   }
-  if (!rc && kept) {  // the placements are final now: rank the kept rows
+  if (!rc && rk) {  // the placements are final now: rank the kept rows
     for (int g = 0; g < ng; ++g)
-      if (!only || (*only)[g]) alt_clear(*kept->rk, runs[g].rec[8], runs[g].rec[9]);
-    rc = run_alternates(c, b, kept->rows.p, kept->list, gb, nullptr, assign, status, domain, *kept->rk);
+      if (!only || (*only)[g]) alt_clear(*rk, runs[g].rec[8], runs[g].rec[9]);
+    rc = run_alternates(c, b, b->kept.p, kept, gb, nullptr, assign, status, domain, *rk);
     if (rc) cudaStreamSynchronize(stream_of(c, b));
   }
   release_batch(c, b);
@@ -2074,45 +2193,8 @@ static int32_t place_groups_slow(rbgtopo_ctx* c, const int32_t* gb, int64_t word
 // fails (non-gang groups with an unplaced replica) are re-run through the
 // host-driven loop afterwards (place_groups_slow) — rare, and exact either way.
 namespace {
-struct PlanWave {  // <= RBGTOPO_MAX_STEP_ROLES entries, no heap
-  int n = 0;
-  int role[RBGTOPO_MAX_STEP_ROLES], first[RBGTOPO_MAX_STEP_ROLES], count[RBGTOPO_MAX_STEP_ROLES];
-  void push(int r, int f, int c) { role[n] = r; first[n] = f; count[n] = c; ++n; }
-  int size() const { return n; }
-};
-
-// Static wave structure of a group: same rule as the host loop / plugin.py (a wave = the next
-// <= 32 replicas of <= 8 roles of one level).  Calls f(index, wave) per wave, returns the count.
-extern "C++" {
-template <class F>
-int walk_waves(const int32_t* roles, int q, F&& f) {
-  int cr = 0, taken = 0, nw = 0;
-  while (cr < q) {
-    if (roles[4 * cr + 1] - taken <= 0) { ++cr; taken = 0; continue; }
-    PlanWave w;
-    const int level = roles[4 * cr];
-    int n = 0;
-    while (cr < q && roles[4 * cr] == level && n < RBGTOPO_MAX_STEP_REPLICAS && w.size() < RBGTOPO_MAX_STEP_ROLES) {
-      const int left = roles[4 * cr + 1] - taken;
-      if (left <= 0) { ++cr; taken = 0; continue; }
-      const int take = std::min(left, RBGTOPO_MAX_STEP_REPLICAS - n);
-      w.push(cr, taken, take);
-      n += take;
-      taken += take;
-      if (taken == roles[4 * cr + 1]) { ++cr; taken = 0; }
-    }
-    f(nw, w);
-    ++nw;
-  }
-  return nw;
-}
-}  // extern "C++"
-int gen_waves(const int32_t* roles, int q, PlanWave* out) {  // out == nullptr: count only
-  return walk_waves(roles, q, [out](int i, const PlanWave& w) { if (out) out[i] = w; });
-}
 
 // ---- ranked placement (DESIGN.md §3.10): the role rows to rank and the kernel launch
-const int32_t* group_rec(const int32_t* gb, int g) { return gb + RBGTOPO_HDR_WORDS + (int64_t)g * RBGTOPO_GROUP_WORDS; }
 
 // Replicas (pods) [first, first + count) start with no score and no alternates (what an unplaced or gang-failed one
 // keeps).
@@ -2135,7 +2217,7 @@ int plan_alt_rows(const int32_t* gb, int g, const int32_t* assign, int row, std:
   int ord0[RBGTOPO_MAX_GROUP_ROLES];
   for (int k = 0, acc = 0; k < rec[3]; ++k) { ord0[k] = acc; acc += roles[4 * k + 1]; }
   const int row0 = row;
-  walk_waves(roles, rec[3], [&](int, const PlanWave& w) {
+  walk_waves(roles, rec[3], nullptr, [&](int, const PlanWave& w) {
     for (int p = 0; p < w.n; ++p, ++row) {
       const int rep0 = rec[8] + ord0[w.role[p]] + w.first[p];
       bool placed = false;
@@ -2144,14 +2226,6 @@ int plan_alt_rows(const int32_t* gb, int g, const int32_t* assign, int row, std:
     }
   });
   return row - row0;
-}
-
-// Number of (wave, role) rows of group g: what the host-driven loop may keep for it.
-size_t group_role_rows(const int32_t* gb, int g) {
-  const int32_t* rec = group_rec(gb, g);
-  size_t n = 0;
-  walk_waves(gb + rec[4], rec[3], [&](int, const PlanWave& w) { n += (size_t)w.n; });
-  return n;
 }
 
 // k_alternates over `list` (rows in `rows`, slab_stride floats apart) on the batch's stream, results scattered into
@@ -2168,14 +2242,7 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
                    const RankReq& rk, const CommitDev* cm, bool cm_levels, const HostClaims* hc) {
   const int F = rk.n_alt;
   const int ng = gb[2];
-  std::vector<int> r0((size_t)ng + 1, 0);        // first role of every group in rp
-  std::vector<int64_t> pod0((size_t)ng + 1, 0);  // first pod of every group in assign
-  for (int g = 0; g < ng; ++g) {
-    const int32_t* rec = group_rec(gb, g);
-    r0[g + 1] = r0[g] + rec[3];
-    pod0[g + 1] = pod0[g];
-    for (int q = 0; q < rec[3]; ++q) pod0[g + 1] += (int64_t)gb[rec[4] + 4 * q + 1] * (rp ? rp[2 * (r0[g] + q)] : 1);
-  }
+  const GroupOffsets off(gb, rp);
   const Topology& T = c->topo;
   std::vector<AltJob> jobs;
   std::vector<int2> used, tmp;
@@ -2187,9 +2254,10 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
     for (int g = 0; g < ng; ++g) {
       if (status[g] == RBGTOPO_GANG_FAILED) continue;
       const int32_t* rec = group_rec(gb, g);
-      int64_t i = pod0[g];
+      const int32_t* grp = off.grp(rp, g);
+      int64_t i = off.pod0[g];
       for (int q = 0; q < rec[3]; ++q)
-        for (int64_t k = 0; k < (int64_t)gb[rec[4] + 4 * q + 1] * (rp ? rp[2 * (r0[g] + q)] : 1); ++k, ++i)
+        for (int64_t k = 0; k < (int64_t)gb[rec[4] + 4 * q + 1] * (grp ? grp[2 * q] : 1); ++k, ++i)
           if (assign[i] >= 0) tmp.push_back(make_int2(assign[i], gb[rec[4] + 4 * q + 2]));
     }
     std::sort(tmp.begin(), tmp.end(), [](int2 a, int2 b2) { return a.x < b2.x; });
@@ -2202,11 +2270,11 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
     if (status[r.group] == RBGTOPO_GANG_FAILED) continue;
     const int32_t* rec = group_rec(gb, r.group);
     const int32_t* roles = gb + rec[4];
-    const int32_t* grp = rp ? rp + 2 * r0[r.group] : nullptr;
+    const int32_t* grp = off.grp(rp, r.group);
     auto it = cm ? placed.emplace(r.group, make_int2(0, (int)used.size())).first : placed.find(r.group);
     if (it == placed.end()) {  // (node, amount) per node the group's pods of this call took
       tmp.clear();
-      int64_t i = pod0[r.group];
+      int64_t i = off.pod0[r.group];
       for (int q = 0; q < rec[3]; ++q)
         for (int64_t k = 0; k < (int64_t)roles[4 * q + 1] * (grp ? grp[2 * q] : 1); ++k, ++i)
           if (assign[i] >= 0) tmp.push_back(make_int2(assign[i], roles[4 * q + 2]));
@@ -2327,11 +2395,8 @@ int rank_plan(rbgtopo_ctx* c, Batch* b, const int32_t* gb, const int32_t* assign
 // Builds the plan IN PLACE in b->h_in (pinned); *plan_words = its size.  The GROUPS blob is
 // fully validated here (ranges of every user-provided value), so staging may trust the plan.
 int build_plan(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int64_t* plan_words, Batch* b) {
-  if (words < RBGTOPO_HDR_WORDS || gb[0] != RBGTOPO_GROUPS_MAGIC || gb[1] != RBGTOPO_ABI_VERSION || gb[3] != words)
-    return fail(RBGTOPO_EINVAL, "bad groups blob header");
+  if (const int hrc = check_groups_blob(gb, words)) return hrc;
   const int ng = gb[2];
-  if (ng < 0 || (int64_t)RBGTOPO_HDR_WORDS + (int64_t)ng * RBGTOPO_GROUP_WORDS > words)
-    return fail(RBGTOPO_EINVAL, "group table exceeds blob");
   auto in = [&](long long off, long long cnt) { return off >= 0 && cnt >= 0 && off + cnt <= words; };
   static const bool prof = getenv("RBGTOPO_PROFILE_HOST") != nullptr;
   auto now = [] { return std::chrono::steady_clock::now(); };
@@ -2579,7 +2644,41 @@ struct TopoHost {
   const int* degp1 = nullptr;  // [n] deg + 1, or nullptr = all 1
   int max_degp1 = 1;
   long long wsum_max = 0;
+  long long row_w = RBGTOPO_SELF_W, amax_limit = 0;  // the §3.4 bound: exact while amax * row_w < 2^24, i.e. amax < amax_limit
+  void set_wsum(long long w) {
+    wsum_max = w;
+    row_w = w + RBGTOPO_SELF_W;
+    amax_limit = ((1LL << 24) + row_w - 1) / row_w;
+  }
 };
+// The snapshot's; levels >= 1 are placed when place_levels.
+TopoHost topo_host(const rbgtopo_ctx* c, bool place_levels) {
+  const Topology& T = c->topo;
+  TopoHost th;
+  th.n = T.n;
+  th.n_domains = T.n_domains;
+  th.n_levels = installed_levels(c);
+  th.place_levels = place_levels;
+  th.level_nd = T.lvl_nd.empty() ? nullptr : T.lvl_nd.data();
+  th.degp1 = T.h_degp1.data();
+  th.max_degp1 = T.max_degp1;
+  th.set_wsum(T.wsum_max);
+  return th;
+}
+// The arguments of the describe calls (exclusive levels unknown).
+int topo_host_args(int32_t n_nodes, int32_t n_domains, const int32_t* deg_plus1, int64_t wsum_max, TopoHost* th) {
+  th->n = n_nodes;
+  th->n_domains = n_domains;
+  th->degp1 = deg_plus1;
+  th->max_degp1 = 1;
+  if (deg_plus1)
+    for (int i = 0; i < n_nodes; ++i) {
+      if (deg_plus1[i] < 1) return fail(RBGTOPO_EINVAL, "deg_plus1[%d]", i);
+      th->max_degp1 = std::max(th->max_degp1, deg_plus1[i]);
+    }
+  th->set_wsum(wsum_max);
+  return RBGTOPO_OK;
+}
 // Fleets are made of a few role templates (an RBGSet fans ONE RoleBasedGroup out into N, rolebasedgroupset_controller.go:69-207):
 // what the plan geometry derives from a group's role table and pair matrix alone — validity, pending replicas, the
 // wave structure, per-wave sizes and the shape part of the exactness bound — is computed once per run of identical
@@ -2643,11 +2742,8 @@ using PlanMidHook = std::function<int(const PlanLayout&)>;
 int plan_geometry(const TopoHost& T, int lc, Batch* b, const int32_t* gb, int64_t words, int g_lo, int g_hi,
                   long long pacc0, bool with_blob, PlanLayout* L, const PlanMidHook& mid = nullptr) {
   b->perm_n = 0;
-  if (words < RBGTOPO_HDR_WORDS || gb[0] != RBGTOPO_GROUPS_MAGIC || gb[1] != RBGTOPO_ABI_VERSION || gb[3] != words)
-    return fail(RBGTOPO_EINVAL, "bad groups blob header");
+  if (const int hrc = check_groups_blob(gb, words)) return hrc;
   const int ng_all = gb[2];
-  if (ng_all < 0 || (int64_t)RBGTOPO_HDR_WORDS + (int64_t)ng_all * RBGTOPO_GROUP_WORDS > words)
-    return fail(RBGTOPO_EINVAL, "group table exceeds blob");
   if (g_hi < 0) g_hi = ng_all;
   if (g_lo < 0 || g_lo > g_hi || g_hi > ng_all) return fail(RBGTOPO_EINVAL, "internal: group range");
   const int ng = g_hi - g_lo;  // below, g is the index inside the range; blob records are g_lo + g
@@ -2703,7 +2799,7 @@ int plan_geometry(const TopoHost& T, int lc, Batch* b, const int32_t* gb, int64_
         if (roles[4 * i + 3] & ~RBGTOPO_ROLE_EXCLUSIVE) GROUP_FAIL(RBGTOPO_EINVAL, "group %d role %d: unknown role flags", g, i);
       for (int i = 0; i < q * q; ++i)
         if (gb[rec[5] + i] < 0 || gb[rec[5] + i] > kMaxExactTerm) GROUP_FAIL(RBGTOPO_EINVAL, "group %d: pair weight out of [0, 2^24]", g);
-      nw_g = walk_waves(roles, q, [&](int, const PlanWave& w) { rr_g += w.n; });
+      nw_g = walk_waves(roles, q, nullptr, [&](int, const PlanWave& w) { rr_g += w.n; });
       ShapeCache* v = sc_chk.victim();
       v->set(roles, gb + rec[5], q);
       v->pend = pend;
@@ -2837,10 +2933,9 @@ int plan_geometry(const TopoHost& T, int lc, Batch* b, const int32_t* gb, int64_
   }
   const auto p2 = now();
   // per-step sizes, patch capacity, exactness bound (per group, all its waves)
-  const long long row_w = T.wsum_max + RBGTOPO_SELF_W;
+  const long long row_w = T.row_w, amax_limit = T.amax_limit;
   const int max_degp1 = T.max_degp1;
   const int* const first_of = g_first.data();
-  const long long amax_limit = ((1LL << 24) + row_w - 1) / row_w;  // amax * row_w >= 2^24  <=>  amax >= limit
   auto size_group = [&](int g, bool report) -> int {
     const int32_t* rec = gb + RBGTOPO_HDR_WORDS + (int64_t)(g_lo + g) * RBGTOPO_GROUP_WORDS;
     const int q = rec[3], na = rec[6];
@@ -2891,7 +2986,7 @@ int plan_geometry(const TopoHost& T, int lc, Batch* b, const int32_t* gb, int64_
     bool cacheable = true;
     int placed[RBGTOPO_MAX_GROUP_ROLES] = {0};
     int i0 = 0;
-    const int nw = walk_waves(roles, q, [&](int w, const PlanWave& pw) {
+    const int nw = walk_waves(roles, q, nullptr, [&](int w, const PlanWave& pw) {
       if (rc) return;
       const int P = pw.size();
       int n = 0;
@@ -3022,17 +3117,8 @@ int plan_geometry(const TopoHost& T, int lc, Batch* b, const int32_t* gb, int64_
 int plan_stage(rbgtopo_ctx* c, Batch* b, const int32_t* gb, int64_t words, bool early_emit = false, int g_lo = 0, int g_hi = -1,
                long long pacc0 = 0, const int* dev_groups = nullptr, cudaEvent_t dev_groups_ready = nullptr) {
   NvtxRange nv("rbgtopo:plan_stage");
-  const Topology& T = c->topo;
-  if (!T.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
-  TopoHost th;
-  th.n = T.n;
-  th.n_domains = T.n_domains;
-  th.n_levels = installed_levels(c);
-  th.place_levels = places_levels(c);
-  th.level_nd = c->topo.lvl_nd.empty() ? nullptr : c->topo.lvl_nd.data();
-  th.degp1 = T.h_degp1.data();
-  th.max_degp1 = T.max_degp1;
-  th.wsum_max = T.wsum_max;
+  if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
+  const TopoHost th = topo_host(c, places_levels(c));
   PlanLayout L;
   cudaStream_t s = stream_of(c, b);
   // Runs inside plan_geometry as soon as the step numbering exists: first upload (GROUPS blob + the
@@ -3285,8 +3371,8 @@ struct ShapeFacts {
 // phase 1: the group record, role table and pair matrix (what the row table and the dense matrix depend on);
 // phase 2: the scheduled pods (ranges, neighbourhood sizes) and the exactness bound; phase 3 = both.
 // role_bound: the per-role wave bound of another wave rule (place_groups_lw: pods, §3.11) instead of the replica waves'.
-int group_facts(const TopoHost& T, const int32_t* gb, int64_t words, int g, bool report, long long amax_limit, long long row_w,
-                GroupFacts* out, int phase = 3, const long long* role_bound = nullptr) {
+int group_facts(const TopoHost& T, const int32_t* gb, int64_t words, int g, bool report, GroupFacts* out, int phase = 3,
+                const long long* role_bound = nullptr) {
   auto in = [&](long long off, long long cnt) { return off >= 0 && cnt >= 0 && off + cnt <= words; };
   const int32_t* rec = gb + RBGTOPO_HDR_WORDS + (int64_t)g * RBGTOPO_GROUP_WORDS;
   const int q = rec[3];
@@ -3330,7 +3416,7 @@ int group_facts(const TopoHost& T, const int32_t* gb, int64_t words, int g, bool
     for (int i = 0; i < q; ++i) w.role_bound[i] = 0;
     int placed[RBGTOPO_MAX_GROUP_ROLES] = {0};
     int i0 = 0;
-    w.nw = walk_waves(roles, q, [&](int, const PlanWave& pw) {
+    w.nw = walk_waves(roles, q, nullptr, [&](int, const PlanWave& pw) {
       const int P = pw.size();
       int n = 0;
       for (int k = 0; k < P; ++k) {
@@ -3385,8 +3471,8 @@ int group_facts(const TopoHost& T, const int32_t* gb, int64_t words, int g, bool
     for (int ri = 0; ri < q; ++ri) {
       if (roles[4 * ri + 1] <= 0) continue;  // a role without pending replicas has no row
       const long long amax = std::min(anch_w[ri] + (role_bound ? role_bound : sf->role_bound)[ri], sat);
-      if (amax >= amax_limit)
-        GROUP_FAIL(RBGTOPO_EINEXACT, "group %d role %d: max score bound >= 2^24 (anchor weight %lld x row weight %lld)", g, ri, amax, row_w);
+      if (amax >= T.amax_limit)
+        GROUP_FAIL(RBGTOPO_EINEXACT, "group %d role %d: max score bound >= 2^24 (anchor weight %lld x row weight %lld)", g, ri, amax, T.row_w);
     }
   out->pcp = pc;
   return RBGTOPO_OK;
@@ -3402,14 +3488,14 @@ struct DirectGeom {
 // pass 1: group records, role tables, pair matrices (per-shape caches), the prefix of the assignment offsets, and the
 // launch order of k_plan_group (perm[0 .. n0): groups with pending replicas, heaviest expected table first — the
 // weight is the number of closed neighbourhoods the table will hold: scheduled pods + replicas to place)
-int direct_pass1(const TopoHost& th, const int32_t* gb, int64_t words, int ng, long long amax_limit, long long row_w,
-                 std::vector<GroupFacts>& facts, int32_t* perm, DirectGeom* G) {
+int direct_pass1(const TopoHost& th, const int32_t* gb, int64_t words, int ng, std::vector<GroupFacts>& facts, int32_t* perm,
+                 DirectGeom* G) {
   facts.resize((size_t)ng);
   int first_bad = ng;
 #pragma omp parallel for schedule(static) num_threads(kHostThreads) reduction(min : first_bad) if (ng >= kHostParallelMinGroups && kHostThreads > 1)
   for (int g = 0; g < ng; ++g)
-    if (group_facts(th, gb, words, g, false, amax_limit, row_w, &facts[g], 1) != RBGTOPO_OK) first_bad = std::min(first_bad, g);
-  if (first_bad < ng) return group_facts(th, gb, words, first_bad, true, amax_limit, row_w, &facts[first_bad], 1);
+    if (group_facts(th, gb, words, g, false, &facts[g], 1) != RBGTOPO_OK) first_bad = std::min(first_bad, g);
+  if (first_bad < ng) return group_facts(th, gb, words, first_bad, true, &facts[first_bad], 1);
   long long pacc = 0, wmax = 1;
   for (int g = 0; g < ng; ++g) {
     const int32_t* rec = gb + RBGTOPO_HDR_WORDS + (int64_t)g * RBGTOPO_GROUP_WORDS;
@@ -3445,13 +3531,12 @@ int direct_pass1(const TopoHost& th, const int32_t* gb, int64_t words, int ng, l
 }
 // pass 2: scheduled pods (ranges, neighbourhood sizes), the exactness bound, the table capacity and with it the launch
 // geometry of k_plan_group (as plan_group_cfg)
-int direct_pass2(const TopoHost& th, const int32_t* gb, int64_t words, int ng, long long amax_limit, long long row_w,
-                 std::vector<GroupFacts>& facts, DirectGeom* G) {
+int direct_pass2(const TopoHost& th, const int32_t* gb, int64_t words, int ng, std::vector<GroupFacts>& facts, DirectGeom* G) {
   int first_bad = ng;
 #pragma omp parallel for schedule(static) num_threads(kHostThreads) reduction(min : first_bad) if (ng >= kHostParallelMinGroups && kHostThreads > 1)
   for (int g = 0; g < ng; ++g)
-    if (group_facts(th, gb, words, g, false, amax_limit, row_w, &facts[g], 2) != RBGTOPO_OK) first_bad = std::min(first_bad, g);
-  if (first_bad < ng) return group_facts(th, gb, words, first_bad, true, amax_limit, row_w, &facts[first_bad], 2);
+    if (group_facts(th, gb, words, g, false, &facts[g], 2) != RBGTOPO_OK) first_bad = std::min(first_bad, g);
+  if (first_bad < ng) return group_facts(th, gb, words, first_bad, true, &facts[first_bad], 2);
   for (int g = 0; g < ng; ++g)
     if (facts[g].nw > 0)
       G->max_cap = std::max(G->max_cap, (long long)facts[g].i0_last + facts[g].pcp + (long long)facts[g].i0_last * th.max_degp1);  // the last wave's table
@@ -3493,13 +3578,10 @@ int place_groups_direct(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_
   // world > 1: replicated selection (every rank places every group over all nodes; the dense matrix and its corrections
   // are limited to the rank's column slab by the kernels themselves), exactly as on the staged path
   if (kNoDirect || !kSerialPlan || kVerifyPlan || kPerWavePlan) return RBGTOPO_OK;
-  if (words < RBGTOPO_HDR_WORDS || gb[0] != RBGTOPO_GROUPS_MAGIC || gb[1] != RBGTOPO_ABI_VERSION || gb[3] != words ||
-      words > 0x3FFFFFFFLL)
-    return RBGTOPO_OK;  // the staged path reports what is wrong with the header
+  if (!groups_blob_ok(gb, words) || words > 0x3FFFFFFFLL) return RBGTOPO_OK;  // the staged path reports what is wrong
   const int ng = gb[2];
-  if (ng < 1 || (int64_t)RBGTOPO_HDR_WORDS + (int64_t)ng * RBGTOPO_GROUP_WORDS > words || ng >= kSplitMinGroups) return RBGTOPO_OK;
+  if (ng < 1 || ng >= kSplitMinGroups) return RBGTOPO_OK;
   NvtxRange nv("rbgtopo:place_groups_direct");
-  const Topology& T = c->topo;
   static const bool prof = kProfileHost;
   auto now = [] { return std::chrono::steady_clock::now(); };
   auto us = [](auto a, auto b2) { return std::chrono::duration<double, std::micro>(b2 - a).count(); };
@@ -3536,20 +3618,10 @@ int place_groups_direct(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_
 
   // ---- pass 1: group records, role tables, pair matrices (per-shape caches) — all the row table and the dense
   // matrix depend on; the launch order of k_plan_group from (scheduled pods + pending replicas) per group
-  TopoHost th;
-  th.n = T.n;
-  th.n_domains = T.n_domains;
-  th.n_levels = installed_levels(c);
-  th.place_levels = places_levels(c);
-  th.level_nd = c->topo.lvl_nd.empty() ? nullptr : c->topo.lvl_nd.data();
-  th.degp1 = T.h_degp1.data();
-  th.max_degp1 = T.max_degp1;
-  th.wsum_max = T.wsum_max;
-  const long long row_w = T.wsum_max + RBGTOPO_SELF_W;
-  const long long amax_limit = ((1LL << 24) + row_w - 1) / row_w;
+  const TopoHost th = topo_host(c, places_levels(c));
   static thread_local std::vector<GroupFacts> facts;
   DirectGeom G;
-  rc = direct_pass1(th, gb, words, ng, amax_limit, row_w, facts, b->h_in.p + perm_off, &G);
+  rc = direct_pass1(th, gb, words, ng, facts, b->h_in.p + perm_off, &G);
   if (rc) return done(rc);
   const long long total_r = G.total_r, rrows = G.rrows;
   const int n0 = G.n0, max_q = G.max_q;
@@ -3585,7 +3657,7 @@ int place_groups_direct(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_
   const auto t2b = now();
 
   // ---- pass 2: scheduled pods (ranges, neighbourhood sizes), exactness bound, table capacity
-  rc = direct_pass2(th, gb, words, ng, amax_limit, row_w, facts, &G);
+  rc = direct_pass2(th, gb, words, ng, facts, &G);
   if (rc) return done(rc);
   const int nth = G.nth, HT = G.HT, CAP = G.CAP;
   const size_t smem = G.smem;
@@ -3682,138 +3754,79 @@ int place_groups_direct(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_
 int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
                 long long* total_pods);
 
+// The §3.4 bound at one pod per replica: lw_validate's with (S, C) = (1, -1) for every role, which takes every mix of
+// unplaced earlier replicas a later wave can see (§3.10, §3.11 rule 7).  The group table is checked.
+int exact_one_pod(rbgtopo_ctx* c, const int32_t* gb, int64_t words) {
+  long long qsum = 0, pods = 0;
+  for (int g = 0; g < gb[2]; ++g) {
+    const int q = group_rec(gb, g)[3];
+    if (q < 1 || q > RBGTOPO_MAX_GROUP_ROLES) return fail(RBGTOPO_ELIMIT, "group %d: %d roles", g, q);
+    qsum += q;
+  }
+  std::vector<int32_t> unit(2 * (size_t)qsum);
+  for (size_t i = 0; i < unit.size(); i += 2) { unit[i] = 1; unit[i + 1] = -1; }
+  return lw_validate(c, gb, words, unit.data(), (int64_t)unit.size(), &pods);
+}
+
 // Ranked alternates of a committed batch (DESIGN.md §3.14), once its rounds have converged: the dense row of every
 // (group, wave) that placed a replica is scored again as a step batch — the snapshot's scores, `need` over the
 // replicas still unplaced at that wave, the group's earlier waves as anchors — without consumed records and without
 // the exclusive flag: room and owner are tested by k_alternates_commit after the whole batch, against the final claims
 // in `cm`.  A batch whose rows exceed kReplayBytes is scored and ranked in chunks of steps.  status / domain not null.
-// rp != nullptr: a committed leader-worker batch (§3.15): the (S, C) table of place_groups_lw, pod waves (lw_wave),
+// rp != nullptr: a committed leader-worker batch (§3.15): the (S, C) table of place_groups_lw, pod waves (next_wave),
 // role counts, `need`, anchors and rows in pods; hc: its owner claims (HostClaims).
-int lw_wave(const int32_t* roles, int q, const int32_t* rp, int cr, int taken, int (*w)[3]);
 constexpr long long kReplayBytes = 1LL << 30;
 int rank_committed(rbgtopo_ctx* c, Batch* b, const int32_t* gb, const int32_t* rp, const int32_t* assign,
                    const int32_t* status, const int32_t* domain, const CommitDev& cm, bool lv, const RankReq& rk,
                    int* launches, const HostClaims* hc = nullptr) {
   const int ng = gb[2];
-  std::vector<int64_t> pod0((size_t)ng + 1, 0);  // first pod of every group in assign
-  for (int g = 0, r0 = 0; g < ng; ++g) {
-    const int32_t* rec = group_rec(gb, g);
-    pod0[g + 1] = pod0[g];
-    for (int q = 0; q < rec[3]; ++q, ++r0) pod0[g + 1] += (int64_t)gb[rec[4] + 4 * q + 1] * (rp ? rp[2 * r0] : 1);
-  }
-  alt_clear(rk, 0, rp ? pod0[ng] : gb[4]);
+  const GroupOffsets off(gb, rp);
+  alt_clear(rk, 0, off.pod0[ng]);
   cudaStream_t s = stream_of(c, b);
   CK(cudaStreamWaitEvent(s, c->base_ready, 0));  // the rows read base and free of the snapshot the rounds saw
   const int max_rows = (int)std::max<long long>(RBGTOPO_MAX_STEP_ROLES, kReplayBytes / 4 / c->slab_stride);
-  std::vector<int32_t> tab, data, anchors;  // the chunk's step table, and its sections (offsets from the table's end)
+  StepBlob sb;
   std::vector<AltRow> list;
-  int ns = 0, racc = 0, rowacc = 0, rc = RBGTOPO_OK;
+  int rc = RBGTOPO_OK;
   auto flush = [&]() -> int {
-    if (ns == 0) return RBGTOPO_OK;
-    const int32_t base = RBGTOPO_HDR_WORDS + ns * RBGTOPO_STEP_WORDS;  // a multiple of 4: role records stay aligned
-    std::vector<int32_t> blob((size_t)base, 0);
-    for (int i = 0; i < ns; ++i) {
-      int32_t* st = tab.data() + (size_t)i * RBGTOPO_STEP_WORDS;
-      for (int k : {4, 6, 8, 10}) st[k] += base;
-    }
-    memcpy(blob.data() + RBGTOPO_HDR_WORDS, tab.data(), tab.size() * 4);
-    blob.insert(blob.end(), data.begin(), data.end());
-    blob[0] = RBGTOPO_BLOB_MAGIC;
-    blob[1] = RBGTOPO_ABI_VERSION;
-    blob[2] = ns;
-    blob[3] = (int32_t)blob.size();
-    blob[4] = racc;
-    blob[5] = rowacc;
+    if (sb.ns == 0) return RBGTOPO_OK;
+    const std::vector<int32_t>& blob = sb.build();
     int r2 = stage_into(c, b, blob.data(), (int64_t)blob.size());
     if (!r2) r2 = launch_score(c, b, s);
     if (!r2) r2 = run_alternates(c, b, b->matrix.p, list, gb, rp, assign, status, domain, rk, &cm, lv, hc);
     *launches += 2;
-    tab.clear(); data.clear(); list.clear();
-    ns = racc = rowacc = 0;
+    sb.clear();
+    list.clear();
     return r2;
   };
-  for (int g = 0, r0 = 0; g < ng && !rc; r0 += group_rec(gb, g)[3], ++g) {
+  for (int g = 0; g < ng && !rc; ++g) {
     if (status[g] == RBGTOPO_GANG_FAILED) continue;
-    const int32_t* rec = group_rec(gb, g);
-    const int q = rec[3];
-    const int32_t* roles = gb + rec[4];
-    const int32_t* pair = gb + rec[5];
-    const int32_t* grp = rp ? rp + 2LL * r0 : nullptr;
-    int S[RBGTOPO_MAX_GROUP_ROLES], ord0[RBGTOPO_MAX_GROUP_ROLES], unplaced[RBGTOPO_MAX_GROUP_ROLES];  // in pods
-    for (int k = 0, acc = 0; k < q; ++k) {
-      S[k] = grp ? grp[2 * k] : 1;
-      ord0[k] = acc;
-      unplaced[k] = roles[4 * k + 1] * S[k];
-      acc += unplaced[k];
-    }
-    anchors.assign(gb + rec[7], gb + rec[7] + 3LL * rec[6]);
-    // one wave: (role, first replica, replicas) per role row; pods of role ri from pod0[g] + ord0[ri] + first * S[ri]
-    auto wave = [&](int n_rows, const int (*w)[3]) {
-      if (rc) return;
-      auto first = [&](int p) { return pod0[g] + ord0[w[p][0]] + (int64_t)w[p][1] * S[w[p][0]]; };
+    HostRun r(gb, g, off.grp(rp, g), off.pod0[g]);
+    const PlanWave& w = r.w;
+    // one wave: pods of role ri from pod0 + ord0[ri] + first * S
+    auto first = [&](int p) { return r.pod0 + r.ord0[w.role[p]] + (int64_t)w.first[p] * r.S(w.role[p]); };
+    while (!rc && next_wave(r.roles, r.q, r.rp, r.cur, r.w) > 0) {
       bool any = false;
-      for (int p = 0; p < n_rows; ++p)
-        for (int k = 0; k < w[p][2] * S[w[p][0]]; ++k) any |= assign[first(p) + k] >= 0;
+      for (int p = 0; p < w.n; ++p)
+        for (int k = 0; k < w.count[p] * r.S(w.role[p]); ++k) any |= assign[first(p) + k] >= 0;
       if (any) {
-        if (rowacc + n_rows > max_rows) rc = flush();
-        if (rc) return;
-        int32_t st[RBGTOPO_STEP_WORDS] = {0};
-        st[0] = rec[0];
-        st[2] = -1;
-        st[3] = n_rows;
-        while (data.size() & 3) data.push_back(0);
-        st[4] = (int32_t)data.size();
-        int n = 0;
-        for (int p = 0; p < n_rows; ++p) {
-          const int ri = w[p][0], pods = w[p][2] * S[ri];
-          int need = 0;
-          for (int k = 0; k < q; ++k)
-            if (pair[ri * q + k] > 0) need += unplaced[k];
-          data.push_back(pods);
-          data.push_back(roles[4 * ri + 2]);
-          data.push_back(std::min(need, RBGTOPO_NEED_CAP));
-          data.push_back(0);
-          n += pods;
-          const int64_t rep0 = first(p);
+        if (sb.rowacc + w.n > max_rows) rc = flush();
+        if (rc) break;
+        for (int p = 0; p < w.n; ++p) {
+          const int pods = w.count[p] * r.S(w.role[p]);
           bool placed = false;
-          for (int k = 0; k < pods; ++k) placed |= assign[rep0 + k] >= 0;
-          if (placed) list.push_back(AltRow{rowacc + p, g, ri, (int)rep0, pods});
+          for (int k = 0; k < pods; ++k) placed |= assign[first(p) + k] >= 0;
+          if (placed) list.push_back(AltRow{sb.rowacc + p, g, w.role[p], (int)first(p), pods});
         }
-        st[5] = q;
-        st[6] = (int32_t)data.size();
-        for (int p = 0; p < n_rows; ++p) data.insert(data.end(), pair + w[p][0] * q, pair + (w[p][0] + 1) * q);
-        st[7] = (int32_t)(anchors.size() / 3);
-        st[8] = (int32_t)data.size();
-        data.insert(data.end(), anchors.begin(), anchors.end());
-        st[10] = (int32_t)data.size();
-        st[11] = n;
-        st[12] = racc;
-        st[13] = rowacc;
-        tab.insert(tab.end(), st, st + RBGTOPO_STEP_WORDS);
-        ++ns;
-        racc += n;
-        rowacc += n_rows;
+        sb.add(r, w, 0, -1, 0, false, nullptr, 0);
       }
-      for (int p = 0; p < n_rows; ++p)  // the wave's placements: anchors of the later waves
-        for (int k = 0; k < w[p][2] * S[w[p][0]]; ++k) {
+      for (int p = 0; p < w.n; ++p)  // the wave's placements: anchors of the later waves
+        for (int k = 0; k < w.count[p] * r.S(w.role[p]); ++k) {
           const int node = assign[first(p) + k];
           if (node < 0) continue;
-          anchors.push_back(node); anchors.push_back(w[p][0]); anchors.push_back(1);
-          unplaced[w[p][0]] -= 1;
+          r.anchors.push_back(node); r.anchors.push_back(w.role[p]); r.anchors.push_back(1);
+          r.unplaced[w.role[p]] -= 1;
         }
-    };
-    int w[RBGTOPO_MAX_STEP_ROLES][3];
-    if (grp) {  // pod waves, as place_groups_lw staged them
-      for (int cr = 0, taken = 0, P; (P = lw_wave(roles, q, grp, cr, taken, w)) > 0;) {
-        wave(P, w);
-        cr = w[P - 1][0];
-        taken = w[P - 1][1] + w[P - 1][2];
-      }
-    } else {
-      walk_waves(roles, q, [&](int, const PlanWave& pw) {
-        for (int p = 0; p < pw.n; ++p) { w[p][0] = pw.role[p]; w[p][1] = pw.first[p]; w[p][2] = pw.count[p]; }
-        wave(pw.n, w);
-      });
     }
   }
   if (!rc) rc = flush();
@@ -3824,32 +3837,20 @@ int rank_committed(rbgtopo_ctx* c, Batch* b, const int32_t* gb, const int32_t* r
 int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign, int32_t* status,
                            int32_t* domain, int32_t* rounds_out, const RankReq* rk = nullptr) {
   *rounds_out = 0;
-  if (words < RBGTOPO_HDR_WORDS || gb[0] != RBGTOPO_GROUPS_MAGIC || gb[1] != RBGTOPO_ABI_VERSION || gb[3] != words)
-    return fail(RBGTOPO_EINVAL, "bad groups blob header");
+  if (const int hrc = check_groups_blob(gb, words)) return hrc;
   const int ng = gb[2];
-  if (ng < 0 || (int64_t)RBGTOPO_HDR_WORDS + (int64_t)ng * RBGTOPO_GROUP_WORDS > words)
-    return fail(RBGTOPO_EINVAL, "group table exceeds blob");
   if (words > 0x3FFFFFFFLL) return fail(RBGTOPO_ELIMIT, "groups blob too large");
   NvtxRange nv("rbgtopo:place_groups_committed");
   const Topology& T = c->topo;
-  TopoHost th;
-  th.n = T.n;
-  th.n_domains = T.n_domains;
-  th.n_levels = installed_levels(c);
-  th.place_levels = commits_levels(c);  // levels >= 1 only on a ctx that opted into committed levels (DESIGN.md §3.9)
-  th.level_nd = c->topo.lvl_nd.empty() ? nullptr : c->topo.lvl_nd.data();
-  th.degp1 = T.h_degp1.data();
-  th.max_degp1 = T.max_degp1;
-  th.wsum_max = T.wsum_max;
-  const long long row_w = T.wsum_max + RBGTOPO_SELF_W;
-  const long long amax_limit = ((1LL << 24) + row_w - 1) / row_w;
+  // levels >= 1 only on a ctx that opted into committed levels (DESIGN.md §3.9)
+  const TopoHost th = topo_host(c, commits_levels(c));
   static thread_local std::vector<GroupFacts> facts;
   static thread_local std::vector<int32_t> order, run;
   order.resize((size_t)std::max(ng, 1));
   DirectGeom G;
-  int rc = direct_pass1(th, gb, words, ng, amax_limit, row_w, facts, order.data(), &G);
+  int rc = direct_pass1(th, gb, words, ng, facts, order.data(), &G);
   if (rc) return rc;
-  rc = direct_pass2(th, gb, words, ng, amax_limit, row_w, facts, &G);
+  rc = direct_pass2(th, gb, words, ng, facts, &G);
   if (rc) return rc;
   if (G.max_cap > 0x3FFFFFFFLL || G.smem > kFastSmemMax)
     return fail(RBGTOPO_ELIMIT, "a group's table of patched nodes (%lld entries, %zu B of shared memory) does not fit "
@@ -3857,12 +3858,7 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
   if (rk) {  // before the first round: the ranking must not fail once the batch is placed
     if ((size_t)((T.n + 31) / 32) * 4 > kFastSmemMax)
       return fail(RBGTOPO_ELIMIT, "ranked placement: %d nodes exceed the room bitmap", T.n);
-    // the §3.4 bound over every wave the ranking can score: lw_validate's with one pod per replica (§3.11 rule 7)
-    long long qsum = 0, pods = 0;
-    for (int g = 0; g < ng; ++g) qsum += gb[RBGTOPO_HDR_WORDS + (int64_t)g * RBGTOPO_GROUP_WORDS + 3];
-    std::vector<int32_t> unit(2 * (size_t)qsum);
-    for (size_t i = 0; i < unit.size(); i += 2) { unit[i] = 1; unit[i + 1] = -1; }
-    rc = lw_validate(c, gb, words, unit.data(), (int64_t)unit.size(), &pods);
+    rc = exact_one_pod(c, gb, words);  // over every wave the ranking can score
     if (rc) return rc;
   }
   run.clear();  // groups with pending replicas, ascending: a round runs a suffix of them
@@ -4030,25 +4026,6 @@ int place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int
 }  // namespace
 
 namespace {
-// The exactness bound of a ranked placement (§3.10): lw_validate's with one pod per replica, which takes every mix of
-// unplaced earlier replicas a re-run group's later waves can see.  Only its RBGTOPO_EINEXACT is returned: a malformed
-// blob gets the code the placement itself gives it.
-int ranked_exact(rbgtopo_ctx* c, const int32_t* gb, int64_t words) {
-  if (words < RBGTOPO_HDR_WORDS || gb[0] != RBGTOPO_GROUPS_MAGIC || gb[3] != words) return RBGTOPO_OK;
-  const int ng = gb[2];
-  if (ng < 0 || (int64_t)RBGTOPO_HDR_WORDS + (int64_t)ng * RBGTOPO_GROUP_WORDS > words) return RBGTOPO_OK;
-  long long qsum = 0, pods = 0;
-  for (int g = 0; g < ng; ++g) {
-    const int q = gb[RBGTOPO_HDR_WORDS + (int64_t)g * RBGTOPO_GROUP_WORDS + 3];
-    if (q < 0 || q > RBGTOPO_MAX_GROUP_ROLES) return RBGTOPO_OK;
-    qsum += q;
-  }
-  std::vector<int32_t> unit(2 * (size_t)qsum);
-  for (size_t i = 0; i < unit.size(); i += 2) { unit[i] = 1; unit[i + 1] = -1; }
-  const int rc = lw_validate(c, gb, words, unit.data(), (int64_t)unit.size(), &pods);
-  return rc == RBGTOPO_EINEXACT ? rc : RBGTOPO_OK;
-}
-
 // rbgtopo_place_groups, and its ranked form when rk != nullptr (status and domain are then not null)
 int32_t place_groups_impl(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign, int32_t* status,
                           int32_t* domain, const RankReq* rk) {
@@ -4058,10 +4035,9 @@ int32_t place_groups_impl(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int3
     if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
     if (rk && (size_t)((c->topo.n + 31) / 32) * 4 > kFastSmemMax)  // before placing: the ranking must not fail afterwards
       return fail(RBGTOPO_ELIMIT, "ranked placement: %d nodes exceed the room bitmap", c->topo.n);
-    if (rk) {  // before placing: a group the host loop re-runs must not meet the §3.4 bound in a later wave (§3.10)
-      const int rc0 = ranked_exact(c, gb, words);
-      if (rc0) return rc0;
-    }
+    // before placing: a group the host loop re-runs must not meet the §3.4 bound in a later wave (§3.10).  Only
+    // RBGTOPO_EINEXACT is returned here: a malformed blob gets the code the placement itself gives it.
+    if (rk && groups_blob_ok(gb, words) && exact_one_pod(c, gb, words) == RBGTOPO_EINEXACT) return RBGTOPO_EINEXACT;
     CK(cudaSetDevice(c->cfg.device));
     static const bool prof = getenv("RBGTOPO_PROFILE_HOST") != nullptr;
     auto now = [] { return std::chrono::steady_clock::now(); };
@@ -4149,84 +4125,22 @@ int32_t place_groups_impl(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int3
   bool any = false;
   for (char d : dirty) any |= d != 0;
   if (!any) return RBGTOPO_OK;
-  if (!rk) return place_groups_slow(c, gb, words, assign, status, domain, &dirty);
-  KeptRows kept;
-  kept.rk = rk;
-  for (int g = 0; g < (int)dirty.size(); ++g)
-    if (dirty[g]) kept.cap += group_role_rows(gb, g);
-  CK(kept.rows.reserve(std::max<size_t>(1, kept.cap) * (size_t)c->slab_stride));
-  return place_groups_slow(c, gb, words, assign, status, domain, &dirty, &kept);
+  return place_groups_slow(c, gb, words, assign, status, domain, &dirty, rk);
 }
 }  // namespace
 
 // ---- leader-worker replicas (rbgtopo_place_groups_lw, DESIGN.md §3.11)
 namespace {
-// The next pod wave of a group from replica cursor (cr, taken): the roles of one level in order, at most
-// RBGTOPO_MAX_STEP_ROLES role rows and RBGTOPO_MAX_STEP_REPLICAS pods, a replica's S pods never split.  Returns the
-// role rows; w[k] = (role, first replica, replicas).
-int lw_wave(const int32_t* roles, int q, const int32_t* rp, int cr, int taken, int (*w)[3]) {
-  while (cr < q && roles[4 * cr + 1] - taken <= 0) { ++cr; taken = 0; }
-  if (cr >= q) return 0;
-  const int level = roles[4 * cr];
-  int P = 0, n = 0;
-  while (cr < q && roles[4 * cr] == level && P < RBGTOPO_MAX_STEP_ROLES) {
-    const int left = roles[4 * cr + 1] - taken;
-    if (left <= 0) { ++cr; taken = 0; continue; }
-    const int S = rp[2 * cr];
-    const int take = std::min(left, (RBGTOPO_MAX_STEP_REPLICAS - n) / S);
-    if (take == 0) break;
-    w[P][0] = cr; w[P][1] = taken; w[P][2] = take;
-    ++P;
-    n += take * S;
-    taken += take;
-    if (taken == roles[4 * cr + 1]) { ++cr; taken = 0; }
-  }
-  return P;
-}
-
-struct LwRun {  // one group while its pod waves are placed
-  const int32_t* rec = nullptr;
-  const int32_t* roles = nullptr;
-  const int32_t* pair = nullptr;
-  const int32_t* rp = nullptr;  // (S, C) per role
-  int q = 0, fixed_domain = -1, status = RBGTOPO_PLACED_ALL;
-  bool failed = false;
-  int cur_role = 0, cur_taken = 0;  // replica cursor
-  long long pod0 = 0;               // the group's first pod in assign
-  int ord0[RBGTOPO_MAX_GROUP_ROLES] = {0};      // first pod of every role inside the group's range
-  int unplaced[RBGTOPO_MAX_GROUP_ROLES] = {0};  // pods
-  std::vector<int32_t> anchors;     // (node, role, count)*
-  std::map<int, int> consumed;      // node -> amount (committed: earlier groups' claims included)
-  std::vector<int32_t> owner_claims;  // committed, exclusive group: (node, claim gid)* of claimed domains, by node
-  int w[RBGTOPO_MAX_STEP_ROLES][3];
-  int P = 0;
-  bool done() const { return failed || cur_role >= q; }
-};
-
 // Validation: the checks and messages of rbgtopo_place_groups (group_facts phase 1, offsets), the role_pods table, then
 // group_facts phase 2 (scheduled pods, exactness bound) with the bound taken over the pod waves.
 int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
                 long long* total_pods) {
-  if (words < RBGTOPO_HDR_WORDS || gb[0] != RBGTOPO_GROUPS_MAGIC || gb[1] != RBGTOPO_ABI_VERSION || gb[3] != words)
-    return fail(RBGTOPO_EINVAL, "bad groups blob header");
+  if (const int hrc = check_groups_blob(gb, words)) return hrc;
   const int ng = gb[2];
-  if (ng < 0 || (int64_t)RBGTOPO_HDR_WORDS + (int64_t)ng * RBGTOPO_GROUP_WORDS > words)
-    return fail(RBGTOPO_EINVAL, "group table exceeds blob");
-  const Topology& T = c->topo;
-  TopoHost th;
-  th.n = T.n;
-  th.n_domains = T.n_domains;
-  th.n_levels = installed_levels(c);
-  th.place_levels = places_levels(c);
-  th.level_nd = T.lvl_nd.empty() ? nullptr : T.lvl_nd.data();
-  th.degp1 = T.h_degp1.data();
-  th.max_degp1 = T.max_degp1;
-  th.wsum_max = T.wsum_max;
-  const long long row_w = T.wsum_max + RBGTOPO_SELF_W;
-  const long long amax_limit = ((1LL << 24) + row_w - 1) / row_w;
+  const TopoHost th = topo_host(c, places_levels(c));
   GroupFacts f;
   for (int g = 0; g < ng; ++g) {
-    int rc = group_facts(th, gb, words, g, true, amax_limit, row_w, &f, 1);
+    int rc = group_facts(th, gb, words, g, true, &f, 1);
     if (rc) return rc;
   }
   long long pacc = 0, qsum = 0;
@@ -4267,10 +4181,9 @@ int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t*
     // such mix — the per-wave validation can then never find an inexact step in the middle of a call.
     const bool gang = (rec[1] & RBGTOPO_STEP_GANG) != 0;
     long long bound[RBGTOPO_MAX_GROUP_ROLES] = {0}, placed[RBGTOPO_MAX_GROUP_ROLES] = {0};
-    int cr = 0, taken = 0, w[RBGTOPO_MAX_STEP_ROLES][3];
-    for (int P; (P = lw_wave(roles, q, grp, cr, taken, w)) > 0;) {
-      for (int k = 0; k < P; ++k) {
-        const int ri = w[k][0];
+    walk_waves(roles, q, grp, [&](int, const PlanWave& w) {
+      for (int k = 0; k < w.n; ++k) {
+        const int ri = w.role[k];
         long long need = 0, bnd = 0;
         for (int j = 0; j < q; ++j) {
           if (pair[ri * q + j] > 0) need += (long long)roles[4 * j + 1] * grp[2 * j] - placed[j];
@@ -4293,11 +4206,9 @@ int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t*
         }
         bound[ri] = std::max(bound[ri], bnd);
       }
-      for (int k = 0; k < P; ++k) placed[w[k][0]] += (long long)w[k][2] * grp[2 * w[k][0]];
-      cr = w[P - 1][0];
-      taken = w[P - 1][1] + w[P - 1][2];
-    }
-    int rc = group_facts(th, gb, words, g, true, amax_limit, row_w, &f, 2, bound);
+      for (int k = 0; k < w.n; ++k) placed[w.role[k]] += (long long)w.count[k] * grp[2 * w.role[k]];
+    });
+    int rc = group_facts(th, gb, words, g, true, &f, 2, bound);
     if (rc) return rc;
   }
   *total_pods = pods;
@@ -4307,18 +4218,6 @@ int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t*
 // One CTA per step up to the CTAs that fit the device at once; with a co-location level in the wave, no more CTAs
 // than kLwScratchBytes of level-C domain scratch (12 bytes per domain) allow.
 constexpr size_t kLwScratchBytes = 64u << 20;
-
-// (wave, role) rows of a group's pod waves: what the ranked form may keep for it.
-size_t lw_role_rows(const int32_t* roles, int q, const int32_t* grp) {
-  size_t n = 0;
-  int w[RBGTOPO_MAX_STEP_ROLES][3];
-  for (int cr = 0, taken = 0, P; (P = lw_wave(roles, q, grp, cr, taken, w)) > 0;) {
-    n += (size_t)P;
-    cr = w[P - 1][0];
-    taken = w[P - 1][1] + w[P - 1][2];
-  }
-  return n;
-}
 
 // What a group of a committed leader-worker batch takes from the groups after it (§3.13): (node, demand) of its placed
 // pods, aggregated by node, and the exclusive domain it reports (-1 = none).  A gang-failed group takes nothing.
@@ -4351,41 +4250,18 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
                                     "committed (levels >= 1: rbgtopo_place_groups_committed)", g, group_rec(gb, g)[10]);
   const size_t smem = (size_t)((T.n + 31) / 32) * 4;
   if (smem > kFastSmemMax) return fail(RBGTOPO_ELIMIT, "leader-worker placement: %d nodes exceed the room bitmap", T.n);
-  std::vector<LwRun> runs(ng);
-  std::vector<int> rp0(ng + 1, 0);
-  std::vector<long long> pod0(ng + 1, 0);
-  for (int g = 0; g < ng; ++g) {
-    const int32_t* rec = group_rec(gb, g);
-    rp0[g + 1] = rp0[g] + rec[3];
-    long long pods = 0;
-    for (int i = 0; i < rec[3]; ++i) pods += (long long)gb[rec[4] + 4 * i + 1] * rp[2LL * (rp0[g] + i)];
-    pod0[g + 1] = pod0[g] + pods;
-  }
+  const GroupOffsets off(gb, rp);
+  std::vector<HostRun> runs(ng);
   auto init_run = [&](int g) {
-    LwRun& r = runs[g];
-    r = LwRun();
-    r.rec = group_rec(gb, g);
-    r.q = r.rec[3];
-    r.roles = gb + r.rec[4];
-    r.pair = gb + r.rec[5];
-    r.rp = rp + 2LL * rp0[g];
-    r.fixed_domain = r.rec[2];
-    r.pod0 = pod0[g];
-    for (int i = 0, acc = 0; i < r.q; ++i) {
-      r.ord0[i] = acc;
-      r.unplaced[i] = r.roles[4 * i + 1] * r.rp[2 * i];
-      acc += r.unplaced[i];
-    }
-    r.anchors.assign(gb + r.rec[7], gb + r.rec[7] + 3LL * r.rec[6]);
-    while (r.cur_role < r.q && r.roles[4 * r.cur_role + 1] == 0) ++r.cur_role;
-    for (long long k = pod0[g]; k < pod0[g + 1]; ++k) assign[k] = -1;
+    runs[g] = HostRun(gb, g, off.grp(rp, g), off.pod0[g]);
+    for (int64_t k = off.pod0[g]; k < off.pod0[g + 1]; ++k) assign[k] = -1;
   };
   const bool keep = rk && !rounds;
-  std::vector<AltRow> kept;  // keep: the (wave, role) rows that placed a pod, in b->lw_kept
+  std::vector<AltRow> kept;  // keep: the (wave, role) rows that placed a pod, in b->kept
   size_t kept_cap = 0, kept_used = 0;
   for (int g = 0; g < ng; ++g) {
     init_run(g);
-    if (keep) kept_cap += lw_role_rows(runs[g].roles, runs[g].q, runs[g].rp);
+    if (keep) kept_cap += group_role_rows(gb, g, off.grp(rp, g));
   }
   std::vector<LwClaims> claims(rounds ? ng : 0);  // committed: every group's claims as the latest round left them
   std::vector<int> dom_ptr, dom_nodes;             // committed: the nodes of every level-0 domain
@@ -4404,15 +4280,13 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
   rc = acquire_batch(c, &b);
   if (rc) return rc;
   cudaStream_t s = stream_of(c, b);
-  if (keep) {
-    cudaError_t e = b->lw_kept.reserve(std::max<size_t>(1, kept_cap) * (size_t)c->slab_stride);
-    if (e != cudaSuccess) {
-      release_batch(c, b);
-      return fail(RBGTOPO_ECUDA, "rows of the ranked leader-worker placement: %s", cudaGetErrorString(e));
-    }
+  if (keep && (rc = reserve_kept(c, b, kept_cap))) {
+    release_batch(c, b);
+    return rc;
   }
   rbgtopo_timing total{};
-  std::vector<int32_t> blob, w_assign, w_status, w_domain, side;
+  StepBlob sb;
+  std::vector<int32_t> w_assign, w_status, w_domain, side, cons;
   std::vector<int> active;
   std::vector<std::pair<int, int>> oc;
   int lo = 0, n_rounds = 0;  // committed: the round's first group, rounds run
@@ -4422,9 +4296,9 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
       std::map<int, int> cap, own;  // node -> capacity taken; level-0 domain -> gid of its last reporter
       for (int g = 0; g < ng; ++g) {
         if (g >= lo) {
-          LwRun& r = runs[g];
           if (n_rounds > 0) init_run(g);
-          r.consumed = cap;
+          HostRun& r = runs[g];
+          r.taken = cap;
           if (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) {
             oc.clear();
             for (const auto& [d, gid] : own)
@@ -4444,58 +4318,26 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
       if (active.empty()) break;
       // ---- this wave's step blob: role counts in pods, need over unplaced pods
       const int ns = (int)active.size();
-      blob.assign((size_t)RBGTOPO_HDR_WORDS + (size_t)ns * RBGTOPO_STEP_WORDS, 0);
+      sb.clear();
       side.assign((size_t)ns * MAXP, 0);
-      int racc = 0, rowacc = 0, dmax = 0;
+      int dmax = 0;
       for (int i = 0; i < ns; ++i) {
-        LwRun& r = runs[active[i]];
-        r.P = lw_wave(r.roles, r.q, r.rp, r.cur_role, r.cur_taken, r.w);
-        int32_t st[RBGTOPO_STEP_WORDS] = {0};
-        st[0] = r.rec[0];
-        st[1] = r.rec[1] & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG);
-        st[2] = (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) ? r.fixed_domain : -1;
-        st[3] = r.P;
-        while (blob.size() & 3) blob.push_back(0);  // role records are read as 16-byte vectors
-        st[4] = (int32_t)blob.size();
-        int n = 0;
-        for (int p = 0; p < r.P; ++p) {
-          const int ri = r.w[p][0], S = r.rp[2 * ri], C = r.rp[2 * ri + 1];
-          int need = 0;
-          for (int q = 0; q < r.q; ++q)
-            if (r.pair[ri * r.q + q] > 0) need += r.unplaced[q];
-          blob.push_back(r.w[p][2] * S);
-          blob.push_back(r.roles[4 * ri + 2]);
-          blob.push_back(std::min(need, RBGTOPO_NEED_CAP));
-          blob.push_back(r.roles[4 * ri + 3] & RBGTOPO_ROLE_EXCLUSIVE);
-          side[(size_t)i * MAXP + p] = lw_pack_role(S, C);
+        HostRun& r = runs[active[i]];
+        next_wave(r.roles, r.q, r.rp, r.cur, r.w);
+        for (int p = 0; p < r.w.n; ++p) {
+          const int ri = r.w.role[p], C = r.rp[2 * ri + 1];
+          side[(size_t)i * MAXP + p] = lw_pack_role(r.S(ri), C);
           if (C >= 0) dmax = std::max(dmax, lv.nd[C]);
-          n += r.w[p][2] * S;
         }
-        st[5] = r.q;
-        st[6] = (int32_t)blob.size();
-        for (int p = 0; p < r.P; ++p) blob.insert(blob.end(), r.pair + r.w[p][0] * r.q, r.pair + (r.w[p][0] + 1) * r.q);
-        st[7] = (int32_t)(r.anchors.size() / 3);
-        st[8] = (int32_t)blob.size();
-        blob.insert(blob.end(), r.anchors.begin(), r.anchors.end());
-        st[9] = (int32_t)r.consumed.size();
-        st[10] = (int32_t)blob.size();
-        // by node, one per node.  Only a committed round whose group is re-run later can see claims summing past
-        // free[n] (stale claims of earlier groups), so clamping them to RBGTOPO_MAX_FREE changes no kept result
-        for (const auto& kv : r.consumed) { blob.push_back(kv.first); blob.push_back(std::min(kv.second, RBGTOPO_MAX_FREE)); }
-        st[11] = n;
-        st[12] = racc;
-        st[13] = rowacc;
-        st[14] = r.rec[10];  // exclusive level
-        racc += n;
-        rowacc += r.P;
-        memcpy(blob.data() + RBGTOPO_HDR_WORDS + (size_t)i * RBGTOPO_STEP_WORDS, st, sizeof st);
+        // consumed records by node, one per node.  Only a committed round whose group is re-run later can see claims
+        // summing past free[n] (stale claims of earlier groups), so clamping them to RBGTOPO_MAX_FREE changes no kept result
+        cons.clear();
+        for (const auto& kv : r.taken) { cons.push_back(kv.first); cons.push_back(std::min(kv.second, RBGTOPO_MAX_FREE)); }
+        sb.add(r, r.w, r.rec[1] & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG),
+               (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) ? r.fixed_domain : -1, r.rec[10], true, cons.data(), (int)r.taken.size());
       }
-      blob[0] = RBGTOPO_BLOB_MAGIC;
-      blob[1] = RBGTOPO_ABI_VERSION;
-      blob[2] = ns;
-      blob[3] = (int32_t)blob.size();
-      blob[4] = racc;
-      blob[5] = rowacc;
+      const std::vector<int32_t>& blob = sb.build();
+      const int racc = sb.racc, rowacc = sb.rowacc;
       // committed: per step the offsets of its owner claims, then the (node, gid) records, 8-byte aligned
       size_t claim_at = 0, rec_at = 0;
       if (rounds) {
@@ -4537,15 +4379,8 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
         return RBGTOPO_OK;
       }();
       if (!rc) rc = fetch_batch(c, b, w_assign.data(), w_status.data(), w_domain.data());
-      const size_t slot0 = kept_used;  // this wave's rows in b->lw_kept, in matrix order
-      if (!rc && keep) {
-        const size_t stride = (size_t)c->slab_stride;
-        cudaError_t e = slot0 + rowacc <= kept_cap ? cudaMemcpyAsync(b->lw_kept.p + slot0 * stride, b->matrix.p,
-                                                                      (size_t)rowacc * stride * 4, cudaMemcpyDeviceToDevice, s)
-                                                   : cudaErrorInvalidValue;
-        if (e != cudaSuccess) rc = fail(RBGTOPO_ECUDA, "keeping the dense rows of a wave: %s", cudaGetErrorString(e));
-        kept_used += (size_t)rowacc;
-      }
+      const size_t slot0 = kept_used;  // this wave's rows in b->kept, in matrix order
+      if (!rc && keep) rc = keep_wave_rows(c, b, rowacc, kept_cap, &kept_used);
       if (rc) break;
       {
         std::lock_guard<std::mutex> g(c->stat_mu);
@@ -4556,55 +4391,37 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
         total.h2d_words += c->last.h2d_words;
       }
       // ---- absorb the placements: every pod placed is an anchor (node, role, 1) and consumes (node, demand)
-      int off = 0;
+      int off = 0, row = 0;  // row: the role's dense row in this wave's matrix
       for (int i = 0; i < ns; ++i) {
-        LwRun& r = runs[active[i]];
+        HostRun& r = runs[active[i]];
         bool any = false;
-        for (int p = 0; p < r.P; ++p) {
-          const int ri = r.w[p][0], S = r.rp[2 * ri];
-          const long long first = r.pod0 + r.ord0[ri] + (long long)r.w[p][1] * S;
+        for (int p = 0; p < r.w.n; ++p, ++row) {
+          const int ri = r.w.role[p], S = r.S(ri);
+          const int64_t first = r.pod0 + r.ord0[ri] + (int64_t)r.w.first[p] * S;
           bool placed = false;
-          for (int k = 0; k < r.w[p][2] * S; ++k, ++off) {
+          for (int k = 0; k < r.w.count[p] * S; ++k, ++off) {
             const int node = w_assign[off];
             assign[first + k] = node;
             if (node < 0) continue;
             any = placed = true;
             r.anchors.push_back(node); r.anchors.push_back(ri); r.anchors.push_back(1);
-            r.consumed[node] += r.roles[4 * ri + 2];
+            r.taken[node] += r.roles[4 * ri + 2];
             r.unplaced[ri] -= 1;
           }
-          if (keep && placed) {
-            const int row = blob[RBGTOPO_HDR_WORDS + (size_t)i * RBGTOPO_STEP_WORDS + 13] + p;  // in this wave's matrix
-            kept.push_back(AltRow{(int)slot0 + row, active[i], ri, (int)first, r.w[p][2] * S});
-          }
+          if (keep && placed) kept.push_back(AltRow{(int)slot0 + row, active[i], ri, (int)first, r.w.count[p] * S});
         }
         if ((r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) && w_domain[i] >= 0 && any) r.fixed_domain = w_domain[i];
         r.status = std::max(r.status, w_status[i]);
         if ((r.rec[1] & RBGTOPO_STEP_GANG) && w_status[i] != RBGTOPO_PLACED_ALL) r.failed = true;
-        r.cur_role = r.w[r.P - 1][0];
-        r.cur_taken = r.w[r.P - 1][1] + r.w[r.P - 1][2];
-        if (r.cur_taken >= r.roles[4 * r.cur_role + 1]) { ++r.cur_role; r.cur_taken = 0; }
-        while (r.cur_role < r.q && r.roles[4 * r.cur_role + 1] == 0) ++r.cur_role;
       }
     }
     if (rc) break;
-    for (int g = lo; g < ng; ++g) {
-      const LwRun& r = runs[g];
-      const bool excl = (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) != 0;
-      if (r.failed) {  // gang: nothing of the group is placed
-        for (long long k = pod0[g]; k < pod0[g + 1]; ++k) assign[k] = -1;
-        if (status) status[g] = RBGTOPO_GANG_FAILED;
-        if (domain) domain[g] = -1;
-      } else {
-        if (status) status[g] = r.status;
-        if (domain) domain[g] = excl ? r.fixed_domain : -1;
-      }
-    }
+    for (int g = lo; g < ng; ++g) runs[g].results(g, assign, status, domain);
     if (rounds) {
       ++n_rounds;
       int cmin = -1;  // the lowest group whose claims differ from what the groups after it saw
       for (int g = lo; g < ng; ++g) {
-        const LwRun& r = runs[g];
+        const HostRun& r = runs[g];
         LwClaims nc;
         if (!r.failed) {
           std::map<int, int> cap;
@@ -4655,141 +4472,104 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
   }
   if (!rc && keep) {  // the placements are final now: rank the kept rows
     alt_clear(*rk, 0, total_pods);
-    rc = run_alternates(c, b, b->lw_kept.p, kept, gb, rp, assign, status, domain, *rk);
+    rc = run_alternates(c, b, b->kept.p, kept, gb, rp, assign, status, domain, *rk);
     if (rc) cudaStreamSynchronize(s);
   }
   release_batch(c, b);
+  return rc;
+}
+
+// The entry checks of every rbgtopo_place_groups* function, in this order: rounds = 0, null arguments, n_alt, world
+// == 1, lock / topology / device, own status and domain for a ranked form given NULL; then the placement of `form`.
+// rbgtopo_place_groups and its ranked form take the lock inside place_groups_impl, which releases it before the
+// host-driven re-run.
+enum PlaceForm { kPlaceReplicas = 0, kPlaceCommitted = 1, kPlaceLw = 2, kPlaceRanked = 4 };
+int32_t place_entry(int form, rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
+                    int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds, float* score,
+                    int32_t* alt_node, float* alt_score) {
+  const bool committed = form & kPlaceCommitted, lw = form & kPlaceLw, ranked = form & kPlaceRanked;
+  if (rounds) *rounds = 0;
+  if (!c || !gb || !assign || (lw && !rp) || (ranked && (!score || (n_alt > 0 && (!alt_node || !alt_score)))))
+    return fail(RBGTOPO_EINVAL, "null argument");
+  if (ranked && (n_alt < 0 || n_alt > RBGTOPO_MAX_ALTERNATES))
+    return fail(RBGTOPO_EINVAL, "n_alt %d outside [0, %d]", n_alt, RBGTOPO_MAX_ALTERNATES);
+  if ((ranked || lw) && c->cfg.world > 1)
+    return fail(RBGTOPO_ELIMIT, "%s needs world == 1: a rank holds only its slab of every dense row",
+                !lw ? "ranked placement" : committed ? "committed leader-worker placement" : "leader-worker placement");
+  std::shared_lock<std::shared_mutex> lk(c->topo_mu, std::defer_lock);  // one snapshot for the rounds and the ranking
+  if (committed || lw) {
+    lk.lock();
+    if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
+    CK(cudaSetDevice(c->cfg.device));
+  }
+  std::vector<int32_t> own_status, own_domain;  // status / domain may be NULL: the ranking still needs them
+  if (ranked) {
+    const int64_t ng = words >= RBGTOPO_HDR_WORDS ? std::max<int64_t>(0, std::min<int64_t>(gb[2], words / RBGTOPO_GROUP_WORDS)) : 0;
+    if (!status) { own_status.resize((size_t)ng + 1); status = own_status.data(); }
+    if (!domain) { own_domain.resize((size_t)ng + 1); domain = own_domain.data(); }
+  }
+  const RankReq rk{n_alt, score, alt_node, alt_score};
+  const RankReq* rkp = ranked ? &rk : nullptr;
+  if (!lw && !committed) return place_groups_impl(c, gb, words, assign, status, domain, rkp);
+  int32_t r = 0;
+  const int rc = lw ? place_groups_lw(c, gb, words, rp, rp_words, assign, status, domain, rkp, committed ? &r : nullptr)
+                    : place_groups_committed(c, gb, words, assign, status, domain, &r, rkp);
+  if (rounds) *rounds = r;
   return rc;
 }
 }  // namespace
 
 int32_t rbgtopo_place_groups(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign,
                              int32_t* status, int32_t* domain) {
-  if (!c || !gb || !assign) return fail(RBGTOPO_EINVAL, "null argument");
-  return place_groups_impl(c, gb, words, assign, status, domain, nullptr);
+  return place_entry(kPlaceReplicas, c, gb, words, nullptr, 0, 0, assign, status, domain, nullptr, nullptr, nullptr,
+                     nullptr);
 }
 
 int32_t rbgtopo_place_groups_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t n_alt, int32_t* assign,
                                     int32_t* status, int32_t* domain, float* score, int32_t* alt_node, float* alt_score) {
-  if (!c || !gb || !assign || !score || (n_alt > 0 && (!alt_node || !alt_score))) return fail(RBGTOPO_EINVAL, "null argument");
-  if (n_alt < 0 || n_alt > RBGTOPO_MAX_ALTERNATES)
-    return fail(RBGTOPO_EINVAL, "n_alt %d outside [0, %d]", n_alt, RBGTOPO_MAX_ALTERNATES);
-  if (c->cfg.world > 1)
-    return fail(RBGTOPO_ELIMIT, "ranked placement needs world == 1: a rank holds only its slab of every dense row");
-  const int64_t ng = words >= RBGTOPO_HDR_WORDS ? std::max<int64_t>(0, std::min<int64_t>(gb[2], words / RBGTOPO_GROUP_WORDS)) : 0;
-  std::vector<int32_t> own_status, own_domain;  // status / domain may be NULL: the ranking still needs them
-  if (!status) { own_status.resize((size_t)ng + 1); status = own_status.data(); }
-  if (!domain) { own_domain.resize((size_t)ng + 1); domain = own_domain.data(); }
-  const RankReq rk{n_alt, score, alt_node, alt_score};
-  return place_groups_impl(c, gb, words, assign, status, domain, &rk);
+  return place_entry(kPlaceRanked, c, gb, words, nullptr, 0, n_alt, assign, status, domain, nullptr, score, alt_node,
+                     alt_score);
 }
 
 int32_t rbgtopo_place_groups_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t* assign,
                                        int32_t* status, int32_t* domain, int32_t* rounds) {
-  if (rounds) *rounds = 0;
-  if (!c || !gb || !assign) return fail(RBGTOPO_EINVAL, "null argument");
-  std::shared_lock<std::shared_mutex> lk(c->topo_mu);
-  if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
-  CK(cudaSetDevice(c->cfg.device));
-  int32_t r = 0;
-  const int rc = place_groups_committed(c, gb, words, assign, status, domain, &r);
-  if (rounds) *rounds = r;
-  return rc;
+  return place_entry(kPlaceCommitted, c, gb, words, nullptr, 0, 0, assign, status, domain, rounds, nullptr, nullptr,
+                     nullptr);
 }
 
 int32_t rbgtopo_place_groups_committed_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t n_alt,
                                               int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds,
                                               float* score, int32_t* alt_node, float* alt_score) {
-  if (rounds) *rounds = 0;
-  if (!c || !gb || !assign || !score || (n_alt > 0 && (!alt_node || !alt_score))) return fail(RBGTOPO_EINVAL, "null argument");
-  if (n_alt < 0 || n_alt > RBGTOPO_MAX_ALTERNATES)
-    return fail(RBGTOPO_EINVAL, "n_alt %d outside [0, %d]", n_alt, RBGTOPO_MAX_ALTERNATES);
-  if (c->cfg.world > 1)
-    return fail(RBGTOPO_ELIMIT, "ranked placement needs world == 1: a rank holds only its slab of every dense row");
-  std::shared_lock<std::shared_mutex> lk(c->topo_mu);  // one snapshot for the rounds and the ranking
-  if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
-  CK(cudaSetDevice(c->cfg.device));
-  const int64_t ng = words >= RBGTOPO_HDR_WORDS ? std::max<int64_t>(0, std::min<int64_t>(gb[2], words / RBGTOPO_GROUP_WORDS)) : 0;
-  std::vector<int32_t> own_status, own_domain;  // status / domain may be NULL: the ranking still needs them
-  if (!status) { own_status.resize((size_t)ng + 1); status = own_status.data(); }
-  if (!domain) { own_domain.resize((size_t)ng + 1); domain = own_domain.data(); }
-  const RankReq rk{n_alt, score, alt_node, alt_score};
-  int32_t r = 0;
-  const int rc = place_groups_committed(c, gb, words, assign, status, domain, &r, &rk);
-  if (rounds) *rounds = r;
-  return rc;
+  return place_entry(kPlaceCommitted | kPlaceRanked, c, gb, words, nullptr, 0, n_alt, assign, status, domain, rounds,
+                     score, alt_node, alt_score);
 }
 
 int32_t rbgtopo_place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* role_pods,
                                 int64_t role_pods_words, int32_t* assign, int32_t* status, int32_t* domain) {
-  if (!c || !gb || !assign || !role_pods) return fail(RBGTOPO_EINVAL, "null argument");
-  if (c->cfg.world > 1)
-    return fail(RBGTOPO_ELIMIT, "leader-worker placement needs world == 1: a rank holds only its slab of every dense row");
-  std::shared_lock<std::shared_mutex> lk(c->topo_mu);
-  if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
-  CK(cudaSetDevice(c->cfg.device));
-  return place_groups_lw(c, gb, words, role_pods, role_pods_words, assign, status, domain);
+  return place_entry(kPlaceLw, c, gb, words, role_pods, role_pods_words, 0, assign, status, domain, nullptr, nullptr,
+                     nullptr, nullptr);
 }
 
 int32_t rbgtopo_place_groups_lw_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* role_pods,
                                        int64_t role_pods_words, int32_t n_alt, int32_t* assign, int32_t* status,
                                        int32_t* domain, float* score, int32_t* alt_node, float* alt_score) {
-  if (!c || !gb || !assign || !role_pods || !score || (n_alt > 0 && (!alt_node || !alt_score)))
-    return fail(RBGTOPO_EINVAL, "null argument");
-  if (n_alt < 0 || n_alt > RBGTOPO_MAX_ALTERNATES)
-    return fail(RBGTOPO_EINVAL, "n_alt %d outside [0, %d]", n_alt, RBGTOPO_MAX_ALTERNATES);
-  if (c->cfg.world > 1)
-    return fail(RBGTOPO_ELIMIT, "leader-worker placement needs world == 1: a rank holds only its slab of every dense row");
-  std::shared_lock<std::shared_mutex> lk(c->topo_mu);
-  if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
-  CK(cudaSetDevice(c->cfg.device));
-  const int64_t ng = words >= RBGTOPO_HDR_WORDS ? std::max<int64_t>(0, std::min<int64_t>(gb[2], words / RBGTOPO_GROUP_WORDS)) : 0;
-  std::vector<int32_t> own_status, own_domain;  // status / domain may be NULL: the ranking still needs them
-  if (!status) { own_status.resize((size_t)ng + 1); status = own_status.data(); }
-  if (!domain) { own_domain.resize((size_t)ng + 1); domain = own_domain.data(); }
-  const RankReq rk{n_alt, score, alt_node, alt_score};
-  return place_groups_lw(c, gb, words, role_pods, role_pods_words, assign, status, domain, &rk);
+  return place_entry(kPlaceLw | kPlaceRanked, c, gb, words, role_pods, role_pods_words, n_alt, assign, status, domain,
+                     nullptr, score, alt_node, alt_score);
 }
 
 int32_t rbgtopo_place_groups_lw_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* role_pods,
                                           int64_t role_pods_words, int32_t* assign, int32_t* status, int32_t* domain,
                                           int32_t* rounds) {
-  if (rounds) *rounds = 0;
-  if (!c || !gb || !assign || !role_pods) return fail(RBGTOPO_EINVAL, "null argument");
-  if (c->cfg.world > 1)
-    return fail(RBGTOPO_ELIMIT, "committed leader-worker placement needs world == 1: a rank holds only its slab of every dense row");
-  std::shared_lock<std::shared_mutex> lk(c->topo_mu);  // one snapshot for every round
-  if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
-  CK(cudaSetDevice(c->cfg.device));
-  int32_t r = 0;
-  const int rc = place_groups_lw(c, gb, words, role_pods, role_pods_words, assign, status, domain, nullptr, &r);
-  if (rounds) *rounds = r;
-  return rc;
+  return place_entry(kPlaceLw | kPlaceCommitted, c, gb, words, role_pods, role_pods_words, 0, assign, status, domain,
+                     rounds, nullptr, nullptr, nullptr);
 }
 
 int32_t rbgtopo_place_groups_lw_committed_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words,
                                                  const int32_t* role_pods, int64_t role_pods_words, int32_t n_alt,
                                                  int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds,
                                                  float* score, int32_t* alt_node, float* alt_score) {
-  if (rounds) *rounds = 0;
-  if (!c || !gb || !assign || !role_pods || !score || (n_alt > 0 && (!alt_node || !alt_score)))
-    return fail(RBGTOPO_EINVAL, "null argument");
-  if (n_alt < 0 || n_alt > RBGTOPO_MAX_ALTERNATES)
-    return fail(RBGTOPO_EINVAL, "n_alt %d outside [0, %d]", n_alt, RBGTOPO_MAX_ALTERNATES);
-  if (c->cfg.world > 1)
-    return fail(RBGTOPO_ELIMIT, "committed leader-worker placement needs world == 1: a rank holds only its slab of every dense row");
-  std::shared_lock<std::shared_mutex> lk(c->topo_mu);  // one snapshot for the rounds and the ranking
-  if (!c->topo.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
-  CK(cudaSetDevice(c->cfg.device));
-  const int64_t ng = words >= RBGTOPO_HDR_WORDS ? std::max<int64_t>(0, std::min<int64_t>(gb[2], words / RBGTOPO_GROUP_WORDS)) : 0;
-  std::vector<int32_t> own_status, own_domain;  // status / domain may be NULL: the ranking still needs them
-  if (!status) { own_status.resize((size_t)ng + 1); status = own_status.data(); }
-  if (!domain) { own_domain.resize((size_t)ng + 1); domain = own_domain.data(); }
-  const RankReq rk{n_alt, score, alt_node, alt_score};
-  int32_t r = 0;
-  const int rc = place_groups_lw(c, gb, words, role_pods, role_pods_words, assign, status, domain, &rk, &r);
-  if (rounds) *rounds = r;
-  return rc;
+  return place_entry(kPlaceLw | kPlaceCommitted | kPlaceRanked, c, gb, words, role_pods, role_pods_words, n_alt, assign,
+                     status, domain, rounds, score, alt_node, alt_score);
 }
 
 int32_t rbgtopo_plan_describe(const int32_t* gb, int64_t words, int32_t n_nodes, int32_t n_domains,
@@ -4798,16 +4578,7 @@ int32_t rbgtopo_plan_describe(const int32_t* gb, int64_t words, int32_t n_nodes,
   if (!gb || !n_steps) return fail(RBGTOPO_EINVAL, "null argument");
   if (n_nodes < 1 || n_domains < 1 || wsum_max < 0) return fail(RBGTOPO_EINVAL, "n_nodes / n_domains / wsum_max");
   TopoHost th;
-  th.n = n_nodes;
-  th.n_domains = n_domains;
-  th.degp1 = deg_plus1;
-  th.max_degp1 = 1;
-  if (deg_plus1)
-    for (int i = 0; i < n_nodes; ++i) {
-      if (deg_plus1[i] < 1) return fail(RBGTOPO_EINVAL, "deg_plus1[%d]", i);
-      th.max_degp1 = std::max(th.max_degp1, deg_plus1[i]);
-    }
-  th.wsum_max = wsum_max;
+  if (const int trc = topo_host_args(n_nodes, n_domains, deg_plus1, wsum_max, &th)) return trc;
   static thread_local std::unique_ptr<Batch> scratch;  // host vectors + a pageable staging buffer only
   if (!scratch) {
     scratch = std::make_unique<Batch>();
@@ -4830,29 +4601,17 @@ int32_t rbgtopo_place_describe(const int32_t* gb, int64_t words, int32_t n_nodes
                                int64_t wsum_max, int32_t* order, int64_t order_cap, int32_t* geom) {
   if (!gb || !geom) return fail(RBGTOPO_EINVAL, "null argument");
   if (n_nodes < 1 || n_domains < 1 || wsum_max < 0) return fail(RBGTOPO_EINVAL, "n_nodes / n_domains / wsum_max");
-  if (words < RBGTOPO_HDR_WORDS || gb[0] != RBGTOPO_GROUPS_MAGIC || gb[1] != RBGTOPO_ABI_VERSION || gb[3] != words || words > 0x3FFFFFFFLL)
-    return fail(RBGTOPO_EINVAL, "bad groups blob header");
+  if (words > 0x3FFFFFFFLL) return fail(RBGTOPO_EINVAL, "bad groups blob header");
+  if (const int hrc = check_groups_blob(gb, words)) return hrc;
   const int ng = gb[2];
-  if (ng < 0 || (int64_t)RBGTOPO_HDR_WORDS + (int64_t)ng * RBGTOPO_GROUP_WORDS > words) return fail(RBGTOPO_EINVAL, "group table exceeds blob");
   TopoHost th;
-  th.n = n_nodes;
-  th.n_domains = n_domains;
-  th.degp1 = deg_plus1;
-  th.max_degp1 = 1;
-  if (deg_plus1)
-    for (int i = 0; i < n_nodes; ++i) {
-      if (deg_plus1[i] < 1) return fail(RBGTOPO_EINVAL, "deg_plus1[%d]", i);
-      th.max_degp1 = std::max(th.max_degp1, deg_plus1[i]);
-    }
-  th.wsum_max = wsum_max;
-  const long long row_w = wsum_max + RBGTOPO_SELF_W;
-  const long long amax_limit = ((1LL << 24) + row_w - 1) / row_w;
+  if (const int trc = topo_host_args(n_nodes, n_domains, deg_plus1, wsum_max, &th)) return trc;
   static thread_local std::vector<GroupFacts> facts;
   static thread_local std::vector<int32_t> perm;
   perm.assign((size_t)std::max(1, ng), 0);
   DirectGeom G;
-  int rc = direct_pass1(th, gb, words, ng, amax_limit, row_w, facts, perm.data(), &G);
-  if (!rc) rc = direct_pass2(th, gb, words, ng, amax_limit, row_w, facts, &G);
+  int rc = direct_pass1(th, gb, words, ng, facts, perm.data(), &G);
+  if (!rc) rc = direct_pass2(th, gb, words, ng, facts, &G);
   if (rc) return rc;
   geom[0] = (int32_t)G.total_r;
   geom[1] = G.n0;
