@@ -28,10 +28,11 @@ package b200topo
 static void rbgtopo_go_err(rbgtopo_ctx* ctx, int32_t rc, char* err) {
   if (rc != RBGTOPO_OK) rbgtopo_last_error(ctx, err, RBGTOPO_GO_ERRLEN); else err[0] = 0;
 }
-static int32_t rbgtopo_go_create(int32_t device, int32_t rank, int32_t world, rbgtopo_ctx** out, char* err) {
+static int32_t rbgtopo_go_create(int32_t device, int32_t rank, int32_t world, int32_t flags, rbgtopo_ctx** out,
+                                 char* err) {
   rbgtopo_config cfg;
   memset(&cfg, 0, sizeof cfg);
-  cfg.device = device; cfg.rank = rank; cfg.world = world;
+  cfg.device = device; cfg.rank = rank; cfg.world = world; cfg.flags = flags;
   int32_t rc = rbgtopo_create(&cfg, out);
   rbgtopo_go_err(NULL, rc, err);
   return rc;
@@ -178,10 +179,21 @@ type placer struct {
 	nLevels atomic.Int32 // exclusive levels above 0 the snapshot holds (setExclusiveLevels; setTopology clears them)
 }
 
-func newPlacer(device int) (*placer, error) {
+// Config flags of the ctx (include/rbgtopo.h).  CfgLWCommitLevels lets a committed batch with leader-worker groups hold
+// groups at exclusive levels >= 1 (DESIGN.md §3.16); it needs the two flags before it, so its ctx takes all three.
+const (
+	CfgLevelPlacement = int32(C.RBGTOPO_CFG_LEVEL_PLACEMENT)
+	CfgCommitLevels   = int32(C.RBGTOPO_CFG_COMMIT_LEVELS)
+	CfgLWCommitLevels = int32(C.RBGTOPO_CFG_LW_COMMIT_LEVELS)
+)
+
+func newPlacer(device int) (*placer, error) { return newPlacerFlags(device, 0) }
+
+// newPlacerFlags creates the ctx with config flags, e.g. CfgLevelPlacement | CfgCommitLevels | CfgLWCommitLevels.
+func newPlacerFlags(device int, flags int32) (*placer, error) {
 	var buf [C.RBGTOPO_GO_ERRLEN]C.char
 	p := &placer{}
-	rc := C.rbgtopo_go_create(C.int32_t(device), 0, 1, &p.ctx, &buf[0])
+	rc := C.rbgtopo_go_create(C.int32_t(device), 0, 1, C.int32_t(flags), &p.ctx, &buf[0])
 	if err := mkErr(rc, &buf); err != nil {
 		return nil, err
 	}

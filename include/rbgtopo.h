@@ -142,6 +142,10 @@ typedef struct rbgtopo_config {
 #define RBGTOPO_CFG_COMMIT_LEVELS 2    /* rbgtopo_place_groups_committed also places groups
                                           at levels >= 1 (claims across levels); valid only
                                           with RBGTOPO_CFG_LEVEL_PLACEMENT, alone EINVAL */
+#define RBGTOPO_CFG_LW_COMMIT_LEVELS 4 /* rbgtopo_place_groups_lw_committed[_ranked] also place
+                                          groups at levels >= 1 (claims across levels, in
+                                          pods); valid only with both flags above (flags = 7),
+                                          else EINVAL */
 
 /* Per-call device timing, milliseconds from CUDA events on the call's stream. */
 typedef struct rbgtopo_timing {
@@ -433,16 +437,22 @@ int32_t rbgtopo_place_groups_lw_ranked(rbgtopo_ctx* ctx, const int32_t* groups, 
  *     group wins); in occupancy mode node n of D shows owner_0[n] (+) gid instead.
  * Over the batch no node receives more than free[n].  With S = 1 and C = -1 everywhere the results are
  * bit-identical to rbgtopo_place_groups_committed's.  *rounds (may be NULL) = wave-loop rounds run: at most
- * n_groups, 1 for one group.  Limits (RBGTOPO_ELIMIT): a group whose own exclusive level is >= 1, a ctx with
- * world > 1, more nodes than the room bitmap of rbgtopo_place_groups_lw holds.  Alternates:
- * rbgtopo_place_groups_lw_committed_ranked. */
+ * n_groups, 1 for one group.  Limits (RBGTOPO_ELIMIT): a group whose own exclusive level is >= 1 on a ctx without
+ * RBGTOPO_CFG_LW_COMMIT_LEVELS, a ctx with world > 1, more nodes than the room bitmap of rbgtopo_place_groups_lw
+ * holds.  On a ctx created with RBGTOPO_CFG_LW_COMMIT_LEVELS (flags = 7, DESIGN.md §3.16) a group exclusive at level
+ * L_g >= 1 is placed too: a participating role may not use node n when owner_{L_g}[n] (+) K (+) P is neither -1 nor
+ * gid_g, where K merges, for every level L of the batch's exclusive groups, the gid of the last earlier exclusive
+ * group at L (status != 2) that reports dom_L(n), and P the gid of every pod an earlier exclusive group keyed at
+ * another level placed for a participating role in dom_{L_g}(n).  A batch whose groups are all at level 0 gives the
+ * same results and rounds with and without the flag.  Alternates: rbgtopo_place_groups_lw_committed_ranked. */
 int32_t rbgtopo_place_groups_lw_committed(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
                                           const int32_t* role_pods, int64_t role_pods_words, int32_t* assign,
                                           int32_t* status, int32_t* domain, int32_t* rounds);
 
 /* Ranked alternates of a committed leader-worker batch (DESIGN.md §3.15).  rbgtopo_place_groups_lw_committed — same
  * GROUPS blob and (S, C) table, validation, exactness bound, error codes and limits (a group exclusive at a level
- * >= 1 is RBGTOPO_ELIMIT), bit-identical assign / status / domain / *rounds — plus, per pod p (in assign order),
+ * >= 1 is RBGTOPO_ELIMIT without RBGTOPO_CFG_LW_COMMIT_LEVELS), bit-identical assign / status / domain / *rounds —
+ * plus, per pod p (in assign order),
  * score[p] and alt_node[p * n_alt + i] / alt_score[p * n_alt + i], i < n_alt, as by
  * rbgtopo_place_groups_lw_ranked, with room and owners counted after the WHOLE batch:
  *   - the row of p is the one of its replica's (wave, role) in its group's final run of the committed wave loop
@@ -450,8 +460,9 @@ int32_t rbgtopo_place_groups_lw_committed(rbgtopo_ctx* ctx, const int32_t* group
  *     snapshot's;
  *   - a candidate n has a finite score, is not assign[p], and free[n] - used_B[n] >= demand, where used_B sums the
  *     demand of every pod this call placed on n, in all groups (a gang-failed group places nothing);
- *   - for a participating role of an exclusive group g it also lies in domain[g] and the level-0 owner the whole
- *     batch leaves there (§3.13's rule with every group's claims, later groups' included) is -1 or gid_g;
+ *   - for a participating role of an exclusive group g it also lies in domain[g] and the owner the whole batch
+ *     leaves there (§3.13's rule with every group's claims, later groups' included; at levels, with
+ *     RBGTOPO_CFG_LW_COMMIT_LEVELS, owner_{L_g} (+) K (+) P over every group of the batch) is -1 or gid_g;
  *   - for a role with C >= 0 it lies in the level-C domain of the pod's replica (dom_C(n) = dom_C(assign[p])).
  * So moving one pod to one of its alternates over-commits no node, meets no exclusive claim of another gid in this
  * batch and keeps its replica co-located.  A one-group batch gives all six outputs of rbgtopo_place_groups_lw_ranked;

@@ -23,6 +23,7 @@ class Config(C.Structure):
 
 CFG_LEVEL_PLACEMENT = 1  # RBGTOPO_CFG_LEVEL_PLACEMENT: place groups / steps at exclusive levels >= 1
 CFG_COMMIT_LEVELS = 2    # RBGTOPO_CFG_COMMIT_LEVELS: committed batches at levels >= 1 too (with the flag above)
+CFG_LW_COMMIT_LEVELS = 4  # RBGTOPO_CFG_LW_COMMIT_LEVELS: committed leader-worker batches at levels >= 1 (with both above)
 
 
 class Timing(C.Structure):

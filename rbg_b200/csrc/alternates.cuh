@@ -17,7 +17,8 @@
 // then the whole batch's placements, and a node of a participating job must also pass the owner test every group of the
 // batch has left on it (commit_owner with cm.g = n_groups), read only where the room bit is read.
 // k_alternates_commit_coloc ranks the pod rows of a committed leader-worker batch
-// (rbgtopo_place_groups_lw_committed_ranked, §3.15) that has a co-location domain: both conditions at once, level 0 only.
+// (rbgtopo_place_groups_lw_committed_ranked, §3.15) that has a co-location domain: both conditions at once;
+// k_alternates_commit_coloc_lv the same at exclusive levels (§3.16).
 #pragma once
 #include "kernels.cuh"
 #include "plan_group.cuh"
@@ -62,7 +63,8 @@ __device__ __forceinline__ void alt_insert(unsigned long long (&top)[ALT_LIST], 
 // COLOC: some job has a co-location condition.  The <false> form is the ranked placement of one-pod replicas with the
 // registers it had before the condition existed (40; the condition costs 5 more, one CTA per SM less).
 // COMMIT: gids[job] = the job's group gid; LV: the batch has a group at a level >= 1 (commit_owner<LV>).  COMMIT with
-// COLOC only without LV (k_alternates_commit_coloc); the other forms keep the registers they had without it.
+// COLOC: k_alternates_commit_coloc and, at levels, k_alternates_commit_coloc_lv; the other forms keep the registers
+// they had without it.
 template <bool COLOC, bool COMMIT, bool LV>
 __device__ __forceinline__ void alternates_body(TopoDev t, const float* __restrict__ rows,
                                                 const AltJob* __restrict__ jobs, const int2* __restrict__ used,
@@ -195,6 +197,15 @@ k_alternates_commit_coloc(TopoDev t, const float* __restrict__ rows, const AltJo
                           const int2* __restrict__ used, const int* __restrict__ own, int n_alt, int* __restrict__ out,
                           CommitDev cm, const int* __restrict__ gids) {
   alternates_body<true, true, false>(t, rows, jobs, used, own, n_alt, out, cm, gids);
+}
+
+// The same at exclusive levels (§3.16): cm holds the host-built lists in the CommitDev<true> layout (per (level,
+// domain) reporters, pods linked at the other levels of lmask), cm.g = n_groups.
+__global__ void __launch_bounds__(ALT_THREADS)
+k_alternates_commit_coloc_lv(TopoDev t, const float* __restrict__ rows, const AltJob* __restrict__ jobs,
+                             const int2* __restrict__ used, const int* __restrict__ own, int n_alt,
+                             int* __restrict__ out, CommitDev cm, const int* __restrict__ gids) {
+  alternates_body<true, true, true>(t, rows, jobs, used, own, n_alt, out, cm, gids);
 }
 
 }  // namespace rbgtopo

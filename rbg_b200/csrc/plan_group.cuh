@@ -928,6 +928,12 @@ __global__ void __launch_bounds__(32 * RTAB_WARPS) k_commit_claims(const int* __
   }
 }
 
+// The claim lists of a committed leader-worker batch at levels (DESIGN.md §3.16) are built on the host; their heads
+// are dense arrays, so each round only the heads that change are written: heads[set[i].x] = set[i].y.
+__global__ void k_set_heads(int* heads, const int2* __restrict__ set, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) heads[set[i].x] = set[i].y;
+}
+
 // After a round of a committed batch: which later groups can a changed claim affect?  One warp per group of the round
 // (b.perm order).  A group's claims changed when a placement or its reported domain differs from the previous round's
 // (`prev`, which is then updated).  A changed claim on node n matters only when a later group read n this round

@@ -235,6 +235,9 @@ struct Batch {
   // leader-worker placement (place_groups_lw): the wave's (S, C) side table, the per-CTA level-C domain scratch
   DevBuf<int> lw, lw_cap;
   PinBuf<int> h_lw;
+  // ... committed at levels (§3.16): the changed heads, dclaim and pclaim of the round's claim lists (heads in cm_int)
+  DevBuf<int> lwc;
+  PinBuf<int> h_lwc;
   DevBuf<unsigned long long> lw_best;
   // ranked host-driven wave loops (place_groups_slow, place_groups_lw): the dense rows of every (wave, role), kept
   // across calls like the matrix
@@ -877,15 +880,18 @@ int launch_emit_plan(rbgtopo_ctx* c, Batch* b, cudaStream_t s, long long n_rows,
 }
 
 // claim_off != nullptr (step batches of rbgtopo_place_groups_lw_committed only): k_score_emit_claims with the owner
-// claims of earlier groups per step (score.cuh).
+// claims of earlier groups per step (score.cuh).  cm != nullptr (the same call at levels, §3.16):
+// k_score_emit_claims_lv with the group index of every step.
 int launch_score(rbgtopo_ctx* c, Batch* b, cudaStream_t s, const int* claim_off = nullptr,
-                 const int2* claim_rec = nullptr) {
+                 const int2* claim_rec = nullptr, const int* step_grp = nullptr, const CommitDev* cm = nullptr) {
   const BatchMeta& m = b->m;
   if (m.n_steps == 0) return RBGTOPO_OK;
   if (!b->wave_begin.empty()) return launch_emit_plan(c, b, s, m.total_p);  // multi-wave plan: background rows from the row table
   const int items = (int)emit_items(m.n_steps, c->lc);
   const int grid = items / kEmitBlockSteps;  // one CTA per (block of steps, chunk of nodes)
-  if (claim_off)
+  if (cm)
+    k_score_emit_claims_lv<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items, step_grp, *cm);
+  else if (claim_off)
     k_score_emit_claims<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items, claim_off, claim_rec, c->topo.occ);
   else
     k_score_emit<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items);  // step batch: rows + sparse corrections
@@ -1375,10 +1381,12 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
   *out = nullptr;
   if (cfg->world < 1 || cfg->rank < 0 || cfg->rank >= cfg->world)
     return fail(RBGTOPO_EINVAL, "rank %d / world %d", cfg->rank, cfg->world);
-  if (cfg->flags & ~(RBGTOPO_CFG_LEVEL_PLACEMENT | RBGTOPO_CFG_COMMIT_LEVELS))
+  if (cfg->flags & ~(RBGTOPO_CFG_LEVEL_PLACEMENT | RBGTOPO_CFG_COMMIT_LEVELS | RBGTOPO_CFG_LW_COMMIT_LEVELS))
     return fail(RBGTOPO_EINVAL, "unknown config flags 0x%x", cfg->flags);
   if ((cfg->flags & RBGTOPO_CFG_COMMIT_LEVELS) && !(cfg->flags & RBGTOPO_CFG_LEVEL_PLACEMENT))
     return fail(RBGTOPO_EINVAL, "RBGTOPO_CFG_COMMIT_LEVELS needs RBGTOPO_CFG_LEVEL_PLACEMENT (flags 0x%x)", cfg->flags);
+  if ((cfg->flags & RBGTOPO_CFG_LW_COMMIT_LEVELS) && !(cfg->flags & RBGTOPO_CFG_COMMIT_LEVELS))
+    return fail(RBGTOPO_EINVAL, "RBGTOPO_CFG_LW_COMMIT_LEVELS needs RBGTOPO_CFG_COMMIT_LEVELS (flags 0x%x)", cfg->flags);
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess || ndev <= 0)
@@ -2353,7 +2361,7 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
     cmd.dclaim = reinterpret_cast<const int2*>(d + o_dclaim);
   }
   if (cm && coloc)
-    k_alternates_commit_coloc<<<(unsigned)jobs.size(), ALT_THREADS, smem, s>>>(
+    (cm_levels ? k_alternates_commit_coloc_lv : k_alternates_commit_coloc)<<<(unsigned)jobs.size(), ALT_THREADS, smem, s>>>(
         topo_dev(c), rows, reinterpret_cast<const AltJob*>(d), reinterpret_cast<const int2*>(d + w_jobs),
         d + w_jobs + w_used, F, d + w_in, cmd, d + w_jobs + w_used + w_own);
   else if (cm)
@@ -4220,11 +4228,53 @@ int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t*
 constexpr size_t kLwScratchBytes = 64u << 20;
 
 // What a group of a committed leader-worker batch takes from the groups after it (§3.13): (node, demand) of its placed
-// pods, aggregated by node, and the exclusive domain it reports (-1 = none).  A gang-failed group takes nothing.
+// pods, aggregated by node, and the exclusive domain it reports (-1 = none) at its level.  At levels (§3.16) also the
+// nodes of its placed participating pods (sorted), which later groups keyed at other levels read.  A gang-failed group
+// takes nothing.
 struct LwClaims {
   std::vector<std::pair<int, int>> cap;
+  std::vector<int> pods;
   int dom = -1, gid = -1;
-  bool operator==(const LwClaims& o) const { return cap == o.cap && dom == o.dom && gid == o.gid; }
+  bool operator==(const LwClaims& o) const { return cap == o.cap && pods == o.pods && dom == o.dom && gid == o.gid; }
+};
+
+// The claim lists of a committed leader-worker batch at levels (§3.16), in the layout commit_owner<true> reads, built
+// from every group's claims: a reporting group h links into dhead[doff[L_h] + D] (dclaim[h] = {gid, next}), each
+// placed participating pod into phead[doff[L] + dom_L(node)] for every level L != L_h of lmask (pclaim = {group, gid,
+// next, 0}).  Only the heads a list starts at are written (k_set_heads): `heads` maps a slot of cm_int (phead after
+// the lvl_total_d dhead slots) to its first entry, and holds -1 for the slots the previous lists used.  What a round
+// uploads grows with the groups and the placed pods, not with the size of the claimed domains.
+struct LwLists {
+  std::vector<int2> dclaim;
+  std::vector<int4> pclaim;
+  std::map<int, int> heads;
+  void build(const Topology& T, const int32_t* gb, const std::vector<LwClaims>& claims, int lmask) {
+    for (auto& kv : heads) kv.second = -1;
+    const int ng = (int)claims.size();
+    dclaim.assign((size_t)std::max(ng, 1), make_int2(-1, -1));
+    pclaim.clear();
+    int doff[RBGTOPO_MAX_EXCL_LEVELS + 1] = {0};
+    for (int L = 0; L < T.n_levels + 1 && L < RBGTOPO_MAX_EXCL_LEVELS; ++L) doff[L + 1] = doff[L] + level_domains(T, L);
+    auto head = [&](int slot) -> int& { return heads.emplace(slot, -1).first->second; };
+    for (int g = 0; g < ng; ++g) {
+      const LwClaims& cl = claims[g];
+      const int lh = group_rec(gb, g)[10];
+      if (cl.dom >= 0) {
+        int& h = head(doff[lh] + cl.dom);
+        dclaim[g] = make_int2(cl.gid, h);
+        h = g;
+      }
+      for (const int node : cl.pods)
+        for (int m = lmask; m; m &= m - 1) {
+          const int L = __builtin_ctz(m);
+          if (L == lh) continue;
+          const int d = L == 0 ? T.h_domain[node] : T.h_lvl_domain[(size_t)(L - 1) * T.n + node];
+          int& h = head(T.lvl_total_d + doff[L] + d);
+          pclaim.push_back(make_int4(g, cl.gid, h, 0));
+          h = (int)pclaim.size() - 1;
+        }
+    }
+  }
 };
 
 // rk != nullptr: the ranked form (§3.12).  The matrix is overwritten by every wave, so each wave's rows are copied
@@ -4243,11 +4293,19 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
   if (rc) return rc;
   const Topology& T = c->topo;
   const int ng = gb[2];
+  // committed at levels (§3.16): a group at a level >= 1 selects the claim lists of commit_owner<true>, over the levels
+  // of the batch's exclusive groups (lmask); a batch at level 0 keeps the record path
+  bool at_lv = false;
+  int lmask = 0;
   if (rounds)
-    for (int g = 0; g < ng; ++g)
-      if (group_rec(gb, g)[10] > 0)
+    for (int g = 0; g < ng; ++g) {
+      const int32_t* rec = group_rec(gb, g);
+      if (rec[10] > 0 && !(c->cfg.flags & RBGTOPO_CFG_LW_COMMIT_LEVELS))
         return fail(RBGTOPO_ELIMIT, "committed leader-worker batch: group %d is exclusive at level %d; only level 0 is "
-                                    "committed (levels >= 1: rbgtopo_place_groups_committed)", g, group_rec(gb, g)[10]);
+                                    "committed without RBGTOPO_CFG_LW_COMMIT_LEVELS", g, rec[10]);
+      at_lv |= rec[10] > 0;
+      if (rec[1] & RBGTOPO_STEP_EXCLUSIVE) lmask |= 1 << rec[10];
+    }
   const size_t smem = (size_t)((T.n + 31) / 32) * 4;
   if (smem > kFastSmemMax) return fail(RBGTOPO_ELIMIT, "leader-worker placement: %d nodes exceed the room bitmap", T.n);
   const GroupOffsets off(gb, rp);
@@ -4264,8 +4322,8 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
     if (keep) kept_cap += group_role_rows(gb, g, off.grp(rp, g));
   }
   std::vector<LwClaims> claims(rounds ? ng : 0);  // committed: every group's claims as the latest round left them
-  std::vector<int> dom_ptr, dom_nodes;             // committed: the nodes of every level-0 domain
-  if (rounds) {
+  std::vector<int> dom_ptr, dom_nodes;             // committed at level 0: the nodes of every level-0 domain
+  if (rounds && !at_lv) {
     dom_ptr.assign((size_t)T.n_domains + 1, 0);
     for (int n = 0; n < T.n; ++n) ++dom_ptr[T.h_domain[n] + 1];
     for (int d = 0; d < T.n_domains; ++d) dom_ptr[d + 1] += dom_ptr[d];
@@ -4290,8 +4348,57 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
   std::vector<int> active;
   std::vector<std::pair<int, int>> oc;
   int lo = 0, n_rounds = 0;  // committed: the round's first group, rounds run
+  // at_lv: the lists' heads live in cm_int (dhead | phead, all -1 at the start of the call); cm reads them
+  LwLists lists;
+  CommitDev cm{};
+  int list_launches = 0;
+  long long list_words = 0;
+  auto upload_lists = [&]() -> int {
+    lists.build(T, gb, claims, lmask);
+    std::vector<int2> set;
+    for (const auto& [slot, first] : lists.heads) set.push_back(make_int2(slot, first));
+    for (auto it = lists.heads.begin(); it != lists.heads.end();)  // slots back at -1 need no reset next time
+      it = it->second < 0 ? lists.heads.erase(it) : std::next(it);
+    const size_t o_d = 2 * set.size(), o_p = (o_d + 2 * lists.dclaim.size() + 3) & ~(size_t)3;  // int4-aligned
+    const size_t w = o_p + 4 * lists.pclaim.size();
+    CK(b->lwc.reserve(w + 4));
+    CK(b->h_lwc.reserve(w + 4));
+    memcpy(b->h_lwc.p, set.data(), set.size() * 8);
+    memcpy(b->h_lwc.p + o_d, lists.dclaim.data(), lists.dclaim.size() * 8);
+    memcpy(b->h_lwc.p + o_p, lists.pclaim.data(), lists.pclaim.size() * 16);
+    CK(cudaMemcpyAsync(b->lwc.p, b->h_lwc.p, w * 4, cudaMemcpyHostToDevice, s));
+    if (!set.empty()) {
+      k_set_heads<<<(unsigned)std::min<size_t>((set.size() + 255) / 256, 1024), 256, 0, s>>>(
+          b->cm_int.p, reinterpret_cast<const int2*>(b->lwc.p), (int)set.size());
+      CK(cudaGetLastError());
+      ++list_launches;
+    }
+    cm.dclaim = reinterpret_cast<const int2*>(b->lwc.p + o_d);
+    cm.pclaim = reinterpret_cast<int4*>(b->lwc.p + o_p);
+    list_words += (long long)w;
+    return RBGTOPO_OK;
+  };
+  if (at_lv) {
+    rc = [&]() -> int {
+      CK(b->cm_int.reserve(2 * (size_t)T.lvl_total_d));
+      CK(cudaMemsetAsync(b->cm_int.p, 0xFF, 2 * (size_t)T.lvl_total_d * 4, s));
+      return RBGTOPO_OK;
+    }();
+    if (rc) {
+      release_batch(c, b);
+      return rc;
+    }
+    cm.dhead = b->cm_int.p;
+    cm.phead = b->cm_int.p + T.lvl_total_d;
+    cm.ldom = T.lvl_domain.p;
+    cm.doff = T.lvl_doff.p;
+    cm.lstride = level_stride(T.n);
+    cm.lmask = lmask;
+    cm.occ = true;  // levels >= 1 exist in occupancy mode only
+  }
   for (bool more = true; more;) {
     more = false;
+    if (rounds && at_lv && (rc = upload_lists())) break;
     if (rounds) {  // every group of the round starts from the claims of the groups before it
       std::map<int, int> cap, own;  // node -> capacity taken; level-0 domain -> gid of its last reporter
       for (int g = 0; g < ng; ++g) {
@@ -4299,7 +4406,7 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
           if (n_rounds > 0) init_run(g);
           HostRun& r = runs[g];
           r.taken = cap;
-          if (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) {
+          if (!at_lv && (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE)) {
             oc.clear();
             for (const auto& [d, gid] : own)
               for (int k = dom_ptr[d]; k < dom_ptr[d + 1]; ++k) oc.emplace_back(dom_nodes[k], gid);
@@ -4338,9 +4445,13 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
       }
       const std::vector<int32_t>& blob = sb.build();
       const int racc = sb.racc, rowacc = sb.rowacc;
-      // committed: per step the offsets of its owner claims, then the (node, gid) records, 8-byte aligned
+      // committed: per step the offsets of its owner claims, then the (node, gid) records, 8-byte aligned; at levels
+      // the group index of every step instead
       size_t claim_at = 0, rec_at = 0;
-      if (rounds) {
+      if (rounds && at_lv) {
+        claim_at = side.size();
+        side.insert(side.end(), active.begin(), active.end());
+      } else if (rounds) {
         claim_at = side.size();
         int acc = 0;
         side.push_back(0);
@@ -4368,8 +4479,9 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
         CK(cudaMemcpyAsync(b->lw.p, b->h_lw.p, side.size() * 4, cudaMemcpyHostToDevice, s));
         CK(cudaStreamWaitEvent(s, c->base_ready, 0));  // a pending snapshot refresh
         CK(cudaStreamWaitEvent(s, c->topo_ready, 0));
-        int r2 = rounds ? launch_score(c, b, s, b->lw.p + claim_at, reinterpret_cast<const int2*>(b->lw.p + rec_at))
-                        : launch_score(c, b, s);
+        int r2 = rounds && at_lv ? launch_score(c, b, s, nullptr, nullptr, b->lw.p + claim_at, &cm)
+                 : rounds     ? launch_score(c, b, s, b->lw.p + claim_at, reinterpret_cast<const int2*>(b->lw.p + rec_at))
+                              : launch_score(c, b, s);
         if (r2) return r2;
         k_lw_assign<<<(unsigned)grid, LW_THREADS, smem, s>>>(topo_dev(c), batch_dev(c, b), b->lw.p, b->lw_best.p,
                                                              b->lw_cap.p, dmax, lv);
@@ -4433,6 +4545,14 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
             nc.dom = r.fixed_domain;
             nc.gid = r.rec[0];
           }
+          if (at_lv && (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE)) {  // the placed pods of its participating roles
+            for (int i = 0; i < r.q; ++i)
+              if (r.roles[4 * i + 3] & RBGTOPO_ROLE_EXCLUSIVE)
+                for (long long k = 0; k < (long long)r.roles[4 * i + 1] * r.rp[2 * i]; ++k)
+                  if (const int node = assign[r.pod0 + r.ord0[i] + k]; node >= 0) nc.pods.push_back(node);
+            std::sort(nc.pods.begin(), nc.pods.end());
+            if (!nc.pods.empty()) nc.gid = r.rec[0];
+          }
         }
         if (cmin < 0 && !(nc == claims[g])) cmin = g;
         claims[g] = std::move(nc);
@@ -4444,7 +4564,15 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
     }
   }
   if (rounds) *rounds = n_rounds;
-  if (!rc && rk && rounds) {  // the claims are final now: level-0 owner lists for commit_owner<false>, then the replay
+  if (!rc && rk && rounds && at_lv) {  // the claims are final now: the lists of every group for commit_owner<true>
+    rc = upload_lists();
+    cm.g = ng;
+    int rank_launches = 0;
+    if (!rc) rc = rank_committed(c, b, gb, rp, assign, status, domain, cm, true, *rk, &rank_launches);
+    total.launches += rank_launches;
+    std::lock_guard<std::mutex> g(c->stat_mu);
+    c->launches += rank_launches;
+  } else if (!rc && rk && rounds) {  // the claims are final now: level-0 owner lists for commit_owner<false>, then the replay
     HostClaims hc;
     hc.dhead.assign((size_t)T.n_domains, -1);
     hc.dclaim.assign((size_t)std::max(ng, 1), make_int2(-1, -1));
@@ -4466,6 +4594,9 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
     harvest_base_ms(c);
     std::lock_guard<std::mutex> g(c->stat_mu);
     total.base_ms = c->topo.base_ms;
+    total.launches += list_launches;
+    total.h2d_words += (int32_t)std::min<long long>(list_words, INT32_MAX);
+    c->launches += list_launches;
     c->last = total;
   } else {
     cudaStreamSynchronize(s);

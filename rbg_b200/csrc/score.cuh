@@ -25,6 +25,7 @@
 //      in any order.
 #pragma once
 #include "kernels.cuh"
+#include "plan_group.cuh"
 
 namespace rbgtopo {
 
@@ -45,9 +46,13 @@ constexpr int EMIT_MAX_BLOCK = 16;  // upper bound of b.bsteps
 // (occupancy, `occ`); participating rows of exclusive steps are rewritten to need·base[n] or -inf there, BEFORE the
 // consumed and anchor passes (-inf absorbs their adds, and an unblocked node must exist before them).  The step's
 // consumed records are then sorted by node with one record per node, so a record is its node's whole amount.
-template <bool CLAIMS>
+// LV (k_score_emit_claims_lv, a batch with a group at an exclusive level >= 1, DESIGN.md §3.16): no records.  The
+// background pass of an exclusive step reads each node's owner as commit_owner<true> gives it to group
+// step_grp[step] at the step's level (owner_L ⊕ K ⊕ P, the claim lists `cm0` the host built from the previous round).
+template <bool CLAIMS, bool LV = false>
 __device__ __forceinline__ void score_emit(TopoDev t, BatchDev b, int items, const int* __restrict__ claim_off,
-                                           const int2* __restrict__ claim_rec, bool occ) {
+                                           const int2* __restrict__ claim_rec, bool occ,
+                                           const int* __restrict__ step_grp = nullptr, const CommitDev* cm0 = nullptr) {
   const int T = b.chunk, lc = b.lc;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int groups = T >> 2;
@@ -116,7 +121,18 @@ __device__ __forceinline__ void score_emit(TopoDev t, BatchDev b, int items, con
         const int g = tid + j * SCORE_THREADS;
         int4 avx = av[j];  // capacity as seen by exclusive roles: blocked domains are infeasible
         if (excl_step) {
-          const int4 ow = __ldg(reinterpret_cast<const int4*>(at_level(t, step_level(h0.y)).node_owner + n0 + (g << 2)));
+          int4 ow = __ldg(reinterpret_cast<const int4*>(at_level(t, step_level(h0.y)).node_owner + n0 + (g << 2)));
+          if constexpr (LV) {
+            const int n = n0 + (g << 2);
+            const int4 dm = __ldg(reinterpret_cast<const int4*>(at_level(t, step_level(h0.y)).domain + n));
+            CommitDev cm = *cm0;
+            cm.g = __ldg(step_grp + step);
+            cm.level = step_level(h0.y);
+            ow.x = commit_owner<true>(cm, n, dm.x, ow.x);  // n < n1: live
+            if (n + 1 < n1) ow.y = commit_owner<true>(cm, n + 1, dm.y, ow.y);
+            if (n + 2 < n1) ow.z = commit_owner<true>(cm, n + 2, dm.z, ow.z);
+            if (n + 3 < n1) ow.w = commit_owner<true>(cm, n + 3, dm.w, ow.w);
+          }
           if (!(ow.x == -1 || ow.x == gid)) avx.x = -1;
           if (!(ow.y == -1 || ow.y == gid)) avx.y = -1;
           if (!(ow.z == -1 || ow.z == gid)) avx.z = -1;
@@ -137,7 +153,7 @@ __device__ __forceinline__ void score_emit(TopoDev t, BatchDev b, int items, con
         }
       }
 
-      if constexpr (CLAIMS) {
+      if constexpr (CLAIMS && !LV) {
         const int c0 = __ldg(claim_off + step), c1 = __ldg(claim_off + step + 1);
         if (excl_step && c1 > c0) {
           __syncthreads();  // the background stores precede the rewrite
@@ -219,6 +235,13 @@ __global__ void __launch_bounds__(SCORE_THREADS, 6)
 k_score_emit_claims(TopoDev t, BatchDev b, int items, const int* __restrict__ claim_off,
                     const int2* __restrict__ claim_rec, bool occ) {
   score_emit<true>(t, b, items, claim_off, claim_rec, occ);
+}
+
+// rbgtopo_place_groups_lw_committed[_ranked] on a batch with a group at a level >= 1 (DESIGN.md §3.16): step_grp[step]
+// = the step's group index in the batch; cm = the claim lists of the groups' previous-round results.
+__global__ void __launch_bounds__(SCORE_THREADS, 6)
+k_score_emit_claims_lv(TopoDev t, BatchDev b, int items, const int* __restrict__ step_grp, CommitDev cm) {
+  score_emit<true, true>(t, b, items, nullptr, nullptr, true, step_grp, &cm);
 }
 
 }  // namespace rbgtopo

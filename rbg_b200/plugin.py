@@ -324,7 +324,9 @@ class B200TopoPodGroupManager:
         the snapshot does not hold leave such a group without a hint and log why.  A committed batch with such a
         group and no group at an exclusive level >= 1 goes through ONE rbgtopo_place_groups_lw_committed call (§3.13)
         when the placer has `places_lw_committed`: standalone groups take (1, -1) for every role and keep their RoleID
-        keys; otherwise (levels >= 1, or a placer without it) such a group gets no hint and a logged reason.  With
+        keys.  Groups at exclusive levels >= 1 may be in that batch too when the placer also has
+        `places_lw_committed_levels` (a TopoPlacer created with lw_committed_levels=True, §3.16).  Otherwise (levels
+        >= 1 without it, or a placer without `places_lw_committed`) such a group gets no hint and a logged reason.  With
         alternates, such a group is placed through rbgtopo_place_groups_lw_ranked (§3.12) when the placer has
         `places_lw_ranked`, and its alternates are keyed by pod name and stay inside each replica's co-location
         domain; a placer without it gives no hint for such a group.
@@ -357,11 +359,13 @@ class B200TopoPodGroupManager:
         return lv, ""
 
     def lw_committed(self, rbgs: Sequence[RoleBasedGroup], committed: bool) -> bool:
-        """A committed batch placed by one rbgtopo_place_groups_lw_committed call: it has a leader-worker group, no
-        group at an exclusive level >= 1, and the placer places such batches."""
+        """A committed batch placed by one rbgtopo_place_groups_lw_committed call: it has a leader-worker group, the
+        placer places such batches, and it has no group at an exclusive level >= 1 unless the placer places those in
+        such batches too (`places_lw_committed_levels`)."""
         return (committed and getattr(self.placer, "places_lw_committed", False)
                 and any(self.is_leader_worker(r) for r in rbgs)
-                and not any(self.exclusive_level(r, True)[0] > 0 for r in rbgs))
+                and (getattr(self.placer, "places_lw_committed_levels", False)
+                     or not any(self.exclusive_level(r, True)[0] > 0 for r in rbgs)))
 
     def _split_no_hint(self, rbgs: Sequence[RoleBasedGroup], committed: bool = False):
         """The groups that get a hint, and a no-hint Placement per group that does not (logged, hint dropped)."""
