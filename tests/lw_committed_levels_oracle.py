@@ -48,6 +48,42 @@ def batch_claims(G: Sequence[lw.LwGroup], levels, status, domain, assign, n_doma
     return last, pods
 
 
+def place_group(topo, dom, owner, n_domains, X: lw.LwGroup, L: int, claimed, last, pods, other: int,
+                assign: np.ndarray):
+    """Group X at exclusive level L against what the groups before it left: `claimed` (node -> demand), `last`
+    (per level the gid of a domain's reporter) and `pods` ((gid, level, node) of their participating pods).  Writes its
+    pods into `assign`; returns (status, domain)."""
+    X.consumed = dict(claimed)
+    ow = np.array(owner, dtype=np.int32, copy=True)
+    ow[L] = level_owner(dom, owner, n_domains, L, last, pods)
+    t = levels_view.level_view(topo, dom, ow, n_domains, L, X.gid, other)
+    if X.fixed >= 0:    # the view numbers domain d of level L as 2d (2d + 1 for its nodes blocked to g)
+        X.fixed *= 2
+    lco.run_group(t, X, list(dom), t.domain, assign)
+    if X.fixed >= 0:
+        X.fixed //= 2
+    if X.failed:
+        assign[X.pod0:X.pod0 + X.n_pods] = -1
+        return 2, -1
+    return X.status, (X.fixed if X.flags & lw.STEP_EXCLUSIVE else -1)
+
+
+def group_claims(X: lw.LwGroup, assign: np.ndarray, status: int, domain: int):
+    """What a placed group takes from the groups after it: ({node: demand} of its placed pods, the domain it reports
+    (-1 = none), the nodes of its placed participating pods); a gang-failed group takes nothing."""
+    if status == 2:
+        return {}, -1, []
+    cap = {}
+    for ri in range(X.q):
+        lo = X.pod0 + X.first_pod[ri]
+        for node in assign[lo:lo + X.pending[ri] * X.S[ri]]:
+            if node >= 0:
+                cap[int(node)] = cap.get(int(node), 0) + X.demand[ri]
+    if not X.flags & lw.STEP_EXCLUSIVE:
+        return cap, -1, []
+    return cap, int(domain), participating_pods(X, assign)
+
+
 def run_lw_committed_levels(topo, gblob, role_pods, level_domain, owner, n_domains, limit: Optional[int] = None,
                             terms: Sequence[str] = ("K", "P"), reporter: str = "last"):
     """(assign per pod, status[ng], domain[ng]).  level_domain [n_levels + 1][n] (row 0 = the snapshot's domain), owner
@@ -68,37 +104,21 @@ def run_lw_committed_levels(topo, gblob, role_pods, level_domain, owner, n_domai
     other = levels_oracle.unused_gid({X.gid for X in G})
     for g in range(ng if limit is None else min(limit, ng)):
         X, L = G[g], levels[g]
-        X.consumed = dict(claimed)
-        ow = np.array(owner, dtype=np.int32, copy=True)
-        ow[L] = level_owner(dom, owner, n_domains, L, last, pods)
-        t = levels_view.level_view(topo, dom, ow, n_domains, L, X.gid, other)
-        if X.fixed >= 0:    # the view numbers domain d of level L as 2d (2d + 1 for its nodes blocked to g)
-            X.fixed *= 2
-        lco.run_group(t, X, list(dom), t.domain, assign)
-        if X.fixed >= 0:
-            X.fixed //= 2
-        excl = bool(X.flags & lw.STEP_EXCLUSIVE)
-        if X.failed:
-            assign[X.pod0:X.pod0 + X.n_pods] = -1
-            status[g], domain[g] = 2, -1
-            continue
-        status[g] = X.status
-        domain[g] = X.fixed if excl else -1
-        for ri in range(X.q):
-            lo = X.pod0 + X.first_pod[ri]
-            for node in assign[lo:lo + X.pending[ri] * X.S[ri]]:
-                if node >= 0:
-                    claimed[int(node)] = claimed.get(int(node), 0) + X.demand[ri]
-        if excl:
-            if domain[g] >= 0 and "K" in terms and (reporter == "last" or last[L][domain[g]] == FREE):
-                last[L][domain[g]] = X.gid
-            if "P" in terms:
-                pods += [(X.gid, L, m) for m in participating_pods(X, assign)]
+        status[g], domain[g] = place_group(topo, dom, owner, n_domains, X, L, claimed, last, pods, other, assign)
+        cap, rep, mine = group_claims(X, assign, status[g], domain[g])
+        for node, amt in cap.items():
+            claimed[node] = claimed.get(node, 0) + amt
+        if rep >= 0 and "K" in terms and (reporter == "last" or last[L][rep] == FREE):
+            last[L][rep] = X.gid
+        if "P" in terms:
+            pods += [(X.gid, L, m) for m in mine]
     return assign, status, domain
 
 
-def run_lw_committed_levels_ranked(topo, gblob, role_pods, n_alt: int, level_domain, owner, n_domains):
-    """(assign, status, domain, score[P], alt_node[P, n_alt], alt_score[P, n_alt]) of §3.16's ranked form."""
+def run_lw_committed_levels_ranked(topo, gblob, role_pods, n_alt: int, level_domain, owner, n_domains, claims=None):
+    """(assign, status, domain, score[P], alt_node[P, n_alt], alt_score[P, n_alt]) of §3.16's ranked form.  `claims`
+    ((last, pods) as batch_claims gives them) replaces the batch's own claims in the ranking, for the tests'
+    preconditions."""
     first_pod = {X.pod0: g for g, X in enumerate(lco.groups_of(gblob, role_pods)) if X.n_pods}
     rows = {}
     inner = lw.place_wave
@@ -124,7 +144,7 @@ def run_lw_committed_levels_ranked(topo, gblob, role_pods, n_alt: int, level_dom
             for node in assign[lo:lo + X.pending[ri] * X.S[ri]]:
                 if node >= 0:
                     used[node] += X.demand[ri]
-    last, pods = batch_claims(G, levels, status, domain, assign, n_domains, dom.shape[0])
+    last, pods = batch_claims(G, levels, status, domain, assign, n_domains, dom.shape[0]) if claims is None else claims
     P = len(assign)
     score = np.full(P, -np.inf, dtype=np.float32)
     alt_node = np.full((P, n_alt), -1, dtype=np.int32)
