@@ -599,7 +599,11 @@ int32_t rbgtopo_p2p_stats(rbgtopo_ctx* ctx, int64_t* peer_bytes_last_pass, int32
 
 /* Use an external CUDA stream (e.g. the one the caller's NCCL runs on) for
  * every call on this ctx; NULL restores the internal per-slot streams (pass
- * cudaStreamLegacy, (void*)0x1, to select the legacy default stream). */
+ * cudaStreamLegacy, (void*)0x1, to select the legacy default stream).
+ * Work already enqueued stays ordered across a switch, without blocking the
+ * host: the call makes the incoming stream(s) wait for everything enqueued on
+ * the outgoing one(s), so a fetch, read, release, refresh or pass issued after
+ * the switch sees the passes issued before it. */
 int32_t rbgtopo_set_stream(rbgtopo_ctx* ctx, void* cuda_stream);
 
 /* Per-kernel CUDA events inside a pass.  Off (default): a pass is timed as a whole and the selection

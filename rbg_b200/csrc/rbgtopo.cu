@@ -5301,11 +5301,42 @@ int32_t rbgtopo_set_kernel_timing(rbgtopo_ctx* c, int32_t on) {
   return RBGTOPO_OK;
 }
 
+// Joins the outgoing streams into the incoming ones without blocking the host: everything enqueued before the switch
+// (a pass, a staging, a D2H) is ordered before everything enqueued after it, whichever streams the two sides use.  The
+// batch streams are non-blocking, so nothing else orders them against an external stream.  The pending waits make the
+// incoming streams busy, so fence_batches orders a later refresh behind the outgoing work as well.  topo_mu held
+// exclusively: nothing is enqueued meanwhile, and fence_ev / ev[6] / ev[7] are not recorded elsewhere (fence_batches
+// holds it too).
 int32_t rbgtopo_set_stream(rbgtopo_ctx* c, void* stream) {
   if (!c) return fail(RBGTOPO_EINVAL, "null ctx");
   std::unique_lock<std::shared_mutex> lk(c->topo_mu);
-  c->ext_stream = static_cast<cudaStream_t>(stream);
-  c->use_ext_stream = stream != nullptr;
+  cudaStream_t in = static_cast<cudaStream_t>(stream);
+  {
+    CK(cudaSetDevice(c->cfg.device));
+    std::lock_guard<std::mutex> g(c->pool_mu);
+    if (c->use_ext_stream) {
+      if (in != c->ext_stream) {
+        CK(cudaEventRecord(c->fence_ev, c->ext_stream));
+        if (in) {
+          CK(cudaStreamWaitEvent(in, c->fence_ev, 0));
+        } else {
+          for (auto& b : c->batches) {  // a batch acquired later starts on its own streams too
+            CK(cudaStreamWaitEvent(b->stream, c->fence_ev, 0));
+            CK(cudaStreamWaitEvent(b->stream2, c->fence_ev, 0));
+          }
+        }
+      }
+    } else if (in) {
+      for (auto& b : c->batches) {
+        CK(cudaEventRecord(b->ev[6], b->stream));
+        CK(cudaStreamWaitEvent(in, b->ev[6], 0));
+        CK(cudaEventRecord(b->ev[7], b->stream2));
+        CK(cudaStreamWaitEvent(in, b->ev[7], 0));
+      }
+    }
+  }
+  c->ext_stream = in;
+  c->use_ext_stream = in != nullptr;
   return RBGTOPO_OK;
 }
 

@@ -44,6 +44,41 @@ def check_batch(eng, topo, blob, check_matrix=True, check_topk=True, ref=None):
     return ref
 
 
+# ~50 ms of GPU time at H100 clocks: long enough that a host enqueues a whole call sequence behind it, short enough
+# to queue once per case
+SLEEP_CYCLES = 100_000_000
+
+
+def sleep_on(stream, cycles=SLEEP_CYCLES):
+    """Queue a bounded busy kernel on `stream` (a torch.cuda.Stream; None: torch's default, the legacy stream)."""
+    import torch
+    with torch.cuda.stream(stream if stream is not None else torch.cuda.default_stream()):
+        torch.cuda._sleep(int(cycles))
+
+
+def plan_result(eng, h, rows, roles):
+    """What a staged GROUPS handle exposes after its last pass: (assign, status, domain, the dense rows of the replica
+    rows `rows` as float32 bits [len(rows)][slab], the 32 top-K keys of the role rows `roles` [len(roles)][32])."""
+    a, s, d = eng.fetch(h)
+    lo, hi = eng.slab()
+    m = np.zeros((len(rows), hi - lo), dtype=np.uint32)
+    for i, r in enumerate(rows):
+        m[i] = eng.read_scores(h, r).view(np.uint32)
+    topk = np.zeros((len(roles), 32), dtype=np.uint64)
+    for i, p in enumerate(roles):
+        topk[i] = eng.read_topk(h, p, 32)
+    return a.copy(), s.copy(), d.copy(), m, topk
+
+
+def assert_same_result(got, exp, tag):
+    """Bit equality of two plan_result tuples, naming the first differing output and element."""
+    for name, x, y in zip(("assign", "status", "domain", "rows", "topk"), got, exp):
+        assert x.shape == y.shape, (tag, name, x.shape, y.shape)
+        bad = np.argwhere(x != y)
+        assert len(bad) == 0, (tag, name, f"{len(bad)} differ, first at {tuple(int(v) for v in bad[0])}",
+                               x[tuple(bad[0])], y[tuple(bad[0])])
+
+
 def plan_rows(gblob, topo):
     """(group, wave) -> dense-matrix row of the wave's first replica in a staged multi-wave plan
     (rows are in GROUP order: a group's waves are consecutive; rbgtopo_plan_describe column 4)."""

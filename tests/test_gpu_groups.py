@@ -195,11 +195,22 @@ def test_plan_dense_matrix_and_lists_match_oracle_per_wave():
 
 
 def test_chained_batches_equal_separate_runs():
-    """rbgtopo_run_staged_chain: passes round robin over distinct staged batches, the dense-matrix kernel of a pass
-    chained behind the selection kernel of the pass before it (programmatic dependent launch).  Every batch must end
-    with exactly what a plain rbgtopo_run_staged leaves: placements, status, domains and every dense-matrix row —
-    also for tiny batches (few dense-matrix CTAs: the ordering argument must not lean on the grid size), for a single
-    handle, and with kernel timing on (the documented fallbacks)."""
+    """rbgtopo_run_staged_chain: passes round robin over distinct staged batches on one caller stream, the dense-matrix
+    kernel of a pass chained behind the selection kernel of the pass before it (programmatic dependent launch).  Every
+    batch must end with exactly what a plain rbgtopo_run_staged leaves: placements, status, domains and every
+    dense-matrix row — also for tiny batches (few dense-matrix CTAs: the ordering argument must not lean on the grid
+    size), for a single handle, and with kernel timing on (the documented fallbacks).  tests/test_gpu_chain.py holds
+    the chain's full parity tests."""
+    _chained_batches_equal_separate_runs(caller_stream=True)
+
+
+def test_chained_batches_on_their_own_streams_run_plain_passes():
+    """The same batches without rbgtopo_set_stream: every batch has its own stream, so the chain falls back to plain
+    passes, with the same results."""
+    _chained_batches_equal_separate_runs(caller_stream=False)
+
+
+def _chained_batches_equal_separate_runs(caller_stream):
     from gpu_util import new_engine
     n = 3000
     topo = synth.make_topology(n, seed=11, tiers=4, owned_frac=0.2)
@@ -226,6 +237,10 @@ def test_chained_batches_equal_separate_runs():
                 got = eng.read_scores(h, r)
                 assert np.array_equal(got.view(np.uint32), exp.view(np.uint32)), (i, r)
 
+    if caller_stream:
+        import torch
+        st = torch.cuda.Stream()
+        eng.set_stream(st.cuda_stream)
     hs = [eng.stage_groups(gb) for gb in blobs]
     eng.run_staged_chain(hs, 4)           # one pass each
     check(hs, range(4))

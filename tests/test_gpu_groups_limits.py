@@ -55,39 +55,64 @@ def check_staged(eng, topo, states, waves, gblob):
     h = eng.stage_groups(gblob)
     try:
         eng.run_staged(h, 1)
-        a, s, d = eng.fetch(h)
-        first = {(int(st[0]), int(st[1])): (int(st[4]), int(st[5])) for st in plan_steps(gblob, topo.n, len(topo.domain_owner))}
-        lost = set()
-        rows = 0
-        for w, gis, r in waves:
-            off = rr = 0
-            for k, gi in enumerate(gis):
-                wave = states[gi].waves[w]
-                cnt, P = sum(c for _, _, c in wave), len(wave)
-                if gi not in lost:
-                    row0, role0 = first[(gi, w)]
-                    for j in range(cnt):
-                        got, exp = eng.read_scores(h, row0 + j), r["matrix"][off + j]
-                        bad = np.nonzero(got.view(np.uint32) != exp.view(np.uint32))[0]
-                        assert len(bad) == 0, ("row", w, gi, j, len(bad), int(bad[0]), float(got[bad[0]]), float(exp[bad[0]]))
-                    for p in range(P):
-                        got = eng.read_topk(h, role0 + p, 32)
-                        assert np.array_equal(got, r["topk"][rr + p]), ("topk", w, gi, p, got[:6], r["topk"][rr + p][:6])
-                    rows += cnt
-                    if (r["assign"][off:off + cnt] < 0).any():
-                        lost.add(gi)
-                off += cnt
-                rr += P
-        for i, (st, sl) in enumerate(zip(states, group_slices(states))):
-            res = st.result()
-            if res["status"] == 1:
-                assert int(s[i]) == 1, ("staged", i)
-                continue
-            assert a[sl].tolist() == st.assign_in_group_order(), ("staged", i)
-            assert (int(s[i]), int(d[i])) == (res["status"], res["domain"]), ("staged", i)
-        return rows
+        return check_handle(eng, topo, states, waves, gblob, h)
     finally:
         eng.release(h)
+
+
+def defined_rows(topo, states, waves, gblob):
+    """The replica rows and role rows whose content a pass defines, i.e. those check_handle compares: every wave the
+    oracle ran, a group that lost a replica only up to that wave (later waves of it are not selected)."""
+    first = {(int(st[0]), int(st[1])): (int(st[4]), int(st[5])) for st in plan_steps(gblob, topo.n, len(topo.domain_owner))}
+    lost, rows, roles = set(), [], []
+    for w, gis, r in waves:
+        off = 0
+        for gi in gis:
+            wave = states[gi].waves[w]
+            cnt = sum(c for _, _, c in wave)
+            if gi not in lost:
+                row0, role0 = first[(gi, w)]
+                rows += range(row0, row0 + cnt)
+                roles += range(role0, role0 + len(wave))
+                if (r["assign"][off:off + cnt] < 0).any():
+                    lost.add(gi)
+            off += cnt
+    return rows, roles
+
+
+def check_handle(eng, topo, states, waves, gblob, h):
+    """The checks of check_staged on a handle whose last pass has been enqueued; returns the rows compared."""
+    a, s, d = eng.fetch(h)
+    first = {(int(st[0]), int(st[1])): (int(st[4]), int(st[5])) for st in plan_steps(gblob, topo.n, len(topo.domain_owner))}
+    lost = set()
+    rows = 0
+    for w, gis, r in waves:
+        off = rr = 0
+        for k, gi in enumerate(gis):
+            wave = states[gi].waves[w]
+            cnt, P = sum(c for _, _, c in wave), len(wave)
+            if gi not in lost:
+                row0, role0 = first[(gi, w)]
+                for j in range(cnt):
+                    got, exp = eng.read_scores(h, row0 + j), r["matrix"][off + j]
+                    bad = np.nonzero(got.view(np.uint32) != exp.view(np.uint32))[0]
+                    assert len(bad) == 0, ("row", w, gi, j, len(bad), int(bad[0]), float(got[bad[0]]), float(exp[bad[0]]))
+                for p in range(P):
+                    got = eng.read_topk(h, role0 + p, 32)
+                    assert np.array_equal(got, r["topk"][rr + p]), ("topk", w, gi, p, got[:6], r["topk"][rr + p][:6])
+                rows += cnt
+                if (r["assign"][off:off + cnt] < 0).any():
+                    lost.add(gi)
+            off += cnt
+            rr += P
+    for i, (st, sl) in enumerate(zip(states, group_slices(states))):
+        res = st.result()
+        if res["status"] == 1:
+            assert int(s[i]) == 1, ("staged", i)
+            continue
+        assert a[sl].tolist() == st.assign_in_group_order(), ("staged", i)
+        assert (int(s[i]), int(d[i])) == (res["status"], res["domain"]), ("staged", i)
+    return rows
 
 
 def pending_groups(gblob):
