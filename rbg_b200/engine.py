@@ -73,6 +73,9 @@ class TopoPlacer:
         self.places_lw_committed_ranked = True  # place_groups_lw_committed_ranked: alternates of committed LW batches (§3.15)
         h = C.c_void_p()
         self._h = None
+        # blob totals of every live staged handle (fetch sizes its outputs from them); created here, not on the first
+        # stage, so that threads staging on a new placer all write into the same dict
+        self._staged_totals = {}
         self._check(self.lib.rbgtopo_create(C.byref(cfg), C.byref(h)))
         self._h = h
         self.n_nodes = 0
@@ -301,7 +304,6 @@ class TopoPlacer:
         blob = _i32(blob)
         h = C.c_int32(-1)
         self._check(self.lib.rbgtopo_stage(self._h, _p(blob), len(blob), C.byref(h)))
-        self._staged_totals = getattr(self, "_staged_totals", {})
         self._staged_totals[h.value] = blob_totals(blob)
         return h.value
 
@@ -310,7 +312,6 @@ class TopoPlacer:
         gb = _i32(groups_blob)
         h = C.c_int32(-1)
         self._check(self.lib.rbgtopo_stage_groups(self._h, _p(gb), len(gb), C.byref(h)))
-        self._staged_totals = getattr(self, "_staged_totals", {})
         self._staged_totals[h.value] = (int(gb[2]), int(gb[4]), 0)   # fetch: per group / per pending replica
         return h.value
 
@@ -332,8 +333,13 @@ class TopoPlacer:
         return assign[:tr], status[:ns], domain[:ns]
 
     def release(self, handle: int) -> None:
-        self._check(self.lib.rbgtopo_release(self._h, handle))
-        self._staged_totals.pop(handle, None)
+        # Handle ids are pool slots: once rbgtopo_release returns, another thread's stage can receive the same id and
+        # store its totals.  Dropping ours first keeps that thread's entry; a refused release puts ours back.
+        totals = self._staged_totals.pop(handle, None)
+        rc = self.lib.rbgtopo_release(self._h, handle)
+        if rc != 0 and totals is not None:
+            self._staged_totals[handle] = totals
+        self._check(rc)
 
     def read_scores(self, handle: int, row: int) -> np.ndarray:
         lo, hi = self.slab()
