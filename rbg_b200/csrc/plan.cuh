@@ -12,7 +12,7 @@
 //   [aux_off, +8*ns)          per step: group, wave, sec_off, sec_end, rep_off, row_off, next_step, i0
 //   [tail_off, +tail_words)   poff[ns + 1], copied behind the plan
 //
-// The wave rule is the one of plugin.py / place_groups_slow (a wave = the next
+// The wave rule is the one of plugin.py / next_wave (a wave = the next
 // <= 32 replicas of <= 8 roles of one dependency level); it is replayed per step
 // from the group's role table, so the host does not ship the wave table either.
 #pragma once

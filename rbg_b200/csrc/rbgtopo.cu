@@ -20,6 +20,7 @@
 #include <memory>
 #include <map>
 #include <mutex>
+#include <optional>
 #include <shared_mutex>
 #include <string>
 #include <vector>
@@ -239,7 +240,7 @@ struct Batch {
   DevBuf<int> lwc;
   PinBuf<int> h_lwc;
   DevBuf<unsigned long long> lw_best;
-  // ranked host-driven wave loops (place_groups_slow, place_groups_lw): the dense rows of every (wave, role), kept
+  // ranked host-driven wave loops (run_waves): the dense rows of every (wave, role), kept
   // across calls like the matrix
   DevBuf<float> kept;
   ~Batch() {
@@ -1895,14 +1896,14 @@ int gen_waves(const int32_t* roles, int q, PlanWave* out) {  // out == nullptr: 
   return walk_waves(roles, q, nullptr, [out](int i, const PlanWave& w) { if (out) out[i] = w; });
 }
 
-// One group while a host-driven loop places its waves (or rank_committed replays them).  Counts are in pods: S pods per
-// replica from rp (place_groups_lw), one without it.
+// One group while a host-driven loop places its waves (run_waves) or rank_committed replays them.  Counts are in pods:
+// S pods per replica from rp (place_groups_lw), one without it.
 struct HostRun {
   const int32_t* rec = nullptr;
   const int32_t* roles = nullptr;  // q x (level, pending, demand, role_flags)
   const int32_t* pair = nullptr;   // q x q
   const int32_t* rp = nullptr;     // (S, C) per role, or nullptr
-  int q = 0, fixed_domain = -1, status = RBGTOPO_PLACED_ALL;
+  int g = 0, q = 0, fixed_domain = -1, status = RBGTOPO_PLACED_ALL;
   bool failed = false;
   int64_t pod0 = 0, pods = 0;                   // the group's pods in assign
   int ord0[RBGTOPO_MAX_GROUP_ROLES] = {0};      // first pod of every role inside the group's range
@@ -1910,12 +1911,12 @@ struct HostRun {
   WaveCursor cur;
   PlanWave w;                         // the wave in flight
   std::vector<int32_t> anchors;       // (node, role, count)*
-  std::vector<int32_t> consumed;      // place_groups_slow: (node, amount)*, one per placed replica
-  std::map<int, int> taken;           // place_groups_lw: node -> amount (committed: earlier groups' claims included)
-  std::vector<int32_t> owner_claims;  // committed, exclusive group: (node, claim gid)* of claimed domains, by node
+  std::vector<int32_t> consumed;      // rp == nullptr: (node, amount)*, one per placed replica
+  std::map<int, int> taken;           // rp != nullptr: node -> amount (committed: earlier groups' claims included)
+  std::vector<int32_t> owner_claims;  // committed at level 0, exclusive group: (node, claim gid)* of claimed domains, by node
   HostRun() = default;
   HostRun(const int32_t* gb, int g, const int32_t* grp, int64_t first_pod)
-      : rec(group_rec(gb, g)), roles(gb + rec[4]), pair(gb + rec[5]), rp(grp), q(rec[3]), fixed_domain(rec[2]),
+      : rec(group_rec(gb, g)), roles(gb + rec[4]), pair(gb + rec[5]), rp(grp), g(g), q(rec[3]), fixed_domain(rec[2]),
         pod0(first_pod) {
     for (int i = 0; i < q; ++i) {
       ord0[i] = (int)pods;
@@ -1927,8 +1928,29 @@ struct HostRun {
   }
   int S(int ri) const { return rp ? rp[2 * ri] : 1; }
   bool done() const { return failed || cur.role >= q; }
+  // The consumed records of the group's next step: without rp one per placed replica; with rp one per node, sorted (what
+  // k_lw_assign relies on).  Only a committed round whose group is re-run later can see claims summing past free[n]
+  // (stale claims of earlier groups), so clamping them to RBGTOPO_MAX_FREE changes no kept result.
+  void step_consumed(std::vector<int32_t>& out) const {
+    if (!rp) {
+      out.assign(consumed.begin(), consumed.end());
+      return;
+    }
+    out.clear();
+    for (const auto& [node, amount] : taken) { out.push_back(node); out.push_back(std::min(amount, RBGTOPO_MAX_FREE)); }
+  }
+  // A pod of role ri placed on node: an anchor (node, ri, 1) of the later waves, and the demand it consumes.
+  void place(int ri, int node) {
+    anchors.push_back(node); anchors.push_back(ri); anchors.push_back(1);
+    if (rp) {
+      taken[node] += roles[4 * ri + 2];
+    } else {
+      consumed.push_back(node); consumed.push_back(roles[4 * ri + 2]);
+    }
+    unplaced[ri] -= 1;
+  }
   // The group's results once its waves are placed: a failed gang places nothing.
-  void results(int g, int32_t* assign, int32_t* status_out, int32_t* domain_out) const {
+  void results(int32_t* assign, int32_t* status_out, int32_t* domain_out) const {
     if (failed) {
       for (int64_t k = pod0; k < pod0 + pods; ++k) assign[k] = -1;
       if (status_out) status_out[g] = RBGTOPO_GANG_FAILED;
@@ -2056,6 +2078,116 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
                    const RankReq& rk, const CommitDev* cm = nullptr, bool cm_levels = false,
                    const HostClaims* hc = nullptr);
 void alt_clear(const RankReq& rk, int64_t first, int64_t count);
+
+rbgtopo_timing add_timing(const rbgtopo_timing& a, const rbgtopo_timing& b) {
+  rbgtopo_timing t = a;
+  t.h2d_ms += b.h2d_ms;
+  t.score_ms += b.score_ms;
+  t.select_ms += b.select_ms;
+  t.d2h_ms += b.d2h_ms;
+  t.total_ms += b.total_ms;
+  t.launches += b.launches;
+  t.h2d_words += b.h2d_words;
+  t.scores += b.scores;
+  t.algo_bytes += b.algo_bytes;
+  return t;
+}
+
+struct KeptRows {  // a ranked host-driven loop: the (wave, role) rows that placed a pod, in b->kept (cap rows reserved)
+  std::vector<AltRow> list;
+  size_t cap = 0, used = 0;
+};
+struct WaveBufs {  // run_waves' host buffers, reused by every wave of a call, across its rounds too
+  StepBlob sb;
+  std::vector<int32_t> w_assign, w_status, w_domain, cons;
+  std::vector<int> active;
+};
+
+// The host-driven wave loop of place_groups_slow and place_groups_lw: per wave, the next wave of every run of
+// runs[lo, end) not yet done becomes one step of a blob, which is staged; launch(active) enqueues the wave's kernels
+// (active: the indices of those runs, in step order), the results come back and every placed pod feeds the later waves
+// of its run.  Once every run is done their results are written.  total sums each wave's timing; keep != nullptr: each
+// wave's dense rows go to b->kept.
+extern "C++" {
+template <class Launch>
+int run_waves(rbgtopo_ctx* c, Batch* b, std::vector<HostRun>& runs, int lo, int32_t* assign, int32_t* status,
+              int32_t* domain, KeptRows* keep, rbgtopo_timing& total, WaveBufs& wb, Launch&& launch) {
+  auto& [sb, w_assign, w_status, w_domain, cons, active] = wb;
+  while (true) {
+    active.clear();
+    for (int i = lo; i < (int)runs.size(); ++i)
+      if (!runs[i].done()) active.push_back(i);
+    if (active.empty()) break;
+    sb.clear();
+    for (int i : active) {
+      HostRun& r = runs[i];
+      next_wave(r.roles, r.q, r.rp, r.cur, r.w);
+      r.step_consumed(cons);
+      sb.add(r, r.w, r.rec[1] & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG),  // as build_plan / k_expand_plan
+             (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) ? r.fixed_domain : -1, r.rec[10], true, cons.data(),
+             (int)(cons.size() / 2));
+    }
+    const std::vector<int32_t>& blob = sb.build();
+    w_assign.resize(sb.racc);
+    w_status.resize(sb.ns);
+    w_domain.resize(sb.ns);
+    const size_t slot0 = keep ? keep->used : 0;  // this wave's rows in b->kept, in matrix order
+    int rc = stage_into(c, b, blob.data(), (int64_t)blob.size());
+    if (!rc) rc = launch(active);
+    if (!rc) rc = fetch_batch(c, b, w_assign.data(), w_status.data(), w_domain.data());
+    if (!rc && keep) rc = keep_wave_rows(c, b, sb.rowacc, keep->cap, &keep->used);
+    if (rc) return rc;
+    {
+      std::lock_guard<std::mutex> g(c->stat_mu);
+      total = add_timing(total, c->last);
+    }
+    int off = 0, row = 0;  // row: the role's dense row in this wave's matrix
+    for (int i = 0; i < sb.ns; ++i) {
+      HostRun& r = runs[active[i]];
+      bool any = false;
+      for (int p = 0; p < r.w.n; ++p, ++row) {
+        const int ri = r.w.role[p], pods = r.w.count[p] * r.S(ri);
+        const int64_t first = r.pod0 + r.ord0[ri] + (int64_t)r.w.first[p] * r.S(ri);
+        bool placed = false;
+        for (int k = 0; k < pods; ++k, ++off) {
+          const int node = w_assign[off];
+          assign[first + k] = node;
+          if (node < 0) continue;
+          any = placed = true;
+          r.place(ri, node);
+        }
+        if (keep && placed) keep->list.push_back(AltRow{(int)slot0 + row, r.g, ri, (int)first, pods});
+      }
+      if ((r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) && w_domain[i] >= 0 && any) r.fixed_domain = w_domain[i];
+      r.status = std::max(r.status, w_status[i]);
+      if ((r.rec[1] & RBGTOPO_STEP_GANG) && w_status[i] != RBGTOPO_PLACED_ALL) r.failed = true;
+    }
+  }
+  for (int i = lo; i < (int)runs.size(); ++i) runs[i].results(assign, status, domain);
+  return RBGTOPO_OK;
+}
+}  // extern "C++"
+
+// The end of a host-driven loop on b, which it releases: after a failure the batch's stream is drained; otherwise total
+// becomes the call's timing and, with keep, the kept rows of every run are ranked now that the placements are final.
+int finish_waves(rbgtopo_ctx* c, Batch* b, int rc, rbgtopo_timing total, const std::vector<HostRun>& runs,
+                 const KeptRows* keep, const int32_t* gb, const int32_t* rp, const int32_t* assign,
+                 const int32_t* status, const int32_t* domain, const RankReq* rk) {
+  if (!rc) {
+    std::lock_guard<std::mutex> g(c->stat_mu);
+    total.base_ms = c->topo.base_ms;
+    c->last = total;
+  } else {
+    cudaStreamSynchronize(stream_of(c, b));
+  }
+  if (!rc && keep) {
+    for (const HostRun& r : runs) alt_clear(*rk, r.pod0, r.pods);
+    rc = run_alternates(c, b, b->kept.p, keep->list, gb, rp, assign, status, domain, *rk);
+    if (rc) cudaStreamSynchronize(stream_of(c, b));
+  }
+  release_batch(c, b);
+  return rc;
+}
 }  // namespace
 
 // The host-driven wave loop: one batched launch pair per wave, placements fed back
@@ -2073,7 +2205,6 @@ static int32_t place_groups_slow(rbgtopo_ctx* c, const int32_t* gb, int64_t word
     return fail(RBGTOPO_ELIMIT, "ranked placement: %d nodes exceed the room bitmap", c->topo.n);
   CK(cudaSetDevice(c->cfg.device));
   auto in = [&](long long off, long long cnt) { return off >= 0 && cnt >= 0 && off + cnt <= words; };
-  std::vector<HostRun> runs(ng);
   long long pacc = 0;
   for (int g = 0; g < ng; ++g) {
     const int32_t* rec = group_rec(gb, g);
@@ -2090,105 +2221,27 @@ static int32_t place_groups_slow(rbgtopo_ctx* c, const int32_t* gb, int64_t word
     }
     if (rec[8] != pacc || rec[9] != pend) return fail(RBGTOPO_EINVAL, "group %d: bad assign_off/n_pending", g);
     pacc += pend;
-    runs[g] = HostRun(gb, g, nullptr, rec[8]);
   }
   if (gb[4] != pacc) return fail(RBGTOPO_EINVAL, "total pending mismatch");
-  size_t kept_cap = 0, kept_used = 0;  // rk: the role rows of the groups placed here
+  std::vector<HostRun> runs;  // the groups placed here; the others keep their results
+  KeptRows kept;              // rk: the role rows of the groups placed here
   for (int g = 0; g < ng; ++g) {
-    if (only && !(*only)[g]) {
-      runs[g].cur.role = runs[g].q;  // not ours: done from the start, results untouched
-      continue;
-    }
-    for (int k = 0; k < runs[g].rec[9]; ++k) assign[runs[g].rec[8] + k] = -1;
-    if (rk) kept_cap += group_role_rows(gb, g, nullptr);
+    if (only && !(*only)[g]) continue;
+    const HostRun& r = runs.emplace_back(gb, g, nullptr, group_rec(gb, g)[8]);
+    for (int64_t k = r.pod0; k < r.pod0 + r.pods; ++k) assign[k] = -1;
+    if (rk) kept.cap += group_role_rows(gb, g, nullptr);
   }
 
   Batch* b = nullptr;
   int rc = acquire_batch(c, &b);
   if (rc) return rc;
-  if (rk) rc = reserve_kept(c, b, kept_cap);
+  if (rk) rc = reserve_kept(c, b, kept.cap);
   rbgtopo_timing total{};
-  StepBlob sb;
-  std::vector<int32_t> w_assign, w_status, w_domain;
-  std::vector<int> active;
-  std::vector<AltRow> kept;  // rk: the (wave, role) rows that placed a replica, in b->kept
-  while (!rc) {
-    active.clear();
-    for (int g = 0; g < ng; ++g)
-      if (!runs[g].done()) active.push_back(g);
-    if (active.empty()) break;
-    // ---- build this wave's step blob
-    sb.clear();
-    for (int g : active) {
-      HostRun& r = runs[g];
-      next_wave(r.roles, r.q, nullptr, r.cur, r.w);
-      sb.add(r, r.w, r.rec[1] & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG),  // as build_plan / k_expand_plan
-             (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) ? r.fixed_domain : -1, r.rec[10], true, r.consumed.data(),
-             (int)(r.consumed.size() / 2));
-    }
-    const std::vector<int32_t>& blob = sb.build();
-    const int ns = sb.ns;
-    w_assign.resize(sb.racc);
-    w_status.resize(ns);
-    w_domain.resize(ns);
-    const size_t slot0 = kept_used;  // this wave's rows in b->kept, in matrix order
-    rc = stage_into(c, b, blob.data(), (int64_t)blob.size());
-    if (!rc) rc = run_batch(c, b, 1);
-    if (!rc) rc = fetch_batch(c, b, w_assign.data(), w_status.data(), w_domain.data());
-    if (!rc && rk) rc = keep_wave_rows(c, b, sb.rowacc, kept_cap, &kept_used);
-    if (rc) break;
-    {
-      std::lock_guard<std::mutex> g(c->stat_mu);
-      total.h2d_ms += c->last.h2d_ms; total.score_ms += c->last.score_ms;
-      total.select_ms += c->last.select_ms; total.d2h_ms += c->last.d2h_ms;
-      total.total_ms += c->last.total_ms; total.launches += c->last.launches;
-      total.scores += c->last.scores; total.algo_bytes += c->last.algo_bytes;
-      total.h2d_words += c->last.h2d_words;
-    }
-    // ---- absorb the placements
-    int off = 0, row = 0;  // row: the role's dense row in this wave's matrix
-    for (int i = 0; i < ns; ++i) {
-      HostRun& r = runs[active[i]];
-      bool any = false;
-      for (int p = 0; p < r.w.n; ++p, ++row) {
-        const int ri = r.w.role[p];
-        const int64_t first = r.pod0 + r.ord0[ri] + r.w.first[p];
-        bool placed = false;
-        for (int k = 0; k < r.w.count[p]; ++k, ++off) {
-          const int node = w_assign[off];
-          assign[first + k] = node;
-          if (node >= 0) {
-            any = true;
-            placed = true;
-            r.anchors.push_back(node); r.anchors.push_back(ri); r.anchors.push_back(1);
-            r.consumed.push_back(node); r.consumed.push_back(r.roles[4 * ri + 2]);
-            r.unplaced[ri] -= 1;
-          }
-        }
-        if (rk && placed) kept.push_back(AltRow{(int)slot0 + row, active[i], ri, (int)first, r.w.count[p]});
-      }
-      if ((r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) && w_domain[i] >= 0 && any) r.fixed_domain = w_domain[i];
-      r.status = std::max(r.status, w_status[i]);
-      if ((r.rec[1] & RBGTOPO_STEP_GANG) && w_status[i] != RBGTOPO_PLACED_ALL) r.failed = true;
-    }
-  }
-  if (!rc) {
-    for (int g = 0; g < ng; ++g)
-      if (!only || (*only)[g]) runs[g].results(g, assign, status, domain);
-    std::lock_guard<std::mutex> g(c->stat_mu);
-    total.base_ms = c->topo.base_ms;
-    c->last = total;
-  } else {
-    cudaStreamSynchronize(stream_of(c, b));
-  }
-  if (!rc && rk) {  // the placements are final now: rank the kept rows
-    for (int g = 0; g < ng; ++g)
-      if (!only || (*only)[g]) alt_clear(*rk, runs[g].rec[8], runs[g].rec[9]);
-    rc = run_alternates(c, b, b->kept.p, kept, gb, nullptr, assign, status, domain, *rk);
-    if (rc) cudaStreamSynchronize(stream_of(c, b));
-  }
-  release_batch(c, b);
-  return rc;
+  WaveBufs wb;
+  if (!rc)
+    rc = run_waves(c, b, runs, 0, assign, status, domain, rk ? &kept : nullptr, total, wb,
+                   [&](const std::vector<int>&) { return run_batch(c, b, 1); });
+  return finish_waves(c, b, rc, total, runs, rk ? &kept : nullptr, gb, nullptr, assign, status, domain, rk);
 }
 
 // ---- device-resident multi-wave plan ------------------------------------------
@@ -3331,22 +3384,6 @@ void plan_results(const Batch* b, int32_t* assign, int32_t* status, int32_t* dom
 }  // namespace
 
 namespace {
-rbgtopo_timing add_timing(const rbgtopo_timing& a, const rbgtopo_timing& b) {
-  rbgtopo_timing t = a;
-  t.h2d_ms += b.h2d_ms;
-  t.score_ms += b.score_ms;
-  t.select_ms += b.select_ms;
-  t.d2h_ms += b.d2h_ms;
-  t.total_ms += b.total_ms;
-  t.launches += b.launches;
-  t.h2d_words += b.h2d_words;
-  t.scores += b.scores;
-  t.algo_bytes += b.algo_bytes;
-  return t;
-}
-}  // namespace
-
-namespace {
 // ---- rbgtopo_place_groups, direct path -------------------------------------------------------------------------------
 // No expanded plan and nothing per step on the host: the GROUPS blob goes up as it came (the upload is enqueued before
 // it is validated: bytes only), the host validates every group, checks the exactness bound and collects a handful of
@@ -3759,13 +3796,12 @@ int place_groups_direct(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_
 // read-back.  Groups up to that lowest group are final, the next round re-runs the groups above it: it only grows, so
 // there are at most n_groups rounds, and a batch whose groups read nothing an earlier group took needs one.  The host
 // validates the blob exactly as the direct path of rbgtopo_place_groups does (same codes).
-int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
-                long long* total_pods);
+int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words);
 
 // The §3.4 bound at one pod per replica: lw_validate's with (S, C) = (1, -1) for every role, which takes every mix of
 // unplaced earlier replicas a later wave can see (§3.10, §3.11 rule 7).  The group table is checked.
 int exact_one_pod(rbgtopo_ctx* c, const int32_t* gb, int64_t words) {
-  long long qsum = 0, pods = 0;
+  long long qsum = 0;
   for (int g = 0; g < gb[2]; ++g) {
     const int q = group_rec(gb, g)[3];
     if (q < 1 || q > RBGTOPO_MAX_GROUP_ROLES) return fail(RBGTOPO_ELIMIT, "group %d: %d roles", g, q);
@@ -3773,7 +3809,7 @@ int exact_one_pod(rbgtopo_ctx* c, const int32_t* gb, int64_t words) {
   }
   std::vector<int32_t> unit(2 * (size_t)qsum);
   for (size_t i = 0; i < unit.size(); i += 2) { unit[i] = 1; unit[i + 1] = -1; }
-  return lw_validate(c, gb, words, unit.data(), (int64_t)unit.size(), &pods);
+  return lw_validate(c, gb, words, unit.data(), (int64_t)unit.size());
 }
 
 // Ranked alternates of a committed batch (DESIGN.md §3.14), once its rounds have converged: the dense row of every
@@ -4141,8 +4177,7 @@ int32_t place_groups_impl(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int3
 namespace {
 // Validation: the checks and messages of rbgtopo_place_groups (group_facts phase 1, offsets), the role_pods table, then
 // group_facts phase 2 (scheduled pods, exactness bound) with the bound taken over the pod waves.
-int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
-                long long* total_pods) {
+int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words) {
   if (const int hrc = check_groups_blob(gb, words)) return hrc;
   const int ng = gb[2];
   const TopoHost th = topo_host(c, places_levels(c));
@@ -4219,7 +4254,6 @@ int lw_validate(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t*
     int rc = group_facts(th, gb, words, g, true, &f, 2, bound);
     if (rc) return rc;
   }
-  *total_pods = pods;
   return RBGTOPO_OK;
 }
 
@@ -4277,27 +4311,27 @@ struct LwLists {
   }
 };
 
-// rk != nullptr: the ranked form (§3.12).  The matrix is overwritten by every wave, so each wave's rows are copied
-// out before the next wave scores (one copy per wave); once the placements are final one k_alternates launch ranks
-// the rows of every (wave, role) that placed a pod.
-// rounds != nullptr: the committed form (§3.13).  A round runs the wave loop for groups [lo, ng); group g sees the
-// claims of groups < g as the previous round left them (final below lo).  c = the lowest group whose claims changed:
-// groups <= c saw their final input, the next round starts at c + 1, and a round that changes nothing ends the call.
-// Both: the committed ranked form (§3.15).  The rounds keep no rows (a re-run would keep its rows again); once they
-// converge, rank_committed replays the rows of every group's final run and ranks them after the whole batch.
-int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
-                    int32_t* assign, int32_t* status, int32_t* domain, const RankReq* rk = nullptr,
-                    int32_t* rounds = nullptr) {
-  long long total_pods = 0;
-  int rc = lw_validate(c, gb, words, rp, rp_words, &total_pods);
-  if (rc) return rc;
-  const Topology& T = c->topo;
-  const int ng = gb[2];
-  // committed at levels (§3.16): a group at a level >= 1 selects the claim lists of commit_owner<true>, over the levels
-  // of the batch's exclusive groups (lmask); a batch at level 0 keeps the record path
+// The committed rounds of a leader-worker batch (§3.13): every group's claims as the latest round left them, and what a
+// round hands the groups it re-runs.  Capacity claims seed a run's `taken`.  Owner claims are, in a batch at level 0,
+// the (node, claim gid) records of every node of a claimed domain, per step in the wave's side table; in a batch with a
+// group at a level >= 1 (§3.16), the claim lists of commit_owner<true> (LwLists) over the levels of the batch's
+// exclusive groups (lmask), read through cm.
+struct LwRounds {
+  const Topology& T;
+  const int32_t* gb;
+  int ng, lmask = 0;
   bool at_lv = false;
-  int lmask = 0;
-  if (rounds)
+  std::vector<LwClaims> claims;
+  std::vector<int> dom_ptr, dom_nodes;  // level 0: the nodes of every level-0 domain
+  std::vector<std::pair<int, int>> oc;  // level 0: a run's owner claims as (node, gid) while seed sorts them
+  LwLists lists;
+  CommitDev cm{};  // at levels: the lists' heads live in cm_int (dhead | phead, all -1 at the start of the call)
+  int lo = 0, n_rounds = 0;  // the round's first group, rounds run
+  int list_launches = 0;
+  long long list_words = 0;
+  size_t sec_at = 0, rec_at = 0;  // the wave's claim section in the side table; at level 0 its records, 8-byte aligned
+  LwRounds(const Topology& topo, const int32_t* groups) : T(topo), gb(groups), ng(groups[2]), claims((size_t)groups[2]) {}
+  int init(const rbgtopo_ctx* c) {
     for (int g = 0; g < ng; ++g) {
       const int32_t* rec = group_rec(gb, g);
       if (rec[10] > 0 && !(c->cfg.flags & RBGTOPO_CFG_LW_COMMIT_LEVELS))
@@ -4306,54 +4340,31 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
       at_lv |= rec[10] > 0;
       if (rec[1] & RBGTOPO_STEP_EXCLUSIVE) lmask |= 1 << rec[10];
     }
-  const size_t smem = (size_t)((T.n + 31) / 32) * 4;
-  if (smem > kFastSmemMax) return fail(RBGTOPO_ELIMIT, "leader-worker placement: %d nodes exceed the room bitmap", T.n);
-  const GroupOffsets off(gb, rp);
-  std::vector<HostRun> runs(ng);
-  auto init_run = [&](int g) {
-    runs[g] = HostRun(gb, g, off.grp(rp, g), off.pod0[g]);
-    for (int64_t k = off.pod0[g]; k < off.pod0[g + 1]; ++k) assign[k] = -1;
-  };
-  const bool keep = rk && !rounds;
-  std::vector<AltRow> kept;  // keep: the (wave, role) rows that placed a pod, in b->kept
-  size_t kept_cap = 0, kept_used = 0;
-  for (int g = 0; g < ng; ++g) {
-    init_run(g);
-    if (keep) kept_cap += group_role_rows(gb, g, off.grp(rp, g));
-  }
-  std::vector<LwClaims> claims(rounds ? ng : 0);  // committed: every group's claims as the latest round left them
-  std::vector<int> dom_ptr, dom_nodes;             // committed at level 0: the nodes of every level-0 domain
-  if (rounds && !at_lv) {
+    if (at_lv) return RBGTOPO_OK;
     dom_ptr.assign((size_t)T.n_domains + 1, 0);
     for (int n = 0; n < T.n; ++n) ++dom_ptr[T.h_domain[n] + 1];
     for (int d = 0; d < T.n_domains; ++d) dom_ptr[d + 1] += dom_ptr[d];
     dom_nodes.resize(T.n);
     std::vector<int> fill(dom_ptr.begin(), dom_ptr.end() - 1);
     for (int n = 0; n < T.n; ++n) dom_nodes[fill[T.h_domain[n]]++] = n;
+    return RBGTOPO_OK;
   }
-  LwLevels lv{};
-  for (int L = 0; L <= installed_levels(c); ++L) lv.nd[L] = level_domains(T, L);
-
-  Batch* b = nullptr;
-  rc = acquire_batch(c, &b);
-  if (rc) return rc;
-  cudaStream_t s = stream_of(c, b);
-  if (keep && (rc = reserve_kept(c, b, kept_cap))) {
-    release_batch(c, b);
-    return rc;
+  // At levels: the dense head arrays in b->cm_int, cleared once per call.
+  int start(Batch* b, cudaStream_t s) {
+    if (!at_lv) return RBGTOPO_OK;
+    CK(b->cm_int.reserve(2 * (size_t)T.lvl_total_d));
+    CK(cudaMemsetAsync(b->cm_int.p, 0xFF, 2 * (size_t)T.lvl_total_d * 4, s));
+    cm.dhead = b->cm_int.p;
+    cm.phead = b->cm_int.p + T.lvl_total_d;
+    cm.ldom = T.lvl_domain.p;
+    cm.doff = T.lvl_doff.p;
+    cm.lstride = level_stride(T.n);
+    cm.lmask = lmask;
+    cm.occ = true;  // levels >= 1 exist in occupancy mode only
+    return RBGTOPO_OK;
   }
-  rbgtopo_timing total{};
-  StepBlob sb;
-  std::vector<int32_t> w_assign, w_status, w_domain, side, cons;
-  std::vector<int> active;
-  std::vector<std::pair<int, int>> oc;
-  int lo = 0, n_rounds = 0;  // committed: the round's first group, rounds run
-  // at_lv: the lists' heads live in cm_int (dhead | phead, all -1 at the start of the call); cm reads them
-  LwLists lists;
-  CommitDev cm{};
-  int list_launches = 0;
-  long long list_words = 0;
-  auto upload_lists = [&]() -> int {
+  // At levels: the lists of the current claims, with the heads that changed written by k_set_heads.
+  int upload(Batch* b, cudaStream_t s) {
     lists.build(T, gb, claims, lmask);
     std::vector<int2> set;
     for (const auto& [slot, first] : lists.heads) set.push_back(make_int2(slot, first));
@@ -4377,237 +4388,211 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
     cm.pclaim = reinterpret_cast<int4*>(b->lwc.p + o_p);
     list_words += (long long)w;
     return RBGTOPO_OK;
-  };
-  if (at_lv) {
-    rc = [&]() -> int {
-      CK(b->cm_int.reserve(2 * (size_t)T.lvl_total_d));
-      CK(cudaMemsetAsync(b->cm_int.p, 0xFF, 2 * (size_t)T.lvl_total_d * 4, s));
-      return RBGTOPO_OK;
-    }();
-    if (rc) {
-      release_batch(c, b);
-      return rc;
-    }
-    cm.dhead = b->cm_int.p;
-    cm.phead = b->cm_int.p + T.lvl_total_d;
-    cm.ldom = T.lvl_domain.p;
-    cm.doff = T.lvl_doff.p;
-    cm.lstride = level_stride(T.n);
-    cm.lmask = lmask;
-    cm.occ = true;  // levels >= 1 exist in occupancy mode only
   }
-  for (bool more = true; more;) {
-    more = false;
-    if (rounds && at_lv && (rc = upload_lists())) break;
-    if (rounds) {  // every group of the round starts from the claims of the groups before it
-      std::map<int, int> cap, own;  // node -> capacity taken; level-0 domain -> gid of its last reporter
-      for (int g = 0; g < ng; ++g) {
-        if (g >= lo) {
-          if (n_rounds > 0) init_run(g);
-          HostRun& r = runs[g];
-          r.taken = cap;
-          if (!at_lv && (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE)) {
-            oc.clear();
-            for (const auto& [d, gid] : own)
-              for (int k = dom_ptr[d]; k < dom_ptr[d + 1]; ++k) oc.emplace_back(dom_nodes[k], gid);
-            std::sort(oc.begin(), oc.end());
-            for (const auto& [n, gid] : oc) { r.owner_claims.push_back(n); r.owner_claims.push_back(gid); }
-          }
+  // The start of a round: every run of [lo, ng) starts from the claims of the groups before it.
+  int seed(std::vector<HostRun>& runs, Batch* b, cudaStream_t s) {
+    if (at_lv)
+      if (const int rc = upload(b, s)) return rc;
+    std::map<int, int> cap, own;  // node -> capacity taken; level-0 domain -> gid of its last reporter
+    for (int g = 0; g < ng; ++g) {
+      if (g >= lo) {
+        HostRun& r = runs[g];
+        r.taken = cap;
+        if (!at_lv && (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE)) {
+          oc.clear();
+          for (const auto& [d, gid] : own)
+            for (int k = dom_ptr[d]; k < dom_ptr[d + 1]; ++k) oc.emplace_back(dom_nodes[k], gid);
+          std::sort(oc.begin(), oc.end());
+          for (const auto& [n, gid] : oc) { r.owner_claims.push_back(n); r.owner_claims.push_back(gid); }
         }
-        for (const auto& [n, a] : claims[g].cap) cap[n] += a;
-        if (claims[g].dom >= 0) own[claims[g].dom] = claims[g].gid;
       }
+      for (const auto& [n, a] : claims[g].cap) cap[n] += a;
+      if (claims[g].dom >= 0) own[claims[g].dom] = claims[g].gid;
     }
-    while (true) {
-      active.clear();
-      for (int g = lo; g < ng; ++g)
-        if (!runs[g].done()) active.push_back(g);
-      if (active.empty()) break;
-      // ---- this wave's step blob: role counts in pods, need over unplaced pods
-      const int ns = (int)active.size();
-      sb.clear();
-      side.assign((size_t)ns * MAXP, 0);
-      int dmax = 0;
-      for (int i = 0; i < ns; ++i) {
-        HostRun& r = runs[active[i]];
-        next_wave(r.roles, r.q, r.rp, r.cur, r.w);
-        for (int p = 0; p < r.w.n; ++p) {
-          const int ri = r.w.role[p], C = r.rp[2 * ri + 1];
-          side[(size_t)i * MAXP + p] = lw_pack_role(r.S(ri), C);
-          if (C >= 0) dmax = std::max(dmax, lv.nd[C]);
-        }
-        // consumed records by node, one per node.  Only a committed round whose group is re-run later can see claims
-        // summing past free[n] (stale claims of earlier groups), so clamping them to RBGTOPO_MAX_FREE changes no kept result
-        cons.clear();
-        for (const auto& kv : r.taken) { cons.push_back(kv.first); cons.push_back(std::min(kv.second, RBGTOPO_MAX_FREE)); }
-        sb.add(r, r.w, r.rec[1] & (RBGTOPO_STEP_EXCLUSIVE | RBGTOPO_STEP_GANG),
-               (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) ? r.fixed_domain : -1, r.rec[10], true, cons.data(), (int)r.taken.size());
-      }
-      const std::vector<int32_t>& blob = sb.build();
-      const int racc = sb.racc, rowacc = sb.rowacc;
-      // committed: per step the offsets of its owner claims, then the (node, gid) records, 8-byte aligned; at levels
-      // the group index of every step instead
-      size_t claim_at = 0, rec_at = 0;
-      if (rounds && at_lv) {
-        claim_at = side.size();
-        side.insert(side.end(), active.begin(), active.end());
-      } else if (rounds) {
-        claim_at = side.size();
-        int acc = 0;
-        side.push_back(0);
-        for (int i = 0; i < ns; ++i) side.push_back(acc += (int)runs[active[i]].owner_claims.size() / 2);
-        if (side.size() & 1) side.push_back(0);
-        rec_at = side.size();
-        for (int i = 0; i < ns; ++i) side.insert(side.end(), runs[active[i]].owner_claims.begin(), runs[active[i]].owner_claims.end());
-      }
-      w_assign.resize(racc);
-      w_status.resize(ns);
-      w_domain.resize(ns);
-      rc = stage_into(c, b, blob.data(), (int64_t)blob.size());
-      if (rc) break;
-      rc = [&]() -> int {
-        // grid: every step resident at once if the device holds them, the level-C scratch bounded by kLwScratchBytes
-        int per_sm = 0;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_lw_assign, LW_THREADS, smem));
-        long long grid = std::min<long long>(ns, (long long)std::max(1, per_sm) * c->sm_count);
-        if (dmax > 0) grid = std::min<long long>(grid, std::max<long long>(1, kLwScratchBytes / (12LL * dmax)));
-        CK(b->lw.reserve(side.size()));
-        CK(b->h_lw.reserve(side.size()));
-        CK(b->lw_best.reserve((size_t)grid * dmax + 1));
-        CK(b->lw_cap.reserve((size_t)grid * dmax + 1));
-        memcpy(b->h_lw.p, side.data(), side.size() * 4);
-        CK(cudaMemcpyAsync(b->lw.p, b->h_lw.p, side.size() * 4, cudaMemcpyHostToDevice, s));
-        CK(cudaStreamWaitEvent(s, c->base_ready, 0));  // a pending snapshot refresh
-        CK(cudaStreamWaitEvent(s, c->topo_ready, 0));
-        int r2 = rounds && at_lv ? launch_score(c, b, s, nullptr, nullptr, b->lw.p + claim_at, &cm)
-                 : rounds     ? launch_score(c, b, s, b->lw.p + claim_at, reinterpret_cast<const int2*>(b->lw.p + rec_at))
-                              : launch_score(c, b, s);
-        if (r2) return r2;
-        k_lw_assign<<<(unsigned)grid, LW_THREADS, smem, s>>>(topo_dev(c), batch_dev(c, b), b->lw.p, b->lw_best.p,
-                                                             b->lw_cap.p, dmax, lv);
-        CK(cudaGetLastError());
-        b->pend_launches += 2;
-        b->ran = true;
-        return RBGTOPO_OK;
-      }();
-      if (!rc) rc = fetch_batch(c, b, w_assign.data(), w_status.data(), w_domain.data());
-      const size_t slot0 = kept_used;  // this wave's rows in b->kept, in matrix order
-      if (!rc && keep) rc = keep_wave_rows(c, b, rowacc, kept_cap, &kept_used);
-      if (rc) break;
-      {
-        std::lock_guard<std::mutex> g(c->stat_mu);
-        c->launches += 2;
-        total.h2d_ms += c->last.h2d_ms; total.d2h_ms += c->last.d2h_ms;
-        total.total_ms += c->last.total_ms; total.launches += c->last.launches;
-        total.scores += c->last.scores; total.algo_bytes += c->last.algo_bytes;
-        total.h2d_words += c->last.h2d_words;
-      }
-      // ---- absorb the placements: every pod placed is an anchor (node, role, 1) and consumes (node, demand)
-      int off = 0, row = 0;  // row: the role's dense row in this wave's matrix
-      for (int i = 0; i < ns; ++i) {
-        HostRun& r = runs[active[i]];
-        bool any = false;
-        for (int p = 0; p < r.w.n; ++p, ++row) {
-          const int ri = r.w.role[p], S = r.S(ri);
-          const int64_t first = r.pod0 + r.ord0[ri] + (int64_t)r.w.first[p] * S;
-          bool placed = false;
-          for (int k = 0; k < r.w.count[p] * S; ++k, ++off) {
-            const int node = w_assign[off];
-            assign[first + k] = node;
-            if (node < 0) continue;
-            any = placed = true;
-            r.anchors.push_back(node); r.anchors.push_back(ri); r.anchors.push_back(1);
-            r.taken[node] += r.roles[4 * ri + 2];
-            r.unplaced[ri] -= 1;
-          }
-          if (keep && placed) kept.push_back(AltRow{(int)slot0 + row, active[i], ri, (int)first, r.w.count[p] * S});
-        }
-        if ((r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) && w_domain[i] >= 0 && any) r.fixed_domain = w_domain[i];
-        r.status = std::max(r.status, w_status[i]);
-        if ((r.rec[1] & RBGTOPO_STEP_GANG) && w_status[i] != RBGTOPO_PLACED_ALL) r.failed = true;
-      }
+    return RBGTOPO_OK;
+  }
+  // The claim section of a wave's side table (active: the steps' groups): at levels the group index of every step; at
+  // level 0 per step the offsets of its owner claims, then the (node, gid) records.
+  void add_side(const std::vector<HostRun>& runs, const std::vector<int>& active, std::vector<int32_t>& side) {
+    sec_at = side.size();
+    if (at_lv) {
+      side.insert(side.end(), active.begin(), active.end());
+      return;
     }
-    if (rc) break;
-    for (int g = lo; g < ng; ++g) runs[g].results(g, assign, status, domain);
-    if (rounds) {
-      ++n_rounds;
-      int cmin = -1;  // the lowest group whose claims differ from what the groups after it saw
-      for (int g = lo; g < ng; ++g) {
-        const HostRun& r = runs[g];
-        LwClaims nc;
-        if (!r.failed) {
-          std::map<int, int> cap;
+    int acc = 0;
+    side.push_back(0);
+    for (int i : active) side.push_back(acc += (int)runs[i].owner_claims.size() / 2);
+    if (side.size() & 1) side.push_back(0);
+    rec_at = side.size();
+    for (int i : active) side.insert(side.end(), runs[i].owner_claims.begin(), runs[i].owner_claims.end());
+  }
+  // The wave's dense rows, with the owner claims of the earlier groups (lw: the side table on the device).
+  int score(rbgtopo_ctx* c, Batch* b, cudaStream_t s, const int* lw) const {
+    return at_lv ? launch_score(c, b, s, nullptr, nullptr, lw + sec_at, &cm)
+                 : launch_score(c, b, s, lw + sec_at, reinterpret_cast<const int2*>(lw + rec_at));
+  }
+  // The end of a round: the new claims of the groups it ran.  c = the lowest group whose claims changed; groups <= c
+  // saw their final input.  Returns whether another round is needed; it starts at c + 1.
+  bool settle(const std::vector<HostRun>& runs, const int32_t* assign) {
+    ++n_rounds;
+    int cmin = -1;
+    for (int g = lo; g < ng; ++g) {
+      const HostRun& r = runs[g];
+      LwClaims nc;
+      if (!r.failed) {
+        std::map<int, int> cap;
+        for (int i = 0; i < r.q; ++i)
+          for (long long k = 0; k < (long long)r.roles[4 * i + 1] * r.rp[2 * i]; ++k)
+            if (const int node = assign[r.pod0 + r.ord0[i] + k]; node >= 0) cap[node] += r.roles[4 * i + 2];
+        nc.cap.assign(cap.begin(), cap.end());
+        if ((r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) && r.fixed_domain >= 0) {
+          nc.dom = r.fixed_domain;
+          nc.gid = r.rec[0];
+        }
+        if (at_lv && (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE)) {  // the placed pods of its participating roles
           for (int i = 0; i < r.q; ++i)
-            for (long long k = 0; k < (long long)r.roles[4 * i + 1] * r.rp[2 * i]; ++k)
-              if (const int node = assign[r.pod0 + r.ord0[i] + k]; node >= 0) cap[node] += r.roles[4 * i + 2];
-          nc.cap.assign(cap.begin(), cap.end());
-          if ((r.rec[1] & RBGTOPO_STEP_EXCLUSIVE) && r.fixed_domain >= 0) {
-            nc.dom = r.fixed_domain;
-            nc.gid = r.rec[0];
-          }
-          if (at_lv && (r.rec[1] & RBGTOPO_STEP_EXCLUSIVE)) {  // the placed pods of its participating roles
-            for (int i = 0; i < r.q; ++i)
-              if (r.roles[4 * i + 3] & RBGTOPO_ROLE_EXCLUSIVE)
-                for (long long k = 0; k < (long long)r.roles[4 * i + 1] * r.rp[2 * i]; ++k)
-                  if (const int node = assign[r.pod0 + r.ord0[i] + k]; node >= 0) nc.pods.push_back(node);
-            std::sort(nc.pods.begin(), nc.pods.end());
-            if (!nc.pods.empty()) nc.gid = r.rec[0];
-          }
+            if (r.roles[4 * i + 3] & RBGTOPO_ROLE_EXCLUSIVE)
+              for (long long k = 0; k < (long long)r.roles[4 * i + 1] * r.rp[2 * i]; ++k)
+                if (const int node = assign[r.pod0 + r.ord0[i] + k]; node >= 0) nc.pods.push_back(node);
+          std::sort(nc.pods.begin(), nc.pods.end());
+          if (!nc.pods.empty()) nc.gid = r.rec[0];
         }
-        if (cmin < 0 && !(nc == claims[g])) cmin = g;
-        claims[g] = std::move(nc);
       }
-      if (cmin >= 0 && cmin + 1 < ng) {
-        lo = cmin + 1;
-        more = true;
-      }
+      if (cmin < 0 && !(nc == claims[g])) cmin = g;
+      claims[g] = std::move(nc);
     }
+    if (cmin < 0 || cmin + 1 >= ng) return false;
+    lo = cmin + 1;
+    return true;
   }
-  if (rounds) *rounds = n_rounds;
-  if (!rc && rk && rounds && at_lv) {  // the claims are final now: the lists of every group for commit_owner<true>
-    rc = upload_lists();
-    cm.g = ng;
+  // The end of the rounds, which ended with rc.  rk: the committed ranked form (§3.15), rank_committed against every
+  // group's final claims, the lists of commit_owner<true> at levels, and at level 0 the owner lists of
+  // commit_owner<false> (HostClaims), which are LwLists' dhead / dclaim.  What the claim lists took (k_set_heads
+  // launches, uploaded words) counts toward a call that succeeds.
+  int finish(rbgtopo_ctx* c, Batch* b, int rc, const int32_t* rp, const int32_t* assign, const int32_t* status,
+             const int32_t* domain, const RankReq* rk, rbgtopo_timing& total) {
     int rank_launches = 0;
-    if (!rc) rc = rank_committed(c, b, gb, rp, assign, status, domain, cm, true, *rk, &rank_launches);
-    total.launches += rank_launches;
-    std::lock_guard<std::mutex> g(c->stat_mu);
-    c->launches += rank_launches;
-  } else if (!rc && rk && rounds) {  // the claims are final now: level-0 owner lists for commit_owner<false>, then the replay
-    HostClaims hc;
-    hc.dhead.assign((size_t)T.n_domains, -1);
-    hc.dclaim.assign((size_t)std::max(ng, 1), make_int2(-1, -1));
-    for (int g = 0; g < ng; ++g)
-      if (claims[g].dom >= 0) {
-        hc.dclaim[g] = make_int2(claims[g].gid, hc.dhead[claims[g].dom]);
-        hc.dhead[claims[g].dom] = g;
+    if (!rc && rk) {
+      HostClaims hc;
+      if (at_lv) {
+        rc = upload(b, stream_of(c, b));
+      } else {
+        lists.build(T, gb, claims, lmask);
+        hc.dhead.assign((size_t)T.n_domains, -1);
+        for (const auto& [d, first] : lists.heads) hc.dhead[d] = first;
+        hc.dclaim = std::move(lists.dclaim);
+        cm.occ = T.occ;
       }
-    CommitDev cm{};
-    cm.g = ng;
-    cm.occ = T.occ;
-    int rank_launches = 0;
-    rc = rank_committed(c, b, gb, rp, assign, status, domain, cm, false, *rk, &rank_launches, &hc);
+      cm.g = ng;
+      if (!rc)
+        rc = rank_committed(c, b, gb, rp, assign, status, domain, cm, at_lv, *rk, &rank_launches, at_lv ? nullptr : &hc);
+    }
+    std::lock_guard<std::mutex> g(c->stat_mu);
     total.launches += rank_launches;
-    std::lock_guard<std::mutex> g(c->stat_mu);
     c->launches += rank_launches;
-  }
-  if (!rc) {
-    harvest_base_ms(c);
-    std::lock_guard<std::mutex> g(c->stat_mu);
-    total.base_ms = c->topo.base_ms;
+    if (rc) return rc;
     total.launches += list_launches;
     total.h2d_words += (int32_t)std::min<long long>(list_words, INT32_MAX);
     c->launches += list_launches;
-    c->last = total;
-  } else {
-    cudaStreamSynchronize(s);
+    return RBGTOPO_OK;
   }
-  if (!rc && keep) {  // the placements are final now: rank the kept rows
-    alt_clear(*rk, 0, total_pods);
-    rc = run_alternates(c, b, b->kept.p, kept, gb, rp, assign, status, domain, *rk);
-    if (rc) cudaStreamSynchronize(s);
+};
+
+// rk != nullptr: the ranked form (§3.12).  The matrix is overwritten by every wave, so each wave's rows are copied
+// out before the next wave scores (one copy per wave); once the placements are final one k_alternates launch ranks
+// the rows of every (wave, role) that placed a pod.
+// rounds != nullptr: the committed form (§3.13, LwRounds).  A round runs the wave loop for groups [lo, ng); group g
+// sees the claims of groups < g as the previous round left them (final below lo).  c = the lowest group whose claims
+// changed: groups <= c saw their final input, the next round starts at c + 1, and a round that changes nothing ends
+// the call.
+// Both: the committed ranked form (§3.15).  The rounds keep no rows (a re-run would keep its rows again); once they
+// converge, rank_committed replays the rows of every group's final run and ranks them after the whole batch.
+int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
+                    int32_t* assign, int32_t* status, int32_t* domain, const RankReq* rk = nullptr,
+                    int32_t* rounds = nullptr) {
+  int rc = lw_validate(c, gb, words, rp, rp_words);
+  if (rc) return rc;
+  const Topology& T = c->topo;
+  const int ng = gb[2];
+  std::optional<LwRounds> cr;  // the committed rounds
+  if (rounds && (rc = cr.emplace(T, gb).init(c))) return rc;
+  const size_t smem = (size_t)((T.n + 31) / 32) * 4;
+  if (smem > kFastSmemMax) return fail(RBGTOPO_ELIMIT, "leader-worker placement: %d nodes exceed the room bitmap", T.n);
+  const GroupOffsets off(gb, rp);
+  std::vector<HostRun> runs(ng);
+  auto init_run = [&](int g) {
+    runs[g] = HostRun(gb, g, off.grp(rp, g), off.pod0[g]);
+    for (int64_t k = off.pod0[g]; k < off.pod0[g + 1]; ++k) assign[k] = -1;
+  };
+  const bool keep = rk && !rounds;
+  KeptRows kept;
+  for (int g = 0; g < ng; ++g) {
+    init_run(g);
+    if (keep) kept.cap += group_role_rows(gb, g, off.grp(rp, g));
   }
-  release_batch(c, b);
-  return rc;
+  LwLevels lv{};
+  for (int L = 0; L <= installed_levels(c); ++L) lv.nd[L] = level_domains(T, L);
+
+  Batch* b = nullptr;
+  rc = acquire_batch(c, &b);
+  if (rc) return rc;
+  cudaStream_t s = stream_of(c, b);
+  if (keep) rc = reserve_kept(c, b, kept.cap);
+  if (!rc && cr) rc = cr->start(b, s);
+  std::vector<int32_t> side;  // per wave: the (S, C) of every role row of every step, then the claim section
+  auto launch = [&](const std::vector<int>& active) -> int {
+    const int ns = (int)active.size();
+    side.assign((size_t)ns * MAXP, 0);
+    int dmax = 0;
+    for (int i = 0; i < ns; ++i) {
+      const HostRun& r = runs[active[i]];
+      for (int p = 0; p < r.w.n; ++p) {
+        const int ri = r.w.role[p], C = r.rp[2 * ri + 1];
+        side[(size_t)i * MAXP + p] = lw_pack_role(r.S(ri), C);
+        if (C >= 0) dmax = std::max(dmax, lv.nd[C]);
+      }
+    }
+    if (cr) cr->add_side(runs, active, side);
+    // grid: every step resident at once if the device holds them, the level-C scratch bounded by kLwScratchBytes
+    int per_sm = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_lw_assign, LW_THREADS, smem));
+    long long grid = std::min<long long>(ns, (long long)std::max(1, per_sm) * c->sm_count);
+    if (dmax > 0) grid = std::min<long long>(grid, std::max<long long>(1, kLwScratchBytes / (12LL * dmax)));
+    CK(b->lw.reserve(side.size()));
+    CK(b->h_lw.reserve(side.size()));
+    CK(b->lw_best.reserve((size_t)grid * dmax + 1));
+    CK(b->lw_cap.reserve((size_t)grid * dmax + 1));
+    memcpy(b->h_lw.p, side.data(), side.size() * 4);
+    CK(cudaMemcpyAsync(b->lw.p, b->h_lw.p, side.size() * 4, cudaMemcpyHostToDevice, s));
+    CK(cudaStreamWaitEvent(s, c->base_ready, 0));  // a pending snapshot refresh
+    CK(cudaStreamWaitEvent(s, c->topo_ready, 0));
+    if (const int r2 = cr ? cr->score(c, b, s, b->lw.p) : launch_score(c, b, s)) return r2;
+    k_lw_assign<<<(unsigned)grid, LW_THREADS, smem, s>>>(topo_dev(c), batch_dev(c, b), b->lw.p, b->lw_best.p,
+                                                         b->lw_cap.p, dmax, lv);
+    CK(cudaGetLastError());
+    b->pend_launches += 2;
+    b->ran = true;
+    std::lock_guard<std::mutex> g(c->stat_mu);
+    c->launches += 2;
+    return RBGTOPO_OK;
+  };
+  rbgtopo_timing total{};
+  WaveBufs wb;
+  while (!rc) {  // the rounds; one when not committed
+    if (cr && (rc = cr->seed(runs, b, s))) break;
+    rc = run_waves(c, b, runs, cr ? cr->lo : 0, assign, status, domain, keep ? &kept : nullptr, total, wb, launch);
+    if (rc || !cr || !cr->settle(runs, assign)) break;
+    for (int g = cr->lo; g < ng; ++g) init_run(g);
+  }
+  if (cr) {
+    *rounds = cr->n_rounds;
+    rc = cr->finish(c, b, rc, rp, assign, status, domain, rk, total);
+  }
+  if (!rc) harvest_base_ms(c);
+  // The waves record no pass events, so their pass times are 0, unless the pooled batch still holds those of a staged
+  // pass released without a fetch; those are not this call's.
+  total.score_ms = total.select_ms = 0.f;
+  return finish_waves(c, b, rc, total, runs, keep ? &kept : nullptr, gb, rp, assign, status, domain, rk);
 }
 
 // The entry checks of every rbgtopo_place_groups* function, in this order: rounds = 0, null arguments, n_alt, world
