@@ -340,7 +340,8 @@ int32_t rbgtopo_place_groups_committed(rbgtopo_ctx* ctx, const int32_t* groups, 
  * gang-failed group get score -inf and no alternates.  n_alt in [0, RBGTOPO_MAX_ALTERNATES], else
  * RBGTOPO_EINVAL; alt_node / alt_score may be NULL when n_alt == 0.
  * Documented limits (RBGTOPO_ELIMIT): a ctx with world > 1 (a rank holds only its slab of every dense
- * row), and more nodes than a shared-memory room bitmap of 200 KB holds (1 638 400).  Both are checked
+ * row: the sharded form is rbgtopo_shard_place_groups_ranked + rbgtopo_shard_alternates_merge, §3.17),
+ * and more nodes than a shared-memory room bitmap of 200 KB holds (1 638 400).  Both are checked
  * before anything is placed: nothing is written then, and the call never fails once it has placed.
  * Exactness (§3.4) is checked before anything is placed too, with the bound rbgtopo_place_groups_lw
  * applies with one pod per replica: a non-gang group the host-driven loop re-runs reaches waves after
@@ -372,13 +373,51 @@ int32_t rbgtopo_place_groups_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int
  * rbgtopo_place_groups_lw checks it with one pod per replica: a non-gang group can reach a wave after unplaced
  * replicas, so such a group can be refused with RBGTOPO_EINEXACT a little below the bound
  * rbgtopo_place_groups_committed applies; nothing is written then, and the call never fails once it has placed.
- * Documented limits (RBGTOPO_ELIMIT): a ctx with world > 1 (a rank holds only its slab of every dense row), more
+ * Documented limits (RBGTOPO_ELIMIT): a ctx with world > 1 (a rank holds only its slab of every dense row: the
+ * sharded form is rbgtopo_shard_place_groups_committed_ranked + rbgtopo_shard_alternates_merge, §3.17), more
  * nodes than a shared-memory room bitmap of 200 KB holds (1 638 400), and a group table that does not fit
  * k_plan_group, as for rbgtopo_place_groups_committed.  The ranked form of a committed leader-worker batch is
  * rbgtopo_place_groups_lw_committed_ranked. */
 int32_t rbgtopo_place_groups_committed_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
                                               int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain,
                                               int32_t* rounds, float* score, int32_t* alt_node, float* alt_score);
+
+/* Ranked alternates on node-axis shards (DESIGN.md §3.17): the ranked placement of one blob split over the ranks
+ * of a world, with one all-gather by the CALLER between two halves.  The library has no transport of its own here
+ * and never waits on a peer.
+ *
+ * Local half, valid for any world (world = 1 included): rbgtopo_shard_place_groups_ranked takes the inputs of
+ * rbgtopo_place_groups_ranked and rbgtopo_shard_place_groups_committed_ranked those of
+ * rbgtopo_place_groups_committed_ranked: same GROUPS blob, validation, exactness check, levels and config rules,
+ * room-bitmap limit on the node count (1 638 400, whatever the world) and error codes, every check before anything
+ * is placed.  assign / status / domain / *rounds are what rbgtopo_place_groups / _committed give, on every rank
+ * (status / domain / rounds may be NULL).  Each rank then ranks every (wave, role) row on its own slab and returns
+ * *xhandle, and *keys_dev / *keys_bytes: its exchange buffer in device memory, owned by the library, complete when
+ * the call returns.  keys_bytes = 72 per ranked row plus 4 per replica, padded to 8 (at least 8); it is the same on
+ * every rank, because the rows follow from the replicated placements.
+ *
+ * Merge half: keys_all_dev = world x keys_bytes in device memory, rank-major (what an all-gather of the exchange
+ * buffers produces).  rbgtopo_shard_alternates_merge fills score[R] / alt_node[R * n_alt] / alt_score[R * n_alt] in
+ * assign order, bit-identical on every rank to what rbgtopo_place_groups_ranked / _committed_ranked give on a
+ * world = 1 ctx with the same snapshot: -1 / -inf fill, unplaced and gang-failed replicas included.  It runs on the
+ * ctx's stream (rbgtopo_set_stream), so an all-gather enqueued on that stream needs no other synchronisation; it
+ * reads no snapshot state (slab bounds and the replica map are kept in the handle), so a refresh between the two
+ * halves does not change its result; it synchronises before it returns.
+ *
+ * The merge consumes the handle, also when it fails on the device; rbgtopo_release frees a handle that will not be
+ * merged (the collective failed, say).  A second merge of the same handle, a staged-batch handle or a NULL argument
+ * is RBGTOPO_EINVAL (the handle stays valid after NULL arguments).  Several exchanges may be in flight on one ctx.
+ * Neither half fails once it has placed, except on a device error (RBGTOPO_ECUDA) and the merge's EINVAL.
+ * Leader-worker forms are not sharded: rbgtopo_place_groups_lw* keep RBGTOPO_ELIMIT at world > 1. */
+int32_t rbgtopo_shard_place_groups_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                          int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain,
+                                          int32_t* xhandle, void** keys_dev, int64_t* keys_bytes);
+int32_t rbgtopo_shard_place_groups_committed_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                                    int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain,
+                                                    int32_t* rounds, int32_t* xhandle, void** keys_dev,
+                                                    int64_t* keys_bytes);
+int32_t rbgtopo_shard_alternates_merge(rbgtopo_ctx* ctx, int32_t xhandle, const void* keys_all_dev, float* score,
+                                       int32_t* alt_node, float* alt_score);
 
 /* Leader-worker replicas (DESIGN.md §3.11).  The GROUPS blob of rbgtopo_place_groups — same validation and
  * error codes — where a replica of a role can be several pods (a leaderWorkerPattern of size S: one leader and

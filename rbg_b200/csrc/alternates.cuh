@@ -19,6 +19,12 @@
 // k_alternates_commit_coloc ranks the pod rows of a committed leader-worker batch
 // (rbgtopo_place_groups_lw_committed_ranked, §3.15) that has a co-location domain: both conditions at once;
 // k_alternates_commit_coloc_lv the same at exclusive levels (§3.16).
+//
+// Node-axis shards (rbgtopo_shard_place_groups*_ranked, §3.17): k_alternates_slab ranks a job on this rank's slab of
+// its row and writes the job's ALT_LIST best keys of the slab, plus S_r[assign[r]] of every replica whose node lies in
+// the slab; after the caller's all-gather, k_alternates_merge merges the world lists of every job into the replicas'
+// lists.  The global top ALT_LIST of a job lies in the union of the per-slab top ALT_LIST lists, so the result is the
+// world = 1 ranking bit for bit.
 #pragma once
 #include "kernels.cuh"
 #include "plan_group.cuh"
@@ -65,7 +71,11 @@ __device__ __forceinline__ void alt_insert(unsigned long long (&top)[ALT_LIST], 
 // COMMIT: gids[job] = the job's group gid; LV: the batch has a group at a level >= 1 (commit_owner<LV>).  COMMIT with
 // COLOC: k_alternates_commit_coloc and, at levels, k_alternates_commit_coloc_lv; the other forms keep the registers
 // they had without it.
-template <bool COLOC, bool COMMIT, bool LV>
+// SLAB (k_alternates_slab, §3.17): the rows are this rank's slab [t.slab_lo, t.slab_hi) of the dense rows (node m at
+// m - slab_lo; slab_lo is a multiple of 128, so the domain vectors, read by global node, stay 16-byte aligned), the
+// room bitmap covers the slab, and `out` is the job's exchange record: ALT_LIST keys per job (u64, job-major), then one
+// score per compact replica at out + 2 * ALT_LIST * gridDim.x (S_r[own] where own lies in the slab, else -inf).
+template <bool COLOC, bool COMMIT, bool LV, bool SLAB = false>
 __device__ __forceinline__ void alternates_body(TopoDev t, const float* __restrict__ rows,
                                                 const AltJob* __restrict__ jobs, const int2* __restrict__ used,
                                                 const int* __restrict__ own, int n_alt, int* __restrict__ out,
@@ -75,13 +85,16 @@ __device__ __forceinline__ void alternates_body(TopoDev t, const float* __restri
   __shared__ unsigned long long sTop[ALT_LIST];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const AltJob J = jobs[blockIdx.x];
-  const int n = t.n;
-  const int words = (n + 31) >> 5;
+  const int lo = SLAB ? t.slab_lo : 0;  // nodes [lo, n) of the row, node m at m - lo
+  const int n = SLAB ? t.slab_hi : t.n;
+  const int words = (n - lo + 31) >> 5;
   for (int i = tid; i < words; i += ALT_THREADS) sFull[i] = 0;
   __syncthreads();
   for (int i = tid; i < J.nused; i += ALT_THREADS) {
     const int2 u = __ldg(used + J.used0 + i);
-    if (__ldg(t.free_ + u.x) - u.y < J.demand) atomicOr(&sFull[u.x >> 5], 1u << (u.x & 31));
+    if constexpr (SLAB)
+      if (u.x < lo || u.x >= n) continue;
+    if (__ldg(t.free_ + u.x) - u.y < J.demand) atomicOr(&sFull[(u.x - lo) >> 5], 1u << ((u.x - lo) & 31));
   }
   __syncthreads();
 
@@ -93,10 +106,10 @@ __device__ __forceinline__ void alternates_body(TopoDev t, const float* __restri
   unsigned long long top[ALT_LIST];
 #pragma unroll
   for (int j = 0; j < ALT_LIST; ++j) top[j] = 0;
-  const int groups = (n + 3) >> 2;
+  const int groups = (n - lo + 3) >> 2;
   for (int g = tid; g < groups; g += ALT_THREADS) {
-    const int n0 = g << 2;
-    const float4 s4 = __ldcs(reinterpret_cast<const float4*>(row + n0));  // read once: do not keep it in L2
+    const int n0 = lo + (g << 2);
+    const float4 s4 = __ldcs(reinterpret_cast<const float4*>(row + (n0 - lo)));  // read once: do not keep it in L2
     int4 d4 = make_int4(J.dom, J.dom, J.dom, J.dom);
     if (need_dom) d4 = __ldg(reinterpret_cast<const int4*>(dom_l + n0));  // padded past n: safe
     int4 c4 = make_int4(J.cdom, J.cdom, J.cdom, J.cdom);
@@ -110,7 +123,7 @@ __device__ __forceinline__ void alternates_body(TopoDev t, const float* __restri
       if (m >= n || s[j] == -INFINITY || d[j] != J.dom || (COLOC && cd[j] != J.cdom)) continue;
       const unsigned long long k = make_key(s[j], m);
       if (k <= top[ALT_LIST - 1]) continue;
-      if ((sFull[m >> 5] >> (m & 31)) & 1u) continue;
+      if ((sFull[(m - lo) >> 5] >> ((m - lo) & 31)) & 1u) continue;
       if constexpr (COMMIT)
         if (need_dom) {  // d[j] = dom_{L_g}(m): the owner every group of the batch left on m
           CommitDev cm = cm0;
@@ -149,6 +162,16 @@ __device__ __forceinline__ void alternates_body(TopoDev t, const float* __restri
   }
   __syncthreads();
 
+  if constexpr (SLAB) {  // the slab's list of the job, and the scores this slab holds
+    unsigned long long* const keys = reinterpret_cast<unsigned long long*>(out);
+    if (tid < ALT_LIST) keys[(size_t)blockIdx.x * ALT_LIST + tid] = sTop[tid];
+    float* const rscore = reinterpret_cast<float*>(out + 2 * ALT_LIST * (size_t)gridDim.x);
+    for (int i = tid; i < J.nrep; i += ALT_THREADS) {
+      const int a = own[J.rep0 + i];
+      rscore[J.rep0 + i] = a >= lo && a < n ? row[a - lo] : -INFINITY;
+    }
+    return;
+  }
   // ---- per replica: the merged list without its own node
   if (tid < J.nrep) {
     const int rep = J.rep0 + tid;
@@ -206,6 +229,83 @@ k_alternates_commit_coloc_lv(TopoDev t, const float* __restrict__ rows, const Al
                              const int2* __restrict__ used, const int* __restrict__ own, int n_alt,
                              int* __restrict__ out, CommitDev cm, const int* __restrict__ gids) {
   alternates_body<true, true, true>(t, rows, jobs, used, own, n_alt, out, cm, gids);
+}
+
+// A job's slab list for the exchange of §3.17 (one-pod replicas: no co-location condition).  out: see SLAB above.
+template <bool COMMIT, bool LV>
+__global__ void __launch_bounds__(ALT_THREADS)
+k_alternates_slab(TopoDev t, const float* __restrict__ rows, const AltJob* __restrict__ jobs,
+                  const int2* __restrict__ used, const int* __restrict__ own, int* __restrict__ out, CommitDev cm,
+                  const int* __restrict__ gids) {
+  alternates_body<false, COMMIT, LV, true>(t, rows, jobs, used, own, 0, out, cm, gids);
+}
+
+// The merge half of §3.17: one warp per job.  keys_all: `world` exchange buffers of `stride` u64 each, rank-major; in
+// each, ALT_LIST keys per job, then one fp32 score per compact replica at word 2 * ALT_LIST * n_jobs.  Keys of
+// different slabs are distinct (their nodes are), 0 = no candidate.  xjob[j] = (first compact replica, replicas);
+// own[] the replicas' nodes; bounds[0 .. world] the slab bounds (empty slabs allowed).  out: per compact replica
+// 1 + 2 * n_alt words, as k_alternates writes them.
+constexpr int ALT_MERGE_WARPS = 4;
+__global__ void __launch_bounds__(32 * ALT_MERGE_WARPS)
+k_alternates_merge(const unsigned long long* __restrict__ keys_all, long long stride, int world, int n_jobs,
+                   const int2* __restrict__ xjob, const int* __restrict__ own, const int* __restrict__ bounds,
+                   int n_alt, int* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int j = blockIdx.x * ALT_MERGE_WARPS + (threadIdx.x >> 5);
+  if (j >= n_jobs) return;  // warp-uniform
+  unsigned long long top[ALT_LIST];
+#pragma unroll
+  for (int i = 0; i < ALT_LIST; ++i) top[i] = 0;
+  for (int i = lane; i < world * ALT_LIST; i += 32) {
+    const int w = i / ALT_LIST;
+    const unsigned long long k = __ldg(keys_all + (size_t)w * stride + (size_t)j * ALT_LIST + (i - w * ALT_LIST));
+    if (k > top[ALT_LIST - 1]) alt_insert(top, k);
+  }
+  unsigned long long best[ALT_LIST];  // the job's merged list, the same in every lane
+#pragma unroll
+  for (int r = 0; r < ALT_LIST; ++r) {
+    const unsigned long long m = warp_max_u64(top[0]);
+    if (m != 0 && top[0] == m) {
+#pragma unroll
+      for (int i = 0; i < ALT_LIST - 1; ++i) top[i] = top[i + 1];
+      top[ALT_LIST - 1] = 0;
+    }
+    best[r] = m;
+  }
+  const int2 J = __ldg(xjob + j);
+  for (int e = lane; e < J.y; e += 32) {
+    const int rep = J.x + e;
+    const int a = __ldg(own + rep);
+    int* o = out + (size_t)rep * (1 + 2 * n_alt);
+    float sc = -INFINITY;
+    if (a >= 0) {  // the rank whose slab holds a: the last w with bounds[w] <= a
+      int w0 = 0, w1 = world - 1;
+      while (w0 < w1) {
+        const int mid = (w0 + w1 + 1) >> 1;
+        if (__ldg(bounds + mid) <= a) w0 = mid;
+        else w1 = mid - 1;
+      }
+      sc = __ldg(reinterpret_cast<const float*>(keys_all + (size_t)w0 * stride + (size_t)n_jobs * ALT_LIST) + rep);
+    }
+    o[0] = __float_as_int(sc);
+    int k = 0;
+    if (a >= 0) {
+#pragma unroll
+      for (int i = 0; i < ALT_LIST; ++i) {
+        const unsigned long long key = best[i];
+        if (k >= n_alt || key == 0) break;
+        const int node = key_node(key);
+        if (node == a) continue;
+        o[1 + k] = node;
+        o[1 + n_alt + k] = __float_as_int(key_score(key));
+        ++k;
+      }
+    }
+    for (; k < n_alt; ++k) {
+      o[1 + k] = -1;
+      o[1 + n_alt + k] = __float_as_int(-INFINITY);
+    }
+  }
 }
 
 }  // namespace rbgtopo

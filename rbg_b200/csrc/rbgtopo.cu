@@ -176,9 +176,30 @@ struct BatchMeta {
   std::vector<int> rowmap;   // step batches: [total_r] dense role row of every replica (rbgtopo_read_scores)
 };
 
+// Ranked alternates on node-axis shards (rbgtopo_shard_place_groups*_ranked, DESIGN.md §3.17): what a handle carries
+// from the local call to the merge.  The jobs are those run_alternates made, in the order it made them (the same on
+// every rank: they follow from replicated placements); the merge reads nothing else, no snapshot state.
+struct AltExchange {
+  int n_alt = 0;
+  int64_t total_r = 0;                   // replicas of the call's assign vector
+  std::vector<int> bounds;               // [world + 1] slab bounds of every rank
+  std::vector<int2> job;                 // per job: first compact replica, replicas
+  std::vector<int> own, idx;             // per compact replica: node, index in assign
+  std::vector<unsigned long long> keys;  // per job ALT_LIST keys of this rank's slab (collected by run_alternates)
+  std::vector<float> rscore;             // per compact replica: S_r[own] where own lies in this slab, else -inf
+  int64_t bytes = 0;                     // the exchange buffer: keys, then rscore, padded to 8 bytes
+  DevBuf<unsigned long long> buf;
+  void reset(int n) {
+    n_alt = n;
+    total_r = bytes = 0;
+    bounds.clear(); job.clear(); own.clear(); idx.clear(); keys.clear(); rscore.clear();
+  }
+};
+
 struct Batch {
   bool in_use = false;    // reserved by a call or a stage handle
   bool staged = false;    // holds a staged blob (handle alive)
+  bool xchg = false;      // holds an exchange of rbgtopo_shard_place_groups*_ranked (handle alive until the merge)
   bool ran = false;
   bool early_emit = false;    // plan_stage already enqueued the dense-matrix kernel of the next pass (+ its two events)
   bool d2h_enqueued = false;  // enqueue_d2h ran for the last pass; fetch_batch only has to wait
@@ -243,6 +264,7 @@ struct Batch {
   // ranked host-driven wave loops (run_waves): the dense rows of every (wave, role), kept
   // across calls like the matrix
   DevBuf<float> kept;
+  AltExchange x;  // xchg: the exchange; the merge's tables and outputs are in alt / h_alt
   ~Batch() {
     if (stream) cudaStreamDestroy(stream);
     if (stream2) cudaStreamDestroy(stream2);
@@ -366,14 +388,17 @@ const int kHostParallelMinGroups = getenv("RBGTOPO_HOST_PARALLEL_MIN") ? std::ma
 // RBGTOPO_PROFILE_HOST: each costs stream time, and the host-buffer entry points are latency-bound.
 inline bool timing_events(const rbgtopo_ctx* c) { return kProfileHost || c->kernel_timing.load(std::memory_order_relaxed); }
 
+// First node of rank g's slab (g = W: n): g * n / W rounded down to 128, so a slab may be empty.
+int slab_bound(int n, int W, int g) {
+  if (g <= 0) return 0;
+  if (g >= W) return n;
+  long long b = (long long)g * n / W;
+  return (int)(b / 128 * 128);
+}
+
 void compute_slab(rbgtopo_ctx* c, int n) {
   const int W = c->cfg.world, r = c->cfg.rank;
-  auto bound = [&](int g) -> int {
-    if (g <= 0) return 0;
-    if (g >= W) return n;
-    long long b = (long long)g * n / W;
-    return (int)(b / 128 * 128);
-  };
+  auto bound = [&](int g) { return slab_bound(n, W, g); };
   c->slab_lo = bound(r);
   c->slab_hi = bound(r + 1);
   int max_len = 0;
@@ -757,6 +782,7 @@ void release_batch(rbgtopo_ctx* c, Batch* b) {
   b->d2h_enqueued = false;
   b->in_use = false;
   b->staged = false;
+  b->xchg = false;
   b->ran = false;
 }
 
@@ -1308,12 +1334,13 @@ int fetch_batch(rbgtopo_ctx* c, Batch* b, int32_t* assign, int32_t* status, int3
   return RBGTOPO_OK;
 }
 
-// any_epoch: rbgtopo_release only — a handle staged against an older topology can still be released.
+// any_epoch: rbgtopo_release only — a handle staged against an older topology can still be released, and so can an
+// exchange handle (§3.17).
 Batch* batch_of(rbgtopo_ctx* c, int handle, bool any_epoch = false) {
   std::lock_guard<std::mutex> g(c->pool_mu);
   if (handle < 0 || handle >= (int)c->batches.size()) return nullptr;
   Batch* b = c->batches[handle].get();
-  if (!(b->in_use && b->staged)) return nullptr;
+  if (!(b->in_use && (b->staged || (any_epoch && b->xchg)))) return nullptr;
   if (!any_epoch && b->epoch != c->topo_epoch) return nullptr;  // sizes / offsets belong to the old topology
   if (!any_epoch && b->m.any_level && b->lvl_epoch != c->lvl_epoch) return nullptr;  // levels of old partitions
   return b;
@@ -1427,6 +1454,8 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
   for (auto* f : {k_alternates<false>, k_alternates<true>})
     CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   for (auto* f : {k_alternates_commit<false>, k_alternates_commit<true>})
+    CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
+  for (auto* f : {k_alternates_slab<false, false>, k_alternates_slab<true, false>, k_alternates_slab<true, true>})
     CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_lw_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_plan_group<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
@@ -2062,6 +2091,7 @@ struct RankReq {  // the ranked outputs of one call, indexed like assign
   float* score;
   int32_t* alt_node;
   float* alt_score;
+  AltExchange* x = nullptr;  // the sharded form (§3.17): the jobs' slab lists go here; the merge writes the outputs
 };
 struct AltRow {  // one role row of one wave: where its dense row is, and its replicas [rep0, rep0 + nrep) in assign order
   int row, group, role, rep0, nrep;
@@ -2260,12 +2290,27 @@ namespace {
 // Replicas (pods) [first, first + count) start with no score and no alternates (what an unplaced or gang-failed one
 // keeps).
 void alt_clear(const RankReq& rk, int64_t first, int64_t count) {
+  if (rk.x) return;  // the merge clears every replica
   for (int64_t k = 0; k < count; ++k) {
     const int64_t r = first + k;
     rk.score[r] = -INFINITY;
     for (int i = 0; i < rk.n_alt; ++i) {
       rk.alt_node[r * rk.n_alt + i] = -1;
       rk.alt_score[r * rk.n_alt + i] = -INFINITY;
+    }
+  }
+}
+
+// The per-replica lists o (1 + 2 * n_alt words per compact replica, as k_alternates writes them) into rk at idx.
+void alt_scatter(const RankReq& rk, const int* o, const int* idx, size_t n) {
+  const int F = rk.n_alt;
+  for (size_t e = 0; e < n; ++e) {
+    const int* v = o + e * (1 + 2 * F);
+    const int64_t r = idx[e];
+    memcpy(&rk.score[r], v, 4);
+    if (F > 0) {
+      memcpy(rk.alt_node + r * F, v + 1, (size_t)F * 4);
+      memcpy(rk.alt_score + r * F, v + 1 + F, (size_t)F * 4);
     }
   }
 }
@@ -2386,6 +2431,9 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
     }
   }
   if (jobs.empty()) return RBGTOPO_OK;
+  if (rk.x && (coloc || hc)) return fail(RBGTOPO_ECUDA, "internal: a co-located job on node-axis shards");
+  if (rk.x && rk.x->bounds.empty())
+    for (int g = 0; g <= c->cfg.world; ++g) rk.x->bounds.push_back(slab_bound(T.n, c->cfg.world, g));
   const size_t smem = (size_t)((c->topo.n + 31) / 32) * 4;
   if (smem > kFastSmemMax) return fail(RBGTOPO_ELIMIT, "ranked placement: %d nodes exceed the room bitmap", c->topo.n);
   static_assert(sizeof(AltJob) % 4 == 0, "jobs are staged as words");
@@ -2393,10 +2441,13 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
   // hc: dhead, then dclaim 8-byte aligned, after the gids
   const size_t o_dhead = w_jobs + w_used + w_own + gids.size();
   const size_t o_dclaim = hc ? (o_dhead + hc->dhead.size() + 1) & ~(size_t)1 : o_dhead;
-  const size_t w_in = hc ? o_dclaim + 2 * hc->dclaim.size() : o_dhead, w_out = own.size() * (size_t)(1 + 2 * F);
+  const size_t w_in = hc ? o_dclaim + 2 * hc->dclaim.size() : o_dhead;
+  // rk.x: the slab lists (8-byte aligned) and the replicas' slab scores instead of the replicas' lists
+  const size_t o_out = rk.x ? (w_in + 1) & ~(size_t)1 : w_in;
+  const size_t w_out = rk.x ? jobs.size() * 2 * ALT_LIST + own.size() : own.size() * (size_t)(1 + 2 * F);
   cudaStream_t s = stream_of(c, b);
-  CK(b->alt.reserve(w_in + w_out));
-  CK(b->h_alt.reserve(w_in + w_out));
+  CK(b->alt.reserve(o_out + w_out));
+  CK(b->h_alt.reserve(o_out + w_out));
   int* h = b->h_alt.p;
   memcpy(h, jobs.data(), w_jobs * 4);
   memcpy(h + w_jobs, used.data(), w_used * 4);
@@ -2413,7 +2464,12 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
     cmd.dhead = d + o_dhead;
     cmd.dclaim = reinterpret_cast<const int2*>(d + o_dclaim);
   }
-  if (cm && coloc)
+  if (rk.x)
+    (cm ? (cm_levels ? k_alternates_slab<true, true> : k_alternates_slab<true, false>) : k_alternates_slab<false, false>)
+        <<<(unsigned)jobs.size(), ALT_THREADS, (size_t)((c->slab_hi - c->slab_lo + 31) / 32) * 4, s>>>(
+        topo_dev(c), rows, reinterpret_cast<const AltJob*>(d), reinterpret_cast<const int2*>(d + w_jobs),
+        d + w_jobs + w_used, d + o_out, cmd, d + w_jobs + w_used + w_own);
+  else if (cm && coloc)
     (cm_levels ? k_alternates_commit_coloc_lv : k_alternates_commit_coloc)<<<(unsigned)jobs.size(), ALT_THREADS, smem, s>>>(
         topo_dev(c), rows, reinterpret_cast<const AltJob*>(d), reinterpret_cast<const int2*>(d + w_jobs),
         d + w_jobs + w_used, F, d + w_in, cmd, d + w_jobs + w_used + w_own);
@@ -2426,18 +2482,22 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
         topo_dev(c), rows, reinterpret_cast<const AltJob*>(d), reinterpret_cast<const int2*>(d + w_jobs),
         d + w_jobs + w_used, F, d + w_in);
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(h + w_in, d + w_in, w_out * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(h + o_out, d + o_out, w_out * 4, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  const int* o = h + w_in;
-  for (size_t e = 0; e < own.size(); ++e) {
-    const int* v = o + e * (1 + 2 * F);
-    const int64_t r = idx[e];
-    memcpy(&rk.score[r], v, 4);
-    if (F > 0) {
-      memcpy(rk.alt_node + r * F, v + 1, (size_t)F * 4);
-      memcpy(rk.alt_score + r * F, v + 1 + F, (size_t)F * 4);
-    }
+  const int* o = h + o_out;
+  if (rk.x) {  // append the jobs, at the next global job index
+    AltExchange& x = *rk.x;
+    const int rep0 = (int)x.own.size();
+    for (const AltJob& j : jobs) x.job.push_back(make_int2(rep0 + j.rep0, j.nrep));
+    x.own.insert(x.own.end(), own.begin(), own.end());
+    x.idx.insert(x.idx.end(), idx.begin(), idx.end());
+    const auto* k = reinterpret_cast<const unsigned long long*>(o);
+    x.keys.insert(x.keys.end(), k, k + jobs.size() * ALT_LIST);
+    const auto* rs = reinterpret_cast<const float*>(o + jobs.size() * 2 * ALT_LIST);
+    x.rscore.insert(x.rscore.end(), rs, rs + own.size());
+    return RBGTOPO_OK;
   }
+  alt_scatter(rk, o, idx.data(), idx.size());
   return RBGTOPO_OK;
 }
 
@@ -4598,18 +4658,21 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
 // The entry checks of every rbgtopo_place_groups* function, in this order: rounds = 0, null arguments, n_alt, world
 // == 1, lock / topology / device, own status and domain for a ranked form given NULL; then the placement of `form`.
 // rbgtopo_place_groups and its ranked form take the lock inside place_groups_impl, which releases it before the
-// host-driven re-run.
-enum PlaceForm { kPlaceReplicas = 0, kPlaceCommitted = 1, kPlaceLw = 2, kPlaceRanked = 4 };
+// host-driven re-run.  kPlaceShard (with kPlaceRanked, x != nullptr): the local half of §3.17, valid at any world; the
+// slab lists go to x and the outputs score / alt_node / alt_score are the merge's.
+enum PlaceForm { kPlaceReplicas = 0, kPlaceCommitted = 1, kPlaceLw = 2, kPlaceRanked = 4, kPlaceShard = 8 };
 int32_t place_entry(int form, rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
                     int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds, float* score,
-                    int32_t* alt_node, float* alt_score) {
+                    int32_t* alt_node, float* alt_score, AltExchange* x = nullptr) {
   const bool committed = form & kPlaceCommitted, lw = form & kPlaceLw, ranked = form & kPlaceRanked;
+  const bool shard = form & kPlaceShard;
   if (rounds) *rounds = 0;
-  if (!c || !gb || !assign || (lw && !rp) || (ranked && (!score || (n_alt > 0 && (!alt_node || !alt_score)))))
+  if (!c || !gb || !assign || (lw && !rp) ||
+      (ranked && !shard && (!score || (n_alt > 0 && (!alt_node || !alt_score)))))
     return fail(RBGTOPO_EINVAL, "null argument");
   if (ranked && (n_alt < 0 || n_alt > RBGTOPO_MAX_ALTERNATES))
     return fail(RBGTOPO_EINVAL, "n_alt %d outside [0, %d]", n_alt, RBGTOPO_MAX_ALTERNATES);
-  if ((ranked || lw) && c->cfg.world > 1)
+  if ((ranked || lw) && !shard && c->cfg.world > 1)
     return fail(RBGTOPO_ELIMIT, "%s needs world == 1: a rank holds only its slab of every dense row",
                 !lw ? "ranked placement" : committed ? "committed leader-worker placement" : "leader-worker placement");
   std::shared_lock<std::shared_mutex> lk(c->topo_mu, std::defer_lock);  // one snapshot for the rounds and the ranking
@@ -4624,7 +4687,7 @@ int32_t place_entry(int form, rbgtopo_ctx* c, const int32_t* gb, int64_t words, 
     if (!status) { own_status.resize((size_t)ng + 1); status = own_status.data(); }
     if (!domain) { own_domain.resize((size_t)ng + 1); domain = own_domain.data(); }
   }
-  const RankReq rk{n_alt, score, alt_node, alt_score};
+  const RankReq rk{n_alt, score, alt_node, alt_score, shard ? x : nullptr};
   const RankReq* rkp = ranked ? &rk : nullptr;
   if (!lw && !committed) return place_groups_impl(c, gb, words, assign, status, domain, rkp);
   int32_t r = 0;
@@ -4686,6 +4749,126 @@ int32_t rbgtopo_place_groups_lw_committed_ranked(rbgtopo_ctx* c, const int32_t* 
                                                  float* score, int32_t* alt_node, float* alt_score) {
   return place_entry(kPlaceLw | kPlaceCommitted | kPlaceRanked, c, gb, words, role_pods, role_pods_words, n_alt, assign,
                      status, domain, rounds, score, alt_node, alt_score);
+}
+
+// ---- ranked alternates on node-axis shards (DESIGN.md §3.17) ---------------------------------------------------------
+namespace {
+// The local half: a handle of its own from the pool, the placement of `form` with the slab lists collected in its
+// AltExchange, then the exchange buffer and the merge's tables uploaded.  Nothing is left behind when the placement
+// fails; once it has placed, only the device can fail.
+int32_t shard_ranked_local(int form, rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t n_alt, int32_t* assign,
+                           int32_t* status, int32_t* domain, int32_t* rounds, int32_t* xhandle, void** keys_dev,
+                           int64_t* keys_bytes) {
+  if (rounds) *rounds = 0;
+  if (!c || !xhandle || !keys_dev || !keys_bytes) return fail(RBGTOPO_EINVAL, "null argument");
+  Batch* xb = nullptr;
+  int rc = acquire_batch(c, &xb);
+  if (rc) return rc;
+  AltExchange& x = xb->x;
+  x.reset(n_alt);
+  rc = place_entry(form | kPlaceRanked | kPlaceShard, c, gb, words, nullptr, 0, n_alt, assign, status, domain, rounds,
+                   nullptr, nullptr, nullptr, &x);
+  if (rc) {
+    release_batch(c, xb);
+    return rc;
+  }
+  rc = [&]() -> int {
+    CK(cudaSetDevice(c->cfg.device));
+    x.total_r = gb[4];
+    const size_t J = x.job.size(), R = x.own.size(), W = x.bounds.size();
+    x.bytes = (int64_t)std::max<size_t>(8, (J * ALT_LIST * 8 + R * 4 + 7) & ~(size_t)7);
+    // pinned: the exchange buffer | the merge's tables (job, own, bounds), then the merge's outputs; device: the
+    // tables | the outputs.  Everything the merge needs is allocated here.
+    const size_t xw = (size_t)x.bytes / 4, tw = 2 * J + R + W, ow = R * (size_t)(1 + 2 * n_alt);
+    CK(x.buf.reserve((size_t)x.bytes / 8));
+    CK(xb->h_alt.reserve(std::max(xw + tw, ow)));
+    CK(xb->alt.reserve(tw + ow + 1));
+    int* h = xb->h_alt.p;
+    memset(h, 0, (size_t)x.bytes);
+    memcpy(h, x.keys.data(), J * ALT_LIST * 8);
+    memcpy(h + 2 * J * ALT_LIST, x.rscore.data(), R * 4);
+    memcpy(h + xw, x.job.data(), J * 8);
+    memcpy(h + xw + 2 * J, x.own.data(), R * 4);
+    memcpy(h + xw + 2 * J + R, x.bounds.data(), W * 4);
+    cudaStream_t s = stream_of(c, xb);
+    CK(cudaMemcpyAsync(x.buf.p, h, (size_t)x.bytes, cudaMemcpyHostToDevice, s));
+    if (tw) CK(cudaMemcpyAsync(xb->alt.p, h + xw, tw * 4, cudaMemcpyHostToDevice, s));
+    CK(cudaStreamSynchronize(s));
+    return RBGTOPO_OK;
+  }();
+  if (rc) {
+    cudaStreamSynchronize(stream_of(c, xb));
+    release_batch(c, xb);
+    return rc;
+  }
+  {
+    std::lock_guard<std::mutex> g(c->pool_mu);
+    xb->xchg = true;
+  }
+  *xhandle = handle_of(c, xb);
+  *keys_dev = x.buf.p;
+  *keys_bytes = x.bytes;
+  return RBGTOPO_OK;
+}
+}  // namespace
+
+int32_t rbgtopo_shard_place_groups_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t n_alt,
+                                          int32_t* assign, int32_t* status, int32_t* domain, int32_t* xhandle,
+                                          void** keys_dev, int64_t* keys_bytes) {
+  return shard_ranked_local(kPlaceReplicas, c, gb, words, n_alt, assign, status, domain, nullptr, xhandle, keys_dev,
+                            keys_bytes);
+}
+
+int32_t rbgtopo_shard_place_groups_committed_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t n_alt,
+                                                    int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds,
+                                                    int32_t* xhandle, void** keys_dev, int64_t* keys_bytes) {
+  return shard_ranked_local(kPlaceCommitted, c, gb, words, n_alt, assign, status, domain, rounds, xhandle, keys_dev,
+                            keys_bytes);
+}
+
+int32_t rbgtopo_shard_alternates_merge(rbgtopo_ctx* c, int32_t xhandle, const void* keys_all_dev, float* score,
+                                       int32_t* alt_node, float* alt_score) {
+  if (!c) return fail(RBGTOPO_EINVAL, "null ctx");
+  std::shared_lock<std::shared_mutex> lk(c->topo_mu);
+  Batch* xb = nullptr;
+  {
+    std::lock_guard<std::mutex> g(c->pool_mu);
+    if (xhandle >= 0 && xhandle < (int)c->batches.size() && c->batches[xhandle]->in_use && c->batches[xhandle]->xchg)
+      xb = c->batches[xhandle].get();
+  }
+  if (!xb) return fail(RBGTOPO_EINVAL, "handle %d is not an exchange of a sharded ranked placement", xhandle);
+  const AltExchange& x = xb->x;
+  const int F = x.n_alt;
+  if (!keys_all_dev || !score || (F > 0 && (!alt_node || !alt_score))) return fail(RBGTOPO_EINVAL, "null argument");
+  const RankReq rk{F, score, alt_node, alt_score};
+  alt_clear(rk, 0, x.total_r);
+  int rc = [&]() -> int {
+    const size_t J = x.job.size(), R = x.own.size();
+    if (J == 0) return RBGTOPO_OK;
+    CK(cudaSetDevice(c->cfg.device));
+    cudaStream_t s = stream_of(c, xb);
+    const int W = (int)x.bounds.size() - 1;
+    int* d = xb->alt.p;
+    const size_t o_out = 2 * J + R + x.bounds.size();
+    const unsigned grid = (unsigned)((J + ALT_MERGE_WARPS - 1) / ALT_MERGE_WARPS);
+    k_alternates_merge<<<grid, 32 * ALT_MERGE_WARPS, 0, s>>>(
+        static_cast<const unsigned long long*>(keys_all_dev), x.bytes / 8, W, (int)J, reinterpret_cast<const int2*>(d),
+        d + 2 * J, d + 2 * J + R, F, d + o_out);
+    CK(cudaGetLastError());
+    int* h = xb->h_alt.p;  // the staged exchange buffer is no longer needed (the local call reserved ow here)
+    const size_t ow = R * (size_t)(1 + 2 * F);
+    CK(cudaMemcpyAsync(h, d + o_out, ow * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    alt_scatter(rk, h, x.idx.data(), R);
+    {
+      std::lock_guard<std::mutex> g(c->stat_mu);
+      c->launches += 1;
+    }
+    return RBGTOPO_OK;
+  }();
+  if (rc) cudaStreamSynchronize(stream_of(c, xb));
+  release_batch(c, xb);
+  return rc;
 }
 
 int32_t rbgtopo_plan_describe(const int32_t* gb, int64_t words, int32_t n_nodes, int32_t n_domains,

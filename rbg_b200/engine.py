@@ -44,6 +44,14 @@ def _i32(a) -> np.ndarray:
     return np.ascontiguousarray(a, dtype=np.int32)
 
 
+class _DevBytes:
+    """A device buffer the library owns, as a uint8 array for torch.as_tensor."""
+
+    def __init__(self, ptr: int, nbytes: int):
+        self.__cuda_array_interface__ = {"shape": (nbytes,), "typestr": "|u1", "data": (ptr, False), "version": 3,
+                                         "strides": None}
+
+
 class TopoPlacer:
     """Device-resident cluster snapshot + placement entry points."""
 
@@ -71,6 +79,8 @@ class TopoPlacer:
         self.places_lw_committed = True  # place_groups_lw_committed: committed leader-worker batches (§3.13)
         self.places_committed_ranked = True  # place_groups_committed_ranked: alternates of committed batches (§3.14)
         self.places_lw_committed_ranked = True  # place_groups_lw_committed_ranked: alternates of committed LW batches (§3.15)
+        # place_groups[_committed]_ranked_sharded: ranked alternates on node-axis shards, any world (§3.17)
+        self.places_sharded_ranked = True
         h = C.c_void_p()
         self._h = None
         # blob totals of every live staged handle (fetch sizes its outputs from them); created here, not on the first
@@ -408,6 +418,91 @@ class TopoPlacer:
     def shard_assign(self, handle: int, keys2_all_ptr: Optional[int]) -> None:
         self._check(self.lib.rbgtopo_shard_assign(self._h, handle,
                                                   C.c_void_p(keys2_all_ptr) if keys2_all_ptr else None))
+
+    # -- ranked alternates on node-axis shards (DESIGN.md §3.17)
+    def shard_place_groups_ranked(self, groups_blob: np.ndarray, n_alt: int):
+        """Local half of place_groups_ranked on this rank: (assign, status, domain, xhandle, keys_ptr, keys_bytes).
+        keys_ptr / keys_bytes: this rank's exchange buffer (library-owned device memory) for the all-gather."""
+        gb = _i32(groups_blob)
+        ng, tp = int(gb[2]), int(gb[4])
+        assign = np.empty(max(tp, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        xh, p, nb = C.c_int32(), C.c_void_p(), C.c_int64()
+        self._check(self.lib.rbgtopo_shard_place_groups_ranked(
+            self._h, _p(gb), len(gb), int(n_alt), _p(assign), _p(status), _p(domain), C.byref(xh), C.byref(p),
+            C.byref(nb)))
+        return assign[:tp], status[:ng], domain[:ng], xh.value, p.value, nb.value
+
+    def shard_place_groups_committed_ranked(self, groups_blob: np.ndarray, n_alt: int):
+        """Local half of place_groups_committed_ranked: (assign, status, domain, rounds, xhandle, keys_ptr,
+        keys_bytes)."""
+        gb = _i32(groups_blob)
+        ng, tp = int(gb[2]), int(gb[4])
+        assign = np.empty(max(tp, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        rounds, xh, p, nb = C.c_int32(), C.c_int32(), C.c_void_p(), C.c_int64()
+        self._check(self.lib.rbgtopo_shard_place_groups_committed_ranked(
+            self._h, _p(gb), len(gb), int(n_alt), _p(assign), _p(status), _p(domain), C.byref(rounds), C.byref(xh),
+            C.byref(p), C.byref(nb)))
+        return assign[:tp], status[:ng], domain[:ng], rounds.value, xh.value, p.value, nb.value
+
+    def shard_alternates_merge(self, xhandle: int, keys_all_ptr: int, n_replicas: int, n_alt: int):
+        """Merge half: (score[R], alt_node[R, n_alt], alt_score[R, n_alt]) from the gathered buffers (world x
+        keys_bytes, rank-major, device memory).  Consumes the handle."""
+        R = int(n_replicas)
+        score = np.empty(max(R, 1), dtype=np.float32)
+        alt_node = np.empty((max(R, 1), max(n_alt, 0)), dtype=np.int32)
+        alt_score = np.empty((max(R, 1), max(n_alt, 0)), dtype=np.float32)
+        self._check(self.lib.rbgtopo_shard_alternates_merge(
+            self._h, int(xhandle), C.c_void_p(keys_all_ptr), _p(score, _lib.f32p), _p(alt_node) if n_alt > 0 else None,
+            _p(alt_score, _lib.f32p) if n_alt > 0 else None))
+        return score[:R], alt_node[:R], alt_score[:R]
+
+    def _default_all_gather(self, ptr: int, nbytes: int):
+        """torch.distributed.all_gather_into_tensor of this rank's exchange buffer over the default process group."""
+        import torch
+        import torch.distributed as dist
+        if not (dist.is_available() and dist.is_initialized()):
+            raise RuntimeError("a sharded ranked placement at world > 1 needs all_gather= or an initialised "
+                               "torch.distributed process group")
+        dev = torch.device("cuda", torch.cuda.current_device())
+        mine = torch.as_tensor(_DevBytes(ptr, nbytes), device=dev)
+        out = torch.empty(self.world * nbytes, dtype=torch.uint8, device=dev)
+        dist.all_gather_into_tensor(out, mine)
+        return out
+
+    def _sharded(self, local, n_alt: int, all_gather):
+        """Local half, all-gather, merge.  all_gather(ptr, nbytes) returns a device buffer of world x nbytes bytes,
+        rank-major (a torch tensor, or anything with data_ptr()), complete when its stream is done: the calling
+        thread's current torch stream is synchronised before the merge.  The handle is released when it fails."""
+        *placed, xh, ptr, nbytes = local
+        if self.world == 1 and all_gather is None:
+            gathered = None
+        else:
+            try:
+                gathered = (all_gather or self._default_all_gather)(ptr, nbytes)
+                import torch
+                torch.cuda.current_stream().synchronize()
+            except BaseException:
+                self.release(xh)
+                raise
+        keys_all = ptr if gathered is None else int(gathered.data_ptr())
+        merged = self.shard_alternates_merge(xh, keys_all, len(placed[0]), n_alt)
+        return (*placed, *merged)
+
+    def place_groups_ranked_sharded(self, groups_blob: np.ndarray, n_alt: int, all_gather=None):
+        """place_groups_ranked on node-axis shards (DESIGN.md §3.17), valid for any world: every rank calls it with
+        the same blob and gets all six outputs of the world = 1 place_groups_ranked, bit for bit.  all_gather(ptr,
+        nbytes) -> a device buffer of world x nbytes, rank-major; default: torch.distributed.all_gather_into_tensor
+        on the initialised default process group (world = 1 needs none)."""
+        return self._sharded(self.shard_place_groups_ranked(groups_blob, n_alt), n_alt, all_gather)
+
+    def place_groups_committed_ranked_sharded(self, groups_blob: np.ndarray, n_alt: int, all_gather=None):
+        """place_groups_committed_ranked on node-axis shards (§3.17): (assign, status, domain, rounds, score,
+        alt_node, alt_score) as the world = 1 call gives them; all_gather as for place_groups_ranked_sharded."""
+        return self._sharded(self.shard_place_groups_committed_ranked(groups_blob, n_alt), n_alt, all_gather)
 
     # -- all-gather over NVLink peer memory inside the library
     def p2p_export(self, rows_cap: int = 0):

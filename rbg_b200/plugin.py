@@ -296,7 +296,8 @@ class B200TopoPodGroupManager:
     """Third ``PodGroupManager`` implementation (plugin type "b200-topo")."""
 
     def __init__(self, placer: TopoPlacer, inner: Optional[str] = "scheduler-plugins",
-                 exclusive_keys: Optional[Sequence[str]] = None, alternates: int = 0, leader_worker: bool = False):
+                 exclusive_keys: Optional[Sequence[str]] = None, alternates: int = 0, leader_worker: bool = False,
+                 all_gather=None):
         """inner: the gang plugin this manager wraps for the PodGroup CR and the pod-group label —
         "scheduler-plugins" (kube), "volcano" or None (the Go manager takes the implementation object).
         exclusive_keys: the topology keys exclusive groups may name (DESIGN.md §3.9), keys[0] = the level-0 label.
@@ -316,6 +317,12 @@ class B200TopoPodGroupManager:
         (below) gets alternates from rbgtopo_place_groups_lw_committed_ranked (§3.15) when the placer has
         `places_lw_committed_ranked`, for its one-pod and its multi-pod groups alike; a placer without it gives that
         batch's hints without alternates.
+        On a placer with world > 1 (node-axis shards) that has `places_sharded_ranked`, the snapshot call and the
+        committed one-pod call with alternates are their sharded forms, place_groups_ranked_sharded and
+        place_groups_committed_ranked_sharded (§3.17): every rank's manager must reconcile the same groups, and gets
+        the hints and alternates of a world = 1 placer.  all_gather(ptr, nbytes) is their collective (None: the
+        placer's default, torch.distributed over the initialised process group).  Leader-worker groups on such a
+        placer are routed as before.
         leader_worker: a group with a role of lws_size > 1 is placed through rbgtopo_place_groups_lw (DESIGN.md
         §3.11): every replica of such a role is lws_size pods, placed all or nothing, and the hints are keyed by pod
         name, "{rbg}-{role}-{ordinal}-{k}" (k = 0 the leader); standalone roles keep "{rbg}-{role}-{ordinal}".  A
@@ -339,6 +346,7 @@ class B200TopoPodGroupManager:
         self.inner = inner
         self.exclusive_keys = None if exclusive_keys is None else tuple(exclusive_keys)
         self.leader_worker = bool(leader_worker)
+        self.all_gather = all_gather
         self.no_hint: Dict[Tuple[str, str], str] = {}
         self._hints: Dict[Tuple[str, str], Placement] = {}
 
@@ -469,11 +477,18 @@ class B200TopoPodGroupManager:
         if plain:
             blob, runs = self.groups_blob([rbgs[i] for i in plain])
             alt_node = None
-            if committed and self.alternates > 0 and getattr(self.placer, "places_committed_ranked", False):
+            sharded = getattr(self.placer, "world", 1) > 1 and getattr(self.placer, "places_sharded_ranked", False)
+            if committed and self.alternates > 0 and sharded:
+                assign, status, domain, _, _, alt_node, _ = self.placer.place_groups_committed_ranked_sharded(
+                    blob, self.alternates, self.all_gather)
+            elif committed and self.alternates > 0 and getattr(self.placer, "places_committed_ranked", False):
                 assign, status, domain, _, _, alt_node, _ = self.placer.place_groups_committed_ranked(
                     blob, self.alternates)
             elif committed:
                 assign, status, domain, _ = self.placer.place_groups_committed(blob)
+            elif self.alternates > 0 and sharded:
+                assign, status, domain, _, alt_node, _ = self.placer.place_groups_ranked_sharded(
+                    blob, self.alternates, self.all_gather)
             elif self.alternates > 0:
                 assign, status, domain, _, alt_node, _ = self.placer.place_groups_ranked(blob, self.alternates)
             else:
