@@ -181,10 +181,13 @@ type placer struct {
 
 // Config flags of the ctx (include/rbgtopo.h).  CfgLWCommitLevels lets a committed batch with leader-worker groups hold
 // groups at exclusive levels >= 1 (DESIGN.md §3.16); it needs the two flags before it, so its ctx takes all three.
+// CfgLWShards lets leader-worker placement run on a ctx with world > 1 (§3.18); this bridge creates world = 1 ctxs,
+// where it changes nothing.
 const (
 	CfgLevelPlacement = int32(C.RBGTOPO_CFG_LEVEL_PLACEMENT)
 	CfgCommitLevels   = int32(C.RBGTOPO_CFG_COMMIT_LEVELS)
 	CfgLWCommitLevels = int32(C.RBGTOPO_CFG_LW_COMMIT_LEVELS)
+	CfgLWShards       = int32(C.RBGTOPO_CFG_LW_SHARDS)
 )
 
 func newPlacer(device int) (*placer, error) { return newPlacerFlags(device, 0) }

@@ -146,6 +146,11 @@ typedef struct rbgtopo_config {
                                           groups at levels >= 1 (claims across levels, in
                                           pods); valid only with both flags above (flags = 7),
                                           else EINVAL */
+#define RBGTOPO_CFG_LW_SHARDS 8        /* rbgtopo_place_groups_lw and _lw_committed also place at
+                                          world > 1: every rank evaluates the rows it needs
+                                          from the snapshot over all nodes and returns the
+                                          world = 1 results (DESIGN.md §3.18); combines with
+                                          the flags above (e.g. 15) */
 
 /* Per-call device timing, milliseconds from CUDA events on the call's stream. */
 typedef struct rbgtopo_timing {
@@ -408,7 +413,14 @@ int32_t rbgtopo_place_groups_committed_ranked(rbgtopo_ctx* ctx, const int32_t* g
  * merged (the collective failed, say).  A second merge of the same handle, a staged-batch handle or a NULL argument
  * is RBGTOPO_EINVAL (the handle stays valid after NULL arguments).  Several exchanges may be in flight on one ctx.
  * Neither half fails once it has placed, except on a device error (RBGTOPO_ECUDA) and the merge's EINVAL.
- * Leader-worker forms are not sharded: rbgtopo_place_groups_lw* keep RBGTOPO_ELIMIT at world > 1. */
+ * Leader-worker forms (§3.18): rbgtopo_shard_place_groups_lw_ranked and
+ * rbgtopo_shard_place_groups_lw_committed_ranked take the inputs of rbgtopo_place_groups_lw_ranked /
+ * _lw_committed_ranked (role_pods included) with their validation, exactness check, levels and config rules and error
+ * codes, and are valid at any world without RBGTOPO_CFG_LW_SHARDS.  Their assign / status / domain / *rounds are
+ * those of rbgtopo_place_groups_lw / _lw_committed, and every ranked row is a POD row: keys_bytes = 72 per job (a
+ * (wave, role) row, or its pods in one co-location domain) plus 4 per pod, padded to 8.  The merge is
+ * rbgtopo_shard_alternates_merge, whose outputs (indexed per pod, in assign order) equal the world = 1 ranked forms'
+ * bit for bit.  The non-shard ranked leader-worker forms keep RBGTOPO_ELIMIT at world > 1. */
 int32_t rbgtopo_shard_place_groups_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
                                           int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain,
                                           int32_t* xhandle, void** keys_dev, int64_t* keys_bytes);
@@ -416,6 +428,15 @@ int32_t rbgtopo_shard_place_groups_committed_ranked(rbgtopo_ctx* ctx, const int3
                                                     int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain,
                                                     int32_t* rounds, int32_t* xhandle, void** keys_dev,
                                                     int64_t* keys_bytes);
+int32_t rbgtopo_shard_place_groups_lw_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                             const int32_t* role_pods, int64_t role_pods_words, int32_t n_alt,
+                                             int32_t* assign, int32_t* status, int32_t* domain, int32_t* xhandle,
+                                             void** keys_dev, int64_t* keys_bytes);
+int32_t rbgtopo_shard_place_groups_lw_committed_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                                       const int32_t* role_pods, int64_t role_pods_words,
+                                                       int32_t n_alt, int32_t* assign, int32_t* status,
+                                                       int32_t* domain, int32_t* rounds, int32_t* xhandle,
+                                                       void** keys_dev, int64_t* keys_bytes);
 int32_t rbgtopo_shard_alternates_merge(rbgtopo_ctx* ctx, int32_t xhandle, const void* keys_all_dev, float* score,
                                        int32_t* alt_node, float* alt_score);
 
@@ -444,7 +465,9 @@ int32_t rbgtopo_shard_alternates_merge(rbgtopo_ctx* ctx, int32_t xhandle, const 
  * group that includes waves after unplaced pods (each raises need and drops an anchor), so such a group can be
  * refused with RBGTOPO_EINEXACT a little below the bound rbgtopo_place_groups applies; no wave fails midway.
  * Documented limits: a ctx with world > 1 holds only its slab of every dense row, so the call returns
- * RBGTOPO_ELIMIT there; more nodes than a shared-memory room bitmap of 200 KB holds (1 638 400): RBGTOPO_ELIMIT. */
+ * RBGTOPO_ELIMIT there unless the ctx was created with RBGTOPO_CFG_LW_SHARDS (§3.18: every rank then evaluates the
+ * rows from the snapshot and returns the world = 1 results, no dense matrix written); more nodes than a shared-memory
+ * room bitmap of 200 KB holds (1 638 400, whatever the world): RBGTOPO_ELIMIT. */
 int32_t rbgtopo_place_groups_lw(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
                                 const int32_t* role_pods, int64_t role_pods_words, int32_t* assign,
                                 int32_t* status, int32_t* domain);
@@ -477,8 +500,8 @@ int32_t rbgtopo_place_groups_lw_ranked(rbgtopo_ctx* ctx, const int32_t* groups, 
  * Over the batch no node receives more than free[n].  With S = 1 and C = -1 everywhere the results are
  * bit-identical to rbgtopo_place_groups_committed's.  *rounds (may be NULL) = wave-loop rounds run: at most
  * n_groups, 1 for one group.  Limits (RBGTOPO_ELIMIT): a group whose own exclusive level is >= 1 on a ctx without
- * RBGTOPO_CFG_LW_COMMIT_LEVELS, a ctx with world > 1, more nodes than the room bitmap of rbgtopo_place_groups_lw
- * holds.  On a ctx created with RBGTOPO_CFG_LW_COMMIT_LEVELS (flags = 7, DESIGN.md §3.16) a group exclusive at level
+ * RBGTOPO_CFG_LW_COMMIT_LEVELS, a ctx with world > 1 unless it was created with RBGTOPO_CFG_LW_SHARDS (§3.18; with
+ * flags = 15 committed levels too), more nodes than the room bitmap of rbgtopo_place_groups_lw holds.  On a ctx created with RBGTOPO_CFG_LW_COMMIT_LEVELS (flags = 7, DESIGN.md §3.16) a group exclusive at level
  * L_g >= 1 is placed too: a participating role may not use node n when owner_{L_g}[n] (+) K (+) P is neither -1 nor
  * gid_g, where K merges, for every level L of the batch's exclusive groups, the gid of the last earlier exclusive
  * group at L (status != 2) that reports dom_L(n), and P the gid of every pod an earlier exclusive group keyed at

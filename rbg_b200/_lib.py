@@ -24,6 +24,7 @@ class Config(C.Structure):
 CFG_LEVEL_PLACEMENT = 1  # RBGTOPO_CFG_LEVEL_PLACEMENT: place groups / steps at exclusive levels >= 1
 CFG_COMMIT_LEVELS = 2    # RBGTOPO_CFG_COMMIT_LEVELS: committed batches at levels >= 1 too (with the flag above)
 CFG_LW_COMMIT_LEVELS = 4  # RBGTOPO_CFG_LW_COMMIT_LEVELS: committed leader-worker batches at levels >= 1 (with both above)
+CFG_LW_SHARDS = 8  # RBGTOPO_CFG_LW_SHARDS: place_groups_lw[_committed] at world > 1, the world = 1 results on every rank
 
 
 class Timing(C.Structure):
@@ -63,6 +64,12 @@ SIGNATURES = {
     "rbgtopo_shard_place_groups_committed_ranked": (C.c_int32, [C.c_void_p, i32p, C.c_int64, C.c_int32, i32p, i32p,
                                                                 i32p, i32p, i32p, C.POINTER(C.c_void_p),
                                                                 C.POINTER(C.c_int64)]),
+    "rbgtopo_shard_place_groups_lw_ranked": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, C.c_int64, C.c_int32, i32p,
+                                                         i32p, i32p, i32p, C.POINTER(C.c_void_p),
+                                                         C.POINTER(C.c_int64)]),
+    "rbgtopo_shard_place_groups_lw_committed_ranked": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, C.c_int64,
+                                                                   C.c_int32, i32p, i32p, i32p, i32p, i32p,
+                                                                   C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]),
     "rbgtopo_shard_alternates_merge": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, f32p, i32p, f32p]),
     "rbgtopo_stage_groups": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p]),
     "rbgtopo_stage": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p]),

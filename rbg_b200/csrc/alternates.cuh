@@ -24,7 +24,7 @@
 // its row and writes the job's ALT_LIST best keys of the slab, plus S_r[assign[r]] of every replica whose node lies in
 // the slab; after the caller's all-gather, k_alternates_merge merges the world lists of every job into the replicas'
 // lists.  The global top ALT_LIST of a job lies in the union of the per-slab top ALT_LIST lists, so the result is the
-// world = 1 ranking bit for bit.
+// world = 1 ranking bit for bit.  k_alternates_slab_coloc does the same for the pod rows of leader-worker forms (§3.18).
 #pragma once
 #include "kernels.cuh"
 #include "plan_group.cuh"
@@ -238,6 +238,15 @@ k_alternates_slab(TopoDev t, const float* __restrict__ rows, const AltJob* __res
                   const int2* __restrict__ used, const int* __restrict__ own, int* __restrict__ out, CommitDev cm,
                   const int* __restrict__ gids) {
   alternates_body<false, COMMIT, LV, true>(t, rows, jobs, used, own, 0, out, cm, gids);
+}
+
+// The same for the pod rows of leader-worker forms (§3.18), whose jobs may carry a co-location domain (cdom, clevel).
+template <bool COMMIT, bool LV>
+__global__ void __launch_bounds__(ALT_THREADS)
+k_alternates_slab_coloc(TopoDev t, const float* __restrict__ rows, const AltJob* __restrict__ jobs,
+                        const int2* __restrict__ used, const int* __restrict__ own, int* __restrict__ out, CommitDev cm,
+                        const int* __restrict__ gids) {
+  alternates_body<true, COMMIT, LV, true>(t, rows, jobs, used, own, 0, out, cm, gids);
 }
 
 // The merge half of §3.17: one warp per job.  keys_all: `world` exchange buffers of `stride` u64 each, rank-major; in

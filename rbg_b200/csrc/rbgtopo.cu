@@ -343,6 +343,8 @@ inline int installed_levels(const rbgtopo_ctx* c) { return c->topo.occ ? c->topo
 inline bool places_levels(const rbgtopo_ctx* c) { return (c->cfg.flags & RBGTOPO_CFG_LEVEL_PLACEMENT) != 0; }
 // committed batches at levels >= 1 (create accepts the flag only together with RBGTOPO_CFG_LEVEL_PLACEMENT)
 inline bool commits_levels(const rbgtopo_ctx* c) { return (c->cfg.flags & RBGTOPO_CFG_COMMIT_LEVELS) != 0; }
+// rbgtopo_place_groups_lw[_committed] at world > 1 (DESIGN.md §3.18)
+inline bool lw_shards(const rbgtopo_ctx* c) { return (c->cfg.flags & RBGTOPO_CFG_LW_SHARDS) != 0; }
 // Domain count of installed level L (level_code accepted it): the range of a fixed domain at that level.
 inline int level_domains(const Topology& T, int L) { return L == 0 ? T.n_domains : T.lvl_nd[L]; }
 constexpr size_t kFastSmemMax = 200 * 1024;
@@ -1409,7 +1411,8 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
   *out = nullptr;
   if (cfg->world < 1 || cfg->rank < 0 || cfg->rank >= cfg->world)
     return fail(RBGTOPO_EINVAL, "rank %d / world %d", cfg->rank, cfg->world);
-  if (cfg->flags & ~(RBGTOPO_CFG_LEVEL_PLACEMENT | RBGTOPO_CFG_COMMIT_LEVELS | RBGTOPO_CFG_LW_COMMIT_LEVELS))
+  if (cfg->flags & ~(RBGTOPO_CFG_LEVEL_PLACEMENT | RBGTOPO_CFG_COMMIT_LEVELS | RBGTOPO_CFG_LW_COMMIT_LEVELS |
+                     RBGTOPO_CFG_LW_SHARDS))
     return fail(RBGTOPO_EINVAL, "unknown config flags 0x%x", cfg->flags);
   if ((cfg->flags & RBGTOPO_CFG_COMMIT_LEVELS) && !(cfg->flags & RBGTOPO_CFG_LEVEL_PLACEMENT))
     return fail(RBGTOPO_EINVAL, "RBGTOPO_CFG_COMMIT_LEVELS needs RBGTOPO_CFG_LEVEL_PLACEMENT (flags 0x%x)", cfg->flags);
@@ -1453,11 +1456,16 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
   }
   for (auto* f : {k_alternates<false>, k_alternates<true>})
     CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
-  for (auto* f : {k_alternates_commit<false>, k_alternates_commit<true>})
+  for (auto* f : {k_alternates_commit<false>, k_alternates_commit<true>, k_alternates_commit_coloc,
+                  k_alternates_commit_coloc_lv})
     CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
-  for (auto* f : {k_alternates_slab<false, false>, k_alternates_slab<true, false>, k_alternates_slab<true, true>})
+  for (auto* f : {k_alternates_slab<false, false>, k_alternates_slab<true, false>, k_alternates_slab<true, true>,
+                  k_alternates_slab_coloc<false, false>, k_alternates_slab_coloc<true, false>,
+                  k_alternates_slab_coloc<true, true>})
     CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_lw_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
+  for (auto* f : {k_lw_assign_repl<LW_REPL>, k_lw_assign_repl<LW_REPL_CLAIMS>, k_lw_assign_repl<LW_REPL_CLAIMS_LV>})
+    CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
   CK(cudaFuncSetAttribute(k_plan_group<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
 #ifdef RBGTOPO_PHASE_CLOCKS
   {
@@ -2431,7 +2439,6 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
     }
   }
   if (jobs.empty()) return RBGTOPO_OK;
-  if (rk.x && (coloc || hc)) return fail(RBGTOPO_ECUDA, "internal: a co-located job on node-axis shards");
   if (rk.x && rk.x->bounds.empty())
     for (int g = 0; g <= c->cfg.world; ++g) rk.x->bounds.push_back(slab_bound(T.n, c->cfg.world, g));
   const size_t smem = (size_t)((c->topo.n + 31) / 32) * 4;
@@ -2465,7 +2472,10 @@ int run_alternates(rbgtopo_ctx* c, Batch* b, const float* rows, const std::vecto
     cmd.dclaim = reinterpret_cast<const int2*>(d + o_dclaim);
   }
   if (rk.x)
-    (cm ? (cm_levels ? k_alternates_slab<true, true> : k_alternates_slab<true, false>) : k_alternates_slab<false, false>)
+    (coloc ? (cm ? (cm_levels ? k_alternates_slab_coloc<true, true> : k_alternates_slab_coloc<true, false>)
+                 : k_alternates_slab_coloc<false, false>)
+           : cm ? (cm_levels ? k_alternates_slab<true, true> : k_alternates_slab<true, false>)
+                : k_alternates_slab<false, false>)
         <<<(unsigned)jobs.size(), ALT_THREADS, (size_t)((c->slab_hi - c->slab_lo + 31) / 32) * 4, s>>>(
         topo_dev(c), rows, reinterpret_cast<const AltJob*>(d), reinterpret_cast<const int2*>(d + w_jobs),
         d + w_jobs + w_used, d + o_out, cmd, d + w_jobs + w_used + w_own);
@@ -4585,6 +4595,9 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
     for (int64_t k = off.pod0[g]; k < off.pod0[g + 1]; ++k) assign[k] = -1;
   };
   const bool keep = rk && !rounds;
+  // world > 1 (RBGTOPO_CFG_LW_SHARDS or a sharded ranked form, §3.18): k_lw_assign_repl evaluates the rows from the
+  // snapshot; the slab rows are emitted only where a ranking reads them (kept per wave; a committed ranking replays them)
+  const bool repl = c->cfg.world > 1, emit = !repl || keep;
   KeptRows kept;
   for (int g = 0; g < ng; ++g) {
     init_run(g);
@@ -4614,8 +4627,11 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
     }
     if (cr) cr->add_side(runs, active, side);
     // grid: every step resident at once if the device holds them, the level-C scratch bounded by kLwScratchBytes
+    const auto repl_k = !cr ? k_lw_assign_repl<LW_REPL>
+                        : cr->at_lv ? k_lw_assign_repl<LW_REPL_CLAIMS_LV> : k_lw_assign_repl<LW_REPL_CLAIMS>;
     int per_sm = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_lw_assign, LW_THREADS, smem));
+    if (repl) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, repl_k, LW_THREADS, smem));
+    else CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_lw_assign, LW_THREADS, smem));
     long long grid = std::min<long long>(ns, (long long)std::max(1, per_sm) * c->sm_count);
     if (dmax > 0) grid = std::min<long long>(grid, std::max<long long>(1, kLwScratchBytes / (12LL * dmax)));
     CK(b->lw.reserve(side.size()));
@@ -4626,14 +4642,28 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
     CK(cudaMemcpyAsync(b->lw.p, b->h_lw.p, side.size() * 4, cudaMemcpyHostToDevice, s));
     CK(cudaStreamWaitEvent(s, c->base_ready, 0));  // a pending snapshot refresh
     CK(cudaStreamWaitEvent(s, c->topo_ready, 0));
-    if (const int r2 = cr ? cr->score(c, b, s, b->lw.p) : launch_score(c, b, s)) return r2;
-    k_lw_assign<<<(unsigned)grid, LW_THREADS, smem, s>>>(topo_dev(c), batch_dev(c, b), b->lw.p, b->lw_best.p,
-                                                         b->lw_cap.p, dmax, lv);
+    if (emit)
+      if (const int r2 = cr ? cr->score(c, b, s, b->lw.p) : launch_score(c, b, s)) return r2;
+    if (!repl) {
+      k_lw_assign<<<(unsigned)grid, LW_THREADS, smem, s>>>(topo_dev(c), batch_dev(c, b), b->lw.p, b->lw_best.p,
+                                                           b->lw_cap.p, dmax, lv);
+    } else {  // the patch tables: one record of 2 + max_p words per patched node of a step
+      const int w = 2 + b->m.max_p;
+      CK(b->corr.reserve((size_t)b->m.patch_cap * w + 1));
+      BatchDev d = batch_dev(c, b);
+      d.corr = b->corr.p;
+      d.corr_w = w;
+      const int* co = cr ? b->lw.p + cr->sec_at : nullptr;
+      const int2* cl = cr && !cr->at_lv ? reinterpret_cast<const int2*>(b->lw.p + cr->rec_at) : nullptr;
+      repl_k<<<(unsigned)grid, LW_THREADS, smem, s>>>(topo_dev(c), d, b->lw.p, b->lw_best.p, b->lw_cap.p, dmax, lv, co,
+                                                      cl, T.occ, cr ? cr->cm : CommitDev{});
+    }
     CK(cudaGetLastError());
-    b->pend_launches += 2;
+    const int launched = emit ? 2 : 1;
+    b->pend_launches += launched;
     b->ran = true;
     std::lock_guard<std::mutex> g(c->stat_mu);
-    c->launches += 2;
+    c->launches += launched;
     return RBGTOPO_OK;
   };
   rbgtopo_timing total{};
@@ -4656,7 +4686,8 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
 }
 
 // The entry checks of every rbgtopo_place_groups* function, in this order: rounds = 0, null arguments, n_alt, world
-// == 1, lock / topology / device, own status and domain for a ranked form given NULL; then the placement of `form`.
+// == 1 (a leader-worker form without ranking also at world > 1 on a ctx with RBGTOPO_CFG_LW_SHARDS, §3.18), lock /
+// topology / device, own status and domain for a ranked form given NULL; then the placement of `form`.
 // rbgtopo_place_groups and its ranked form take the lock inside place_groups_impl, which releases it before the
 // host-driven re-run.  kPlaceShard (with kPlaceRanked, x != nullptr): the local half of §3.17, valid at any world; the
 // slab lists go to x and the outputs score / alt_node / alt_score are the merge's.
@@ -4672,7 +4703,7 @@ int32_t place_entry(int form, rbgtopo_ctx* c, const int32_t* gb, int64_t words, 
     return fail(RBGTOPO_EINVAL, "null argument");
   if (ranked && (n_alt < 0 || n_alt > RBGTOPO_MAX_ALTERNATES))
     return fail(RBGTOPO_EINVAL, "n_alt %d outside [0, %d]", n_alt, RBGTOPO_MAX_ALTERNATES);
-  if ((ranked || lw) && !shard && c->cfg.world > 1)
+  if ((ranked || lw) && !shard && c->cfg.world > 1 && !(lw && !ranked && lw_shards(c)))
     return fail(RBGTOPO_ELIMIT, "%s needs world == 1: a rank holds only its slab of every dense row",
                 !lw ? "ranked placement" : committed ? "committed leader-worker placement" : "leader-worker placement");
   std::shared_lock<std::shared_mutex> lk(c->topo_mu, std::defer_lock);  // one snapshot for the rounds and the ranking
@@ -4756,9 +4787,10 @@ namespace {
 // The local half: a handle of its own from the pool, the placement of `form` with the slab lists collected in its
 // AltExchange, then the exchange buffer and the merge's tables uploaded.  Nothing is left behind when the placement
 // fails; once it has placed, only the device can fail.
-int32_t shard_ranked_local(int form, rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t n_alt, int32_t* assign,
-                           int32_t* status, int32_t* domain, int32_t* rounds, int32_t* xhandle, void** keys_dev,
-                           int64_t* keys_bytes) {
+// rp: the (S, C) table of a leader-worker form (§3.18), whose jobs and compact replicas count pods.
+int32_t shard_ranked_local(int form, rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp,
+                           int64_t rp_words, int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain,
+                           int32_t* rounds, int32_t* xhandle, void** keys_dev, int64_t* keys_bytes) {
   if (rounds) *rounds = 0;
   if (!c || !xhandle || !keys_dev || !keys_bytes) return fail(RBGTOPO_EINVAL, "null argument");
   Batch* xb = nullptr;
@@ -4766,15 +4798,15 @@ int32_t shard_ranked_local(int form, rbgtopo_ctx* c, const int32_t* gb, int64_t 
   if (rc) return rc;
   AltExchange& x = xb->x;
   x.reset(n_alt);
-  rc = place_entry(form | kPlaceRanked | kPlaceShard, c, gb, words, nullptr, 0, n_alt, assign, status, domain, rounds,
-                   nullptr, nullptr, nullptr, &x);
+  rc = place_entry(form | kPlaceRanked | kPlaceShard, c, gb, words, rp, rp_words, n_alt, assign, status, domain,
+                   rounds, nullptr, nullptr, nullptr, &x);
   if (rc) {
     release_batch(c, xb);
     return rc;
   }
   rc = [&]() -> int {
     CK(cudaSetDevice(c->cfg.device));
-    x.total_r = gb[4];
+    x.total_r = rp ? GroupOffsets(gb, rp).pod0[gb[2]] : gb[4];
     const size_t J = x.job.size(), R = x.own.size(), W = x.bounds.size();
     x.bytes = (int64_t)std::max<size_t>(8, (J * ALT_LIST * 8 + R * 4 + 7) & ~(size_t)7);
     // pinned: the exchange buffer | the merge's tables (job, own, bounds), then the merge's outputs; device: the
@@ -4815,15 +4847,31 @@ int32_t shard_ranked_local(int form, rbgtopo_ctx* c, const int32_t* gb, int64_t 
 int32_t rbgtopo_shard_place_groups_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t n_alt,
                                           int32_t* assign, int32_t* status, int32_t* domain, int32_t* xhandle,
                                           void** keys_dev, int64_t* keys_bytes) {
-  return shard_ranked_local(kPlaceReplicas, c, gb, words, n_alt, assign, status, domain, nullptr, xhandle, keys_dev,
-                            keys_bytes);
+  return shard_ranked_local(kPlaceReplicas, c, gb, words, nullptr, 0, n_alt, assign, status, domain, nullptr, xhandle,
+                            keys_dev, keys_bytes);
 }
 
 int32_t rbgtopo_shard_place_groups_committed_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words, int32_t n_alt,
                                                     int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds,
                                                     int32_t* xhandle, void** keys_dev, int64_t* keys_bytes) {
-  return shard_ranked_local(kPlaceCommitted, c, gb, words, n_alt, assign, status, domain, rounds, xhandle, keys_dev,
-                            keys_bytes);
+  return shard_ranked_local(kPlaceCommitted, c, gb, words, nullptr, 0, n_alt, assign, status, domain, rounds, xhandle,
+                            keys_dev, keys_bytes);
+}
+
+int32_t rbgtopo_shard_place_groups_lw_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* role_pods,
+                                             int64_t role_pods_words, int32_t n_alt, int32_t* assign, int32_t* status,
+                                             int32_t* domain, int32_t* xhandle, void** keys_dev, int64_t* keys_bytes) {
+  return shard_ranked_local(kPlaceLw, c, gb, words, role_pods, role_pods_words, n_alt, assign, status, domain, nullptr,
+                            xhandle, keys_dev, keys_bytes);
+}
+
+int32_t rbgtopo_shard_place_groups_lw_committed_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words,
+                                                       const int32_t* role_pods, int64_t role_pods_words, int32_t n_alt,
+                                                       int32_t* assign, int32_t* status, int32_t* domain,
+                                                       int32_t* rounds, int32_t* xhandle, void** keys_dev,
+                                                       int64_t* keys_bytes) {
+  return shard_ranked_local(kPlaceLw | kPlaceCommitted, c, gb, words, role_pods, role_pods_words, n_alt, assign, status,
+                            domain, rounds, xhandle, keys_dev, keys_bytes);
 }
 
 int32_t rbgtopo_shard_alternates_merge(rbgtopo_ctx* c, int32_t xhandle, const void* keys_all_dev, float* score,

@@ -57,24 +57,28 @@ class TopoPlacer:
 
     def __init__(self, device: int = 0, rank: int = 0, world: int = 1, emit_matrix: bool = True,
                  chunk_nodes: int = 0, level_placement: bool = False, committed_levels: bool = False,
-                 lw_committed_levels: bool = False):
+                 lw_committed_levels: bool = False, lw_shards: bool = False):
         """level_placement: place exclusive groups at levels >= 1 of set_exclusive_levels (RBGTOPO_CFG_LEVEL_PLACEMENT,
         DESIGN.md §3.9); without it such a group raises RBGTOPO_ELIMIT.  `places_levels` tells callers which it is.
         committed_levels: place_groups_committed places them too, with claims across levels (RBGTOPO_CFG_COMMIT_LEVELS,
         §3.8; implies level_placement).  `places_committed_levels` tells callers which it is.
         lw_committed_levels: place_groups_lw_committed[_ranked] place them too, with claims across levels counted in
         pods (RBGTOPO_CFG_LW_COMMIT_LEVELS, §3.16; implies committed_levels).  `places_lw_committed_levels` tells
+        callers which it is.
+        lw_shards: place_groups_lw[_committed] also place at world > 1, every rank returning the world = 1 results
+        (RBGTOPO_CFG_LW_SHARDS, §3.18); without it they raise RBGTOPO_ELIMIT there.  `places_lw_sharded` tells
         callers which it is."""
         self.lib = _lib.load()
         committed_levels = committed_levels or lw_committed_levels
         level_placement = level_placement or committed_levels
         flags = ((_lib.CFG_LEVEL_PLACEMENT if level_placement else 0) | (_lib.CFG_COMMIT_LEVELS if committed_levels else 0)
-                 | (_lib.CFG_LW_COMMIT_LEVELS if lw_committed_levels else 0))
+                 | (_lib.CFG_LW_COMMIT_LEVELS if lw_committed_levels else 0) | (_lib.CFG_LW_SHARDS if lw_shards else 0))
         cfg = _lib.Config(device=device, rank=rank, world=world, slots=0,
                           emit_matrix=1 if emit_matrix else 0, chunk_nodes=chunk_nodes, flags=flags)
         self.places_levels = bool(level_placement)
         self.places_committed_levels = bool(committed_levels)
         self.places_lw_committed_levels = bool(lw_committed_levels)
+        self.places_lw_sharded = bool(lw_shards)
         self.places_lw_ranked = True   # place_groups_lw_ranked: alternates for leader-worker pods (DESIGN.md §3.12)
         self.places_lw_committed = True  # place_groups_lw_committed: committed leader-worker batches (§3.13)
         self.places_committed_ranked = True  # place_groups_committed_ranked: alternates of committed batches (§3.14)
@@ -448,6 +452,36 @@ class TopoPlacer:
             C.byref(p), C.byref(nb)))
         return assign[:tp], status[:ng], domain[:ng], rounds.value, xh.value, p.value, nb.value
 
+    def shard_place_groups_lw_ranked(self, groups_blob: np.ndarray, role_pods, n_alt: int):
+        """Local half of place_groups_lw_ranked (DESIGN.md §3.18): (assign per pod, status, domain, xhandle, keys_ptr,
+        keys_bytes)."""
+        gb = _i32(groups_blob)
+        rp = _i32(np.asarray(role_pods, dtype=np.int64).reshape(-1))
+        ng, pods = int(gb[2]), self._lw_pods(gb, rp)
+        assign = np.empty(max(pods, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        xh, p, nb = C.c_int32(), C.c_void_p(), C.c_int64()
+        self._check(self.lib.rbgtopo_shard_place_groups_lw_ranked(
+            self._h, _p(gb), len(gb), _p(rp), len(rp), int(n_alt), _p(assign), _p(status), _p(domain), C.byref(xh),
+            C.byref(p), C.byref(nb)))
+        return assign[:pods], status[:ng], domain[:ng], xh.value, p.value, nb.value
+
+    def shard_place_groups_lw_committed_ranked(self, groups_blob: np.ndarray, role_pods, n_alt: int):
+        """Local half of place_groups_lw_committed_ranked (§3.18): (assign per pod, status, domain, rounds, xhandle,
+        keys_ptr, keys_bytes)."""
+        gb = _i32(groups_blob)
+        rp = _i32(np.asarray(role_pods, dtype=np.int64).reshape(-1))
+        ng, pods = int(gb[2]), self._lw_pods(gb, rp)
+        assign = np.empty(max(pods, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        rounds, xh, p, nb = C.c_int32(), C.c_int32(), C.c_void_p(), C.c_int64()
+        self._check(self.lib.rbgtopo_shard_place_groups_lw_committed_ranked(
+            self._h, _p(gb), len(gb), _p(rp), len(rp), int(n_alt), _p(assign), _p(status), _p(domain),
+            C.byref(rounds), C.byref(xh), C.byref(p), C.byref(nb)))
+        return assign[:pods], status[:ng], domain[:ng], rounds.value, xh.value, p.value, nb.value
+
     def shard_alternates_merge(self, xhandle: int, keys_all_ptr: int, n_replicas: int, n_alt: int):
         """Merge half: (score[R], alt_node[R, n_alt], alt_score[R, n_alt]) from the gathered buffers (world x
         keys_bytes, rank-major, device memory).  Consumes the handle."""
@@ -503,6 +537,19 @@ class TopoPlacer:
         """place_groups_committed_ranked on node-axis shards (§3.17): (assign, status, domain, rounds, score,
         alt_node, alt_score) as the world = 1 call gives them; all_gather as for place_groups_ranked_sharded."""
         return self._sharded(self.shard_place_groups_committed_ranked(groups_blob, n_alt), n_alt, all_gather)
+
+    def place_groups_lw_ranked_sharded(self, groups_blob: np.ndarray, role_pods, n_alt: int, all_gather=None):
+        """place_groups_lw_ranked on node-axis shards (DESIGN.md §3.18), valid for any world: (assign, status, domain,
+        score, alt_node, alt_score) per pod as the world = 1 call gives them; all_gather as for
+        place_groups_ranked_sharded."""
+        return self._sharded(self.shard_place_groups_lw_ranked(groups_blob, role_pods, n_alt), n_alt, all_gather)
+
+    def place_groups_lw_committed_ranked_sharded(self, groups_blob: np.ndarray, role_pods, n_alt: int,
+                                                 all_gather=None):
+        """place_groups_lw_committed_ranked on node-axis shards (§3.18): (assign, status, domain, rounds, score,
+        alt_node, alt_score) per pod as the world = 1 call gives them; all_gather as for place_groups_ranked_sharded."""
+        return self._sharded(self.shard_place_groups_lw_committed_ranked(groups_blob, role_pods, n_alt), n_alt,
+                             all_gather)
 
     # -- all-gather over NVLink peer memory inside the library
     def p2p_export(self, rows_cap: int = 0):

@@ -321,8 +321,11 @@ class B200TopoPodGroupManager:
         committed one-pod call with alternates are their sharded forms, place_groups_ranked_sharded and
         place_groups_committed_ranked_sharded (§3.17): every rank's manager must reconcile the same groups, and gets
         the hints and alternates of a world = 1 placer.  all_gather(ptr, nbytes) is their collective (None: the
-        placer's default, torch.distributed over the initialised process group).  Leader-worker groups on such a
-        placer are routed as before.
+        placer's default, torch.distributed over the initialised process group).  Leader-worker groups and committed
+        leader-worker batches on a placer with world > 1 that has `places_lw_sharded` (a TopoPlacer created with
+        lw_shards=True, §3.18) go through place_groups_lw / place_groups_lw_committed, and with alternates through
+        place_groups_lw_ranked_sharded / place_groups_lw_committed_ranked_sharded over the same all_gather: the hints
+        and alternates of a world = 1 placer, keyed by pod name.  Without it they are routed as at world = 1.
         leader_worker: a group with a role of lws_size > 1 is placed through rbgtopo_place_groups_lw (DESIGN.md
         §3.11): every replica of such a role is lws_size pods, placed all or nothing, and the hints are keyed by pod
         name, "{rbg}-{role}-{ordinal}-{k}" (k = 0 the leader); standalone roles keep "{rbg}-{role}-{ordinal}".  A
@@ -397,6 +400,10 @@ class B200TopoPodGroupManager:
             skipped[i] = Placement(RBGTOPO_NO_HINT, {}, -1, 0)
         return keep, skipped
 
+    def _lw_sharded(self) -> bool:
+        """Leader-worker calls on node-axis shards (§3.18): a placer with world > 1 that places them there."""
+        return getattr(self.placer, "world", 1) > 1 and getattr(self.placer, "places_lw_sharded", False)
+
     def is_leader_worker(self, rbg: RoleBasedGroup) -> bool:
         """Placed through rbgtopo_place_groups_lw: the manager was asked to and a role runs multi-pod replicas."""
         return self.leader_worker and any(r.lws_size > 1 for r in rbg.roles)
@@ -465,7 +472,10 @@ class B200TopoPodGroupManager:
                     for g in runs]
             role_pods = [pods[k][ri] for k, g in enumerate(runs) for ri in g.order]
             alt_node = None
-            if self.alternates > 0 and getattr(self.placer, "places_lw_committed_ranked", False):
+            if self.alternates > 0 and self._lw_sharded():
+                assign, status, domain, _, _, alt_node, _ = self.placer.place_groups_lw_committed_ranked_sharded(
+                    blob, role_pods, self.alternates, self.all_gather)
+            elif self.alternates > 0 and getattr(self.placer, "places_lw_committed_ranked", False):
                 assign, status, domain, _, _, alt_node, _ = self.placer.place_groups_lw_committed_ranked(
                     blob, role_pods, self.alternates)
             else:
@@ -500,7 +510,10 @@ class B200TopoPodGroupManager:
             pods = [self.role_pods(g.rbg)[0] for g in runs]
             role_pods = [pods[k][ri] for k, g in enumerate(runs) for ri in g.order]
             alt_node = None
-            if self.alternates > 0:
+            if self.alternates > 0 and self._lw_sharded():
+                assign, status, domain, _, alt_node, _ = self.placer.place_groups_lw_ranked_sharded(
+                    blob, role_pods, self.alternates, self.all_gather)
+            elif self.alternates > 0:
                 assign, status, domain, _, alt_node, _ = self.placer.place_groups_lw_ranked(blob, role_pods,
                                                                                            self.alternates)
             else:
