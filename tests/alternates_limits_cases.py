@@ -135,12 +135,21 @@ def layout_holds(kind, nodes):
     return (warp_of(nodes) == 7).all()
 
 
-def merge_case(kind, own):
+def merge_case(kind, own, lo=0, n_total=None):
     """One group.  rank0: one replica (demand 1) on the best winner, which keeps room, so the nine winners are its
     node and eight alternates.  rank8: eight replicas of demand 2 fill eight better filler nodes first, then one of
     demand 1 (the designated job, row rank 8) takes the best winner and keeps room.  full: the replica's node
-    outranks everything but has room for it alone.  Six lower tail candidates sit elsewhere in the row."""
+    outranks everything but has room for it alone.  Six lower tail candidates sit elsewhere in the row.
+    lo / n_total: the same case shifted to nodes lo .. lo + N of a snapshot of n_total nodes (free 0 elsewhere)."""
     n, win = layout(kind)
+    if lo or n_total is not None:
+        topo, gb, info = merge_case(kind, own)
+        free = np.zeros(n_total, np.int32)
+        free[lo:lo + n] = topo.free
+        gb = gb.copy()
+        na, anchor_off = int(gb[8 + 6]), int(gb[8 + 7])       # the one group's anchors: (node, role, count)
+        gb[anchor_off:anchor_off + 3 * na:3] += lo
+        return bare_topo(free), gb, dict(win=[m + lo for m in info["win"]], fill=info["fill"] + lo, x=info["x"] + lo)
     rng = np.random.default_rng(MERGE_KINDS.index(kind) * 10 + OWN.index(own))
     rest = np.setdiff1d(np.arange(2, n - 1), win)
     pick = rng.choice(rest, 15, replace=False)
