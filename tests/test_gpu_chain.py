@@ -170,9 +170,15 @@ def profile_chain(eng, st, hs, passes):
     how many k_emit_rows of pass k + 1 started before k_plan_group of pass k ended.  Plain passes (the fallback) launch
     k_emit_rows in stream order behind the previous k_plan_group, so for them the count is 0; a chain overlaps as far
     as timing lets it."""
+    import time
+
     import torch
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        # The profiler keeps only activities that start after its capture window opens, comparing GPU timestamps
+        # converted to host time with the host clock.  A sleep launched the moment the window opens can land a few
+        # microseconds before it after that conversion and be dropped; a margin on the host keeps it inside.
+        time.sleep(0.01)
         sleep_on(st)
         eng.run_staged_chain(hs, passes)
         torch.cuda.synchronize()
