@@ -650,7 +650,10 @@ int32_t rbgtopo_slab(rbgtopo_ctx* ctx, int32_t* lo, int32_t* hi);
  * rbgtopo_run_staged_p2p then enqueues, per pass and wave: k_shard_select -> k_p2p_push (peer stores
  * of the lists into every rank's buffer + a release flag) -> k_p2p_wait (acquire, bounded spin) ->
  * k_merge [-> restricted reselect -> push -> wait] -> k_greedy.  Every rank must make the same calls
- * in the same order.  Results via rbgtopo_fetch; rbgtopo_p2p_stats reports the bytes this rank
+ * in the same order.  The passes of one ctx run one after another on the device: each call waits
+ * for the end of the ctx's previous rbgtopo_run_staged_p2p, whichever handle and stream that used
+ * and even if it returned RBGTOPO_ELIMIT after enqueuing some waves, so a rank may enqueue several
+ * handles without synchronising in between.  Results via rbgtopo_fetch; rbgtopo_p2p_stats reports the bytes this rank
  * stored into peer memory during the last pass and whether a wait timed out (a peer never arrived:
  * the results of that pass are invalid). */
 int32_t rbgtopo_p2p_export(rbgtopo_ctx* ctx, int32_t rows_cap, void* handle_out,

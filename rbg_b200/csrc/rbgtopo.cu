@@ -316,6 +316,9 @@ struct rbgtopo_ctx {
   unsigned long long p2p_seq = 0;
   long long p2p_bytes_last = 0;  // bytes this rank stored into PEER buffers during the last pass
   std::vector<void*> p2p_opened;
+  // recorded on its stream by every rbgtopo_run_staged_p2p; the next one waits for it.  Batches run on streams of their
+  // own, and two exchange passes in flight at once would share the parity slots, the flags and the CTA counter
+  cudaEvent_t p2p_done = nullptr;
   rbgtopo_timing last{};
   std::vector<float> last_score_ms, last_select_ms;  // per pass, harvested by the last fetch (rbgtopo_last_pass_times)
   long long calls = 0, scores_total = 0, launches = 0;
@@ -1442,6 +1445,7 @@ int32_t rbgtopo_create(const rbgtopo_config* cfg, rbgtopo_ctx** out) {
   CK(cudaEventCreate(&c->ev_base_a));
   CK(cudaEventCreate(&c->ev_base_b));
   CK(cudaEventCreateWithFlags(&c->fence_ev, cudaEventDisableTiming));
+  CK(cudaEventCreateWithFlags(&c->p2p_done, cudaEventDisableTiming));
   for (auto& e : c->stage_ev) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   for (auto* f : {k_select_assign_fast<false>, k_select_assign_fast<true>})
     CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFastSmemMax));
@@ -1490,6 +1494,7 @@ int32_t rbgtopo_destroy(rbgtopo_ctx* c) {
   if (c->ev_base_a) cudaEventDestroy(c->ev_base_a);
   if (c->ev_base_b) cudaEventDestroy(c->ev_base_b);
   if (c->fence_ev) cudaEventDestroy(c->fence_ev);
+  if (c->p2p_done) cudaEventDestroy(c->p2p_done);
   for (auto& e : c->stage_ev) if (e) cudaEventDestroy(e);
   delete c;
   return RBGTOPO_OK;
@@ -5408,6 +5413,14 @@ int32_t rbgtopo_run_staged_p2p(rbgtopo_ctx* c, int32_t handle, int32_t iters) {
   const int n_waves = plan ? (int)b->wave_begin.size() - 1 : 1;
   std::lock_guard<std::mutex> seq_guard(c->pool_mu);  // one exchange sequence at a time per ctx (the seq counter is SPMD state)
   CK(cudaStreamWaitEvent(s, c->topo_ready, 0));
+  // ... and one on the device: this pass starts after the ctx's previous pass ended, whichever stream that used.  Every
+  // return below records the end, an RBGTOPO_ELIMIT after some waves were enqueued included
+  CK(cudaStreamWaitEvent(s, c->p2p_done, 0));
+  struct RecordDone {
+    cudaEvent_t e;
+    cudaStream_t s;
+    ~RecordDone() { cudaEventRecord(e, s); }
+  } record_done{c->p2p_done, s};
   int launches = 0;
   for (int it = 0; it < iters; ++it) {
     c->p2p_bytes_last = 0;

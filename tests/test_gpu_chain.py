@@ -176,9 +176,10 @@ def profile_chain(eng, st, hs, passes):
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         # The profiler keeps only activities that start after its capture window opens, comparing GPU timestamps
-        # converted to host time with the host clock.  A sleep launched the moment the window opens can land a few
-        # microseconds before it after that conversion and be dropped; a margin on the host keeps it inside.
-        time.sleep(0.01)
+        # converted to host time with the host clock.  That conversion has been seen off by more than the 50 ms of the
+        # sleep (the sleep and the first passes were dropped behind a 10 ms margin), so the margin on the host is half
+        # a second.
+        time.sleep(0.5)
         sleep_on(st)
         eng.run_staged_chain(hs, passes)
         torch.cuda.synchronize()
