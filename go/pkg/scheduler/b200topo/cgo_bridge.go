@@ -126,6 +126,32 @@ static int32_t rbgtopo_go_place_groups_lw_ranked(rbgtopo_ctx* ctx, const int32_t
   rbgtopo_go_err(ctx, rc, err);
   return rc;
 }
+static int32_t rbgtopo_go_set_node_classes(rbgtopo_ctx* ctx, int32_t n_classes, const int32_t* node_class,
+                                           uint64_t gen, char* err) {
+  int32_t rc = rbgtopo_set_node_classes(ctx, n_classes, node_class, gen);
+  rbgtopo_go_err(ctx, rc, err);
+  return rc;
+}
+static int32_t rbgtopo_go_place_groups_eligible(rbgtopo_ctx* ctx, const int32_t* groups, int64_t words,
+                                                const int32_t* role_pods, int64_t role_pods_words,
+                                                const uint64_t* role_admit, int64_t n_role_admit, int32_t* assign,
+                                                int32_t* status, int32_t* domain, char* err) {
+  int32_t rc = rbgtopo_place_groups_eligible(ctx, groups, words, role_pods, role_pods_words, role_admit, n_role_admit,
+                                             assign, status, domain);
+  rbgtopo_go_err(ctx, rc, err);
+  return rc;
+}
+static int32_t rbgtopo_go_place_groups_eligible_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t words,
+                                                       const int32_t* role_pods, int64_t role_pods_words,
+                                                       const uint64_t* role_admit, int64_t n_role_admit, int32_t n_alt,
+                                                       int32_t* assign, int32_t* status, int32_t* domain, float* score,
+                                                       int32_t* alt_node, float* alt_score, char* err) {
+  int32_t rc = rbgtopo_place_groups_eligible_ranked(ctx, groups, words, role_pods, role_pods_words, role_admit,
+                                                    n_role_admit, n_alt, assign, status, domain, score, alt_node,
+                                                    alt_score);
+  rbgtopo_go_err(ctx, rc, err);
+  return rc;
+}
 */
 import "C"
 
@@ -399,4 +425,59 @@ func (p *placer) placeGroupsLWCommittedRanked(blob, rolePods []int32, nPods, nAl
 		return nil, nil, nil, nil, 0, err
 	}
 	return assign[:nPods], status[:nGroups], domain[:nGroups], altNode[:nPods*nAlt], int32(r), nil
+}
+
+// setNodeClasses installs node classes (DESIGN.md §3.19): nodeClass[n] in [0, nClasses) for every node, nClasses <= 64;
+// setTopology drops them.  Ordered like updateNodes.
+func (p *placer) setNodeClasses(nClasses int, nodeClass []int32, gen uint64) error {
+	var buf [C.RBGTOPO_GO_ERRLEN]C.char
+	rc := C.rbgtopo_go_set_node_classes(p.ctx, C.int32_t(nClasses), p32(nodeClass), C.uint64_t(gen), &buf[0])
+	return mkErr(rc, &buf)
+}
+
+// placeGroupsEligible: placeGroupsLW where role rho may use node n only when bit class[n] of roleAdmit[rho] is set
+// (DESIGN.md §3.19); roleAdmit holds one mask per role of every group in blob order.  rolePods nil: (1, -1) for every
+// role, nPods = the blob's pending replicas.
+func (p *placer) placeGroupsEligible(blob, rolePods []int32, roleAdmit []uint64, nPods int) (assign, status, domain []int32, err error) {
+	nGroups := int(blob[2])
+	assign = make([]int32, max(nPods, 1))
+	status = make([]int32, max(nGroups, 1))
+	domain = make([]int32, max(nGroups, 1))
+	var buf [C.RBGTOPO_GO_ERRLEN]C.char
+	rc := C.rbgtopo_go_place_groups_eligible(p.ctx, p32(blob), C.int64_t(len(blob)), p32(rolePods),
+		C.int64_t(len(rolePods)), pu64(roleAdmit), C.int64_t(len(roleAdmit)), p32(assign), p32(status), p32(domain),
+		&buf[0])
+	if err = mkErr(rc, &buf); err != nil {
+		return nil, nil, nil, err
+	}
+	return assign[:nPods], status[:nGroups], domain[:nGroups], nil
+}
+
+// placeGroupsEligibleRanked: placeGroupsEligible plus, per pod, up to nAlt next-best nodes as placeGroupsLWRanked
+// ranks them, read from the masked rows: no alternate lies on a node the pod's role does not admit.
+func (p *placer) placeGroupsEligibleRanked(blob, rolePods []int32, roleAdmit []uint64, nPods, nAlt int) (assign, status, domain, altNode []int32, err error) {
+	nGroups := int(blob[2])
+	assign = make([]int32, max(nPods, 1))
+	status = make([]int32, max(nGroups, 1))
+	domain = make([]int32, max(nGroups, 1))
+	score := make([]float32, max(nPods, 1))
+	altNode = make([]int32, max(nPods*nAlt, 1))
+	altScore := make([]float32, max(nPods*nAlt, 1))
+	var buf [C.RBGTOPO_GO_ERRLEN]C.char
+	rc := C.rbgtopo_go_place_groups_eligible_ranked(p.ctx, p32(blob), C.int64_t(len(blob)), p32(rolePods),
+		C.int64_t(len(rolePods)), pu64(roleAdmit), C.int64_t(len(roleAdmit)), C.int32_t(nAlt), p32(assign),
+		p32(status), p32(domain), (*C.float)(unsafe.Pointer(&score[0])), p32(altNode),
+		(*C.float)(unsafe.Pointer(&altScore[0])), &buf[0])
+	if err = mkErr(rc, &buf); err != nil {
+		return nil, nil, nil, nil, err
+	}
+	return assign[:nPods], status[:nGroups], domain[:nGroups], altNode[:nPods*nAlt], nil
+}
+
+// pu64: the first element of a uint64 slice for C, nil for an empty one.
+func pu64(s []uint64) *C.uint64_t {
+	if len(s) == 0 {
+		return nil
+	}
+	return (*C.uint64_t)(unsafe.Pointer(&s[0]))
 }

@@ -182,6 +182,22 @@ func (m *Manager) ReconcilePodGroup(ctx context.Context, rbg *workloadsv1alpha2.
 	if g.pending == 0 {
 		return nil
 	}
+	if snap.classes != nil { // node eligibility (DESIGN.md §3.19)
+		masks, restricted, reason := snap.classes.roleMasks(rbg)
+		var colocate []int32
+		if reason == "" && restricted && m.leaderWorker && g.leaderWorker() {
+			colocate, reason = m.colocateLevels(rbg)
+		}
+		if reason != "" {
+			m.hints.Delete(key)
+			m.alts.Delete(key)
+			logger.Info("no placement hint", "rbg", key, "reason", reason)
+			return nil
+		}
+		if restricted {
+			return m.placeEligible(logger, key, g, snap, masks, colocate)
+		}
+	}
 	if m.leaderWorker && g.leaderWorker() {
 		colocate, reason := m.colocateLevels(rbg)
 		if reason != "" {
@@ -305,4 +321,44 @@ func (t *gidTable) id(rbg *workloadsv1alpha2.RoleBasedGroup) int32 {
 	t.ids[k] = t.next
 	t.next++
 	return t.ids[k]
+}
+
+// placeEligible: a group with a role whose template excludes a node class, through
+// rbgtopo_place_groups_eligible[_ranked]; masks in rbg.Spec.Roles order, colocate != nil for a leader-worker group
+// (pod-keyed hints, its (S, C) table), nil for one pod per replica (role_pods NULL, RoleID hints).
+func (m *Manager) placeEligible(logger interface{ Info(string, ...any) }, key string, g *marshalled, snap *snapshot,
+	masks []uint64, colocate []int32) error {
+	admit := make([]uint64, len(g.order)) // the blob's role order
+	for k, ri := range g.order {
+		admit[k] = masks[ri]
+	}
+	var table []int32
+	pods := g.pending
+	if colocate != nil {
+		table, pods = g.rolePods(colocate)
+	}
+	if m.alternates > 0 {
+		assign, status, _, altNode, err := m.placer.placeGroupsEligibleRanked(g.blob, table, admit, pods, m.alternates)
+		if err != nil {
+			return m.degrade(logger, key, err)
+		}
+		if colocate != nil {
+			m.hints.Store(key, g.podIDMap(assign, snap, status[0]))
+			m.alts.Store(key, g.podIDAlternates(altNode, m.alternates, snap, status[0]))
+		} else {
+			m.hints.Store(key, g.roleIDMap(assign, snap, status[0]))
+			m.alts.Store(key, g.roleIDAlternates(altNode, m.alternates, snap, status[0]))
+		}
+		return nil
+	}
+	assign, status, _, err := m.placer.placeGroupsEligible(g.blob, table, admit, pods)
+	if err != nil {
+		return m.degrade(logger, key, err)
+	}
+	if colocate != nil {
+		m.hints.Store(key, g.podIDMap(assign, snap, status[0]))
+	} else {
+		m.hints.Store(key, g.roleIDMap(assign, snap, status[0]))
+	}
+	return nil
 }

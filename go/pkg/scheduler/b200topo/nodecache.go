@@ -51,6 +51,7 @@ type nodeInfo struct {
 	allocatable   int64
 	requested     int64 // summed over the node's non-terminated pods
 	unschedulable bool
+	taints        []corev1.Taint // spec.taints (node eligibility, eligibility.go)
 }
 
 // snapshot = the arrays of rbgtopo_set_topology, immutable once built.
@@ -60,6 +61,7 @@ type snapshot struct {
 	domains                                    []string
 	rowPtr, colIdx, edgeW, free, domain, owner []int32
 	topoGen, capGen                            uint64
+	classes                                    *nodeClasses // nil: node eligibility off (Manager.SetNodeClassKeys)
 }
 
 func (s *snapshot) nodeID(name string) (int32, bool) { id, ok := s.ids[name]; return id, ok }
@@ -72,6 +74,7 @@ type nodeCache struct {
 	pushedTopo, pushedCap uint64
 	snap                  *snapshot
 	dirty                 map[string]struct{} // nodes whose capacity changed since the last push
+	classKeys             []string            // node eligibility: the label keys of the node classes (nil: off)
 }
 
 func newNodeCache() *nodeCache {
@@ -120,13 +123,14 @@ func (nc *nodeCache) upsertNode(n *corev1.Node) {
 		}
 	}
 	old, ok := nc.nodes[n.Name]
-	ni := &nodeInfo{labels: n.Labels, allocatable: alloc.Value(), unschedulable: n.Spec.Unschedulable || !ready}
+	ni := &nodeInfo{labels: n.Labels, allocatable: alloc.Value(), unschedulable: n.Spec.Unschedulable || !ready,
+		taints: n.Spec.Taints}
 	if ok {
 		ni.requested = old.requested
 	}
 	nc.nodes[n.Name] = ni
 	switch {
-	case !ok || tierKeyChanged(old.labels, ni.labels):
+	case !ok || tierKeyChanged(old.labels, ni.labels) || nc.classChanged(old, ni):
 		nc.topoGen++ // node SET or a tier label changed: the CSR is rebuilt (rbgtopo_set_topology)
 	case old.allocatable != ni.allocatable || old.unschedulable != ni.unschedulable:
 		nc.capGen++ // capacity churn only (rbgtopo_update_nodes[_delta])
@@ -287,6 +291,16 @@ func (nc *nodeCache) sync(p *placer) (*snapshot, error) {
 		if err := p.setTopology(s); err != nil {
 			return nil, err
 		}
+		if nc.classKeys != nil { // set_topology dropped the classes: install those of the new node set
+			cls, err := buildNodeClasses(s.names, nc.nodes, nc.classKeys)
+			if err != nil {
+				return nil, err
+			}
+			if err := p.setNodeClasses(len(cls.labels), cls.class, nc.topoGen); err != nil {
+				return nil, err
+			}
+			s.classes = cls
+		}
 		nc.snap, nc.pushedTopo, nc.pushedCap = s, nc.topoGen, nc.capGen
 		nc.dirty = map[string]struct{}{}
 		return s, nil
@@ -317,4 +331,27 @@ func (nc *nodeCache) sync(p *placer) (*snapshot, error) {
 		nc.dirty = map[string]struct{}{}
 	}
 	return nc.snap, nil
+}
+
+// classChanged: a class key's label value or the node's hard taints changed (node eligibility on): the classes are
+// rebuilt with the topology.
+func (nc *nodeCache) classChanged(old, ni *nodeInfo) bool {
+	if nc.classKeys == nil {
+		return false
+	}
+	for _, k := range nc.classKeys {
+		if old.labels[k] != ni.labels[k] {
+			return true
+		}
+	}
+	a, b := hardTaints(old.taints), hardTaints(ni.taints)
+	if len(a) != len(b) {
+		return true
+	}
+	for i := range a {
+		if a[i] != b[i] {
+			return true
+		}
+	}
+	return false
 }

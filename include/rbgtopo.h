@@ -244,6 +244,16 @@ int32_t rbgtopo_set_exclusive_levels(rbgtopo_ctx* ctx, int32_t n_levels, const i
                                      const int32_t* level_n_domains, int32_t n_occ, const int32_t* occ,
                                      uint64_t generation);
 
+/* Node classes (DESIGN.md §3.19): node_class[n] in [0, n_classes) for every node of the topology, grouping nodes that
+ * every role's pod template admits alike (the same values of the label keys selectors read, the same NoSchedule /
+ * NoExecute taints).  Read only by rbgtopo_place_groups_eligible[_ranked]; no other entry point changes.  Ordered like
+ * rbgtopo_update_nodes: a call already in flight keeps the classes it started with, a call issued after the return
+ * sees the new ones.  rbgtopo_set_topology drops them.  Errors: RBGTOPO_ENOTOPO before rbgtopo_set_topology;
+ * n_classes > RBGTOPO_MAX_NODE_CLASSES: RBGTOPO_ELIMIT; n_classes < 1, node_class NULL or a class out of range:
+ * RBGTOPO_EINVAL (the classes installed before stay). */
+#define RBGTOPO_MAX_NODE_CLASSES 64
+int32_t rbgtopo_set_node_classes(rbgtopo_ctx* ctx, int32_t n_classes, const int32_t* node_class, uint64_t generation);
+
 /* ---- the hot path ------------------------------------------------------- */
 /* Score + select + greedy-assign one batch of steps (host buffers in, host
  * buffers out; H2D/D2H inside).  Plugs in between step 5 and step 7 of
@@ -489,6 +499,32 @@ int32_t rbgtopo_place_groups_lw_ranked(rbgtopo_ctx* ctx, const int32_t* groups, 
                                        const int32_t* role_pods, int64_t role_pods_words, int32_t n_alt,
                                        int32_t* assign, int32_t* status, int32_t* domain, float* score,
                                        int32_t* alt_node, float* alt_score);
+
+/* Node eligibility (DESIGN.md §3.19).  rbgtopo_place_groups_lw with one more feasibility term: role rho may not use
+ * node n when bit node_class[n] of its mask admit_rho is clear (bits at or above n_classes are ignored, so all ones
+ * means unrestricted).  Such an entry of the role's dense row is -inf, like a capacity or owner failure, so D*,
+ * co-location domains, all-or-nothing replicas, gang and alternates see admitted nodes only.  Scores, anchors (a
+ * scheduled pod on a node its role no longer admits still anchors its neighbours) and consumed capacity are unchanged.
+ *   role_admit[n_role_admit]: one mask per role of every group, in blob order (like role_pods).
+ *   role_pods == NULL: (S, C) = (1, -1) for every role; assign is then in rbgtopo_place_groups order.
+ * Validation, exactness bound, levels, limits and error codes are rbgtopo_place_groups_lw's, plus RBGTOPO_EINVAL for
+ * role_admit NULL, n_role_admit != the roles of the blob, or no classes installed (rbgtopo_set_node_classes), and
+ * RBGTOPO_ELIMIT at world > 1 (checked before anything is placed).  With every mask admitting every installed class
+ * the outputs are bit-identical to rbgtopo_place_groups_lw (role_pods given) or rbgtopo_place_groups (NULL). */
+int32_t rbgtopo_place_groups_eligible(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                      const int32_t* role_pods, int64_t role_pods_words, const uint64_t* role_admit,
+                                      int64_t n_role_admit, int32_t* assign, int32_t* status, int32_t* domain);
+
+/* Ranked alternates with node eligibility (DESIGN.md §3.19): rbgtopo_place_groups_eligible's inputs, rules and
+ * outputs, plus score / alt_node / alt_score as by rbgtopo_place_groups_lw_ranked, read from the masked rows, so no
+ * alternate lies on a node the pod's role does not admit.  With every mask admitting every installed class all six
+ * outputs are bit-identical to rbgtopo_place_groups_lw_ranked (role_pods given) or rbgtopo_place_groups_ranked
+ * (NULL). */
+int32_t rbgtopo_place_groups_eligible_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                             const int32_t* role_pods, int64_t role_pods_words,
+                                             const uint64_t* role_admit, int64_t n_role_admit, int32_t n_alt,
+                                             int32_t* assign, int32_t* status, int32_t* domain, float* score,
+                                             int32_t* alt_node, float* alt_score);
 
 /* Committed leader-worker batch (DESIGN.md §3.13): rbgtopo_place_groups_lw's inputs, validation, exactness bound,
  * error codes and outputs, with the groups placed in blob order as rbgtopo_place_groups_committed places them.

@@ -45,6 +45,7 @@ SIGNATURES = {
     "rbgtopo_update_nodes": (C.c_int32, [C.c_void_p, i32p, i32p, C.c_uint64]),
     "rbgtopo_update_nodes_delta": (C.c_int32, [C.c_void_p, C.c_int32, i32p, i32p, C.c_uint64]),
     "rbgtopo_set_exclusive_levels": (C.c_int32, [C.c_void_p, C.c_int32, i32p, i32p, C.c_int32, i32p, C.c_uint64]),
+    "rbgtopo_set_node_classes": (C.c_int32, [C.c_void_p, C.c_int32, i32p, C.c_uint64]),
     "rbgtopo_score_assign": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, i32p, i32p]),
     "rbgtopo_place_groups": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, i32p, i32p]),
     "rbgtopo_place_groups_committed": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, i32p, i32p, i32p]),
@@ -59,6 +60,10 @@ SIGNATURES = {
                                                              i32p, i32p, i32p, i32p, f32p, i32p, f32p]),
     "rbgtopo_place_groups_lw_ranked": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, C.c_int64, C.c_int32, i32p, i32p,
                                                    i32p, f32p, i32p, f32p]),
+    "rbgtopo_place_groups_eligible": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, C.c_int64, u64p, C.c_int64, i32p,
+                                                  i32p, i32p]),
+    "rbgtopo_place_groups_eligible_ranked": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, C.c_int64, u64p, C.c_int64,
+                                                         C.c_int32, i32p, i32p, i32p, f32p, i32p, f32p]),
     "rbgtopo_shard_place_groups_ranked": (C.c_int32, [C.c_void_p, i32p, C.c_int64, C.c_int32, i32p, i32p, i32p, i32p,
                                                       C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]),
     "rbgtopo_shard_place_groups_committed_ranked": (C.c_int32, [C.c_void_p, i32p, C.c_int64, C.c_int32, i32p, i32p,

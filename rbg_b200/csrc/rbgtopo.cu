@@ -159,6 +159,10 @@ struct Topology {
   std::vector<int> lvl_nd;                  // [n_levels + 1] domain count of every level (fixed_domain checks)
   std::vector<int> h_lvl_domain;            // [n_levels][n] levels 1..n_levels on the host (co-located alternates)
   DevBuf<int> lvl_domain, lvl_owner, lvl_doff, lvl_tab, occ_rec;
+  // node classes (rbgtopo_set_node_classes, DESIGN.md §3.19): class of every node as u8, zero-padded to 16 B past n
+  // (k_score_emit_elig loads four nodes' classes as one word); n_classes = 0: none installed
+  int n_classes = 0;
+  DevBuf<unsigned char> cls;
 };
 
 struct BatchMeta {
@@ -304,6 +308,7 @@ struct rbgtopo_ctx {
   // update_nodes staging, double buffered: the copy of update k leaves h_free[k & 1]; the host only
   // waits for update k - 2's H2D (long finished) before overwriting it, not for the refresh chain
   PinBuf<int> h_free[2], h_owner[2], h_occ[2];
+  PinBuf<unsigned char> h_cls[2];
   cudaEvent_t stage_ev[2] = {nullptr, nullptr};
   unsigned stage_idx = 0;
   std::mutex stat_mu;
@@ -913,15 +918,19 @@ int launch_emit_plan(rbgtopo_ctx* c, Batch* b, cudaStream_t s, long long n_rows,
 
 // claim_off != nullptr (step batches of rbgtopo_place_groups_lw_committed only): k_score_emit_claims with the owner
 // claims of earlier groups per step (score.cuh).  cm != nullptr (the same call at levels, §3.16):
-// k_score_emit_claims_lv with the group index of every step.
+// k_score_emit_claims_lv with the group index of every step.  admit != nullptr (step batches of
+// rbgtopo_place_groups_eligible[_ranked], §3.19): k_score_emit_elig with MAXP class masks per step.
 int launch_score(rbgtopo_ctx* c, Batch* b, cudaStream_t s, const int* claim_off = nullptr,
-                 const int2* claim_rec = nullptr, const int* step_grp = nullptr, const CommitDev* cm = nullptr) {
+                 const int2* claim_rec = nullptr, const int* step_grp = nullptr, const CommitDev* cm = nullptr,
+                 const unsigned long long* admit = nullptr) {
   const BatchMeta& m = b->m;
   if (m.n_steps == 0) return RBGTOPO_OK;
   if (!b->wave_begin.empty()) return launch_emit_plan(c, b, s, m.total_p);  // multi-wave plan: background rows from the row table
   const int items = (int)emit_items(m.n_steps, c->lc);
   const int grid = items / kEmitBlockSteps;  // one CTA per (block of steps, chunk of nodes)
-  if (cm)
+  if (admit)
+    k_score_emit_elig<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items, c->topo.cls.p, admit);
+  else if (cm)
     k_score_emit_claims_lv<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items, step_grp, *cm);
   else if (claim_off)
     k_score_emit_claims<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items, claim_off, claim_rec, c->topo.occ);
@@ -1608,6 +1617,7 @@ int32_t rbgtopo_set_topology(rbgtopo_ctx* c, int32_t n, int64_t e, const int32_t
   T.occ = false;            // a new topology leaves occupancy mode and drops the levels
   T.n_levels = 0;
   T.lvl_nd.clear();
+  T.n_classes = 0;          // ... and the node classes
   c->delta_repairs = 0;
   int rc = run_base(c, c->topo_stream, true);
   if (rc) return rc;
@@ -1830,6 +1840,48 @@ int32_t rbgtopo_set_exclusive_levels(rbgtopo_ctx* c, int32_t n_levels, const int
   T.generation = generation;
   std::lock_guard<std::mutex> g(c->stat_mu);
   c->launches += n_occ > 0 ? 3 : 2;
+  return RBGTOPO_OK;
+}
+
+// Node classes (DESIGN.md §3.19), ordered like rbgtopo_update_nodes: the copy goes on the refresh stream behind the
+// batches already enqueued (they read the classes they started with) and in front of base_ready / topo_ready, which
+// every later call waits for.  Only a buffer that has to grow waits for the batches in flight.
+int32_t rbgtopo_set_node_classes(rbgtopo_ctx* c, int32_t n_classes, const int32_t* node_class, uint64_t generation) {
+  if (!c) return fail(RBGTOPO_EINVAL, "null ctx");
+  std::unique_lock<std::shared_mutex> lk(c->topo_mu);
+  Topology& T = c->topo;
+  if (!T.valid) return fail(RBGTOPO_ENOTOPO, "set_topology has not been called");
+  if (n_classes > RBGTOPO_MAX_NODE_CLASSES)
+    return fail(RBGTOPO_ELIMIT, "%d node classes (at most %d)", n_classes, RBGTOPO_MAX_NODE_CLASSES);
+  if (n_classes < 1 || !node_class) return fail(RBGTOPO_EINVAL, "n_classes = %d, node_class %p", n_classes, (const void*)node_class);
+  CK(cudaSetDevice(c->cfg.device));
+  cudaStream_t s = c->topo_stream;
+  const size_t need = (size_t)round_up(T.n, 16) + 64;
+  if (T.cls.cap < need) {
+    int frc = fence_batches(c, true);
+    if (frc) return frc;
+    CK(cudaStreamSynchronize(s));
+    CK(T.cls.reserve(need));
+    CK(cudaMemsetAsync(T.cls.p, 0, T.cls.cap, s));
+  } else {
+    int frc = fence_batches(c, false);
+    if (frc) return frc;
+  }
+  const unsigned sb = c->stage_idx++ & 1u;
+  CK(cudaEventSynchronize(c->stage_ev[sb]));
+  CK(c->h_cls[sb].reserve((size_t)T.n));
+  unsigned char* const dst = c->h_cls[sb].p;
+  for (int i = 0; i < T.n; ++i) {
+    const int k = node_class[i];
+    if (k < 0 || k >= n_classes) return fail(RBGTOPO_EINVAL, "node_class[%d] = %d outside [0, %d)", i, k, n_classes);
+    dst[i] = (unsigned char)k;
+  }
+  CK(cudaMemcpyAsync(T.cls.p, dst, (size_t)T.n, cudaMemcpyHostToDevice, s));
+  CK(cudaEventRecord(c->stage_ev[sb], s));
+  CK(cudaEventRecord(c->base_ready, s));
+  CK(cudaEventRecord(c->topo_ready, s));
+  T.n_classes = n_classes;
+  T.generation = generation;
   return RBGTOPO_OK;
 }
 
@@ -4582,13 +4634,20 @@ struct LwRounds {
 // the call.
 // Both: the committed ranked form (§3.15).  The rounds keep no rows (a re-run would keep its rows again); once they
 // converge, rank_committed replays the rows of every group's final run and ranks them after the whole batch.
+// admit != nullptr: the eligible form (§3.19), n_admit class masks, one per role in blob order; every wave's rows are
+// written by k_score_emit_elig with the masks of its role rows, carried after the (S, C) section of the side table.
 int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
                     int32_t* assign, int32_t* status, int32_t* domain, const RankReq* rk = nullptr,
-                    int32_t* rounds = nullptr) {
+                    int32_t* rounds = nullptr, const uint64_t* admit = nullptr, int64_t n_admit = 0) {
   int rc = lw_validate(c, gb, words, rp, rp_words);
   if (rc) return rc;
   const Topology& T = c->topo;
   const int ng = gb[2];
+  if (admit) {
+    if (T.n_classes < 1) return fail(RBGTOPO_EINVAL, "eligible placement: no node classes installed (rbgtopo_set_node_classes)");
+    if (n_admit != rp_words / 2)
+      return fail(RBGTOPO_EINVAL, "role_admit: %lld masks for %lld roles", (long long)n_admit, (long long)(rp_words / 2));
+  }
   std::optional<LwRounds> cr;  // the committed rounds
   if (rounds && (rc = cr.emplace(T, gb).init(c))) return rc;
   const size_t smem = (size_t)((T.n + 31) / 32) * 4;
@@ -4631,6 +4690,16 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
       }
     }
     if (cr) cr->add_side(runs, active, side);
+    const size_t admit_at = side.size();  // admit: MAXP masks per step, 8-byte aligned (MAXP is even)
+    if (admit) {
+      static_assert(MAXP % 2 == 0, "the mask section starts 8-byte aligned");
+      side.resize(admit_at + (size_t)ns * MAXP * 2, 0);
+      for (int i = 0; i < ns; ++i) {
+        const HostRun& r = runs[active[i]];
+        for (int p = 0; p < r.w.n; ++p)
+          memcpy(side.data() + admit_at + 2 * ((size_t)i * MAXP + p), &admit[off.r0[r.g] + r.w.role[p]], 8);
+      }
+    }
     // grid: every step resident at once if the device holds them, the level-C scratch bounded by kLwScratchBytes
     const auto repl_k = !cr ? k_lw_assign_repl<LW_REPL>
                         : cr->at_lv ? k_lw_assign_repl<LW_REPL_CLAIMS_LV> : k_lw_assign_repl<LW_REPL_CLAIMS>;
@@ -4648,7 +4717,11 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
     CK(cudaStreamWaitEvent(s, c->base_ready, 0));  // a pending snapshot refresh
     CK(cudaStreamWaitEvent(s, c->topo_ready, 0));
     if (emit)
-      if (const int r2 = cr ? cr->score(c, b, s, b->lw.p) : launch_score(c, b, s)) return r2;
+      if (const int r2 = cr    ? cr->score(c, b, s, b->lw.p)
+                         : admit ? launch_score(c, b, s, nullptr, nullptr, nullptr, nullptr,
+                                                reinterpret_cast<const unsigned long long*>(b->lw.p + admit_at))
+                                 : launch_score(c, b, s))
+        return r2;
     if (!repl) {
       k_lw_assign<<<(unsigned)grid, LW_THREADS, smem, s>>>(topo_dev(c), batch_dev(c, b), b->lw.p, b->lw_best.p,
                                                            b->lw_cap.p, dmax, lv);
@@ -4697,9 +4770,11 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
 // host-driven re-run.  kPlaceShard (with kPlaceRanked, x != nullptr): the local half of §3.17, valid at any world; the
 // slab lists go to x and the outputs score / alt_node / alt_score are the merge's.
 enum PlaceForm { kPlaceReplicas = 0, kPlaceCommitted = 1, kPlaceLw = 2, kPlaceRanked = 4, kPlaceShard = 8 };
+// admit: the class masks of the eligible forms (§3.19, kPlaceLw only), n_admit of them.
 int32_t place_entry(int form, rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp, int64_t rp_words,
                     int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds, float* score,
-                    int32_t* alt_node, float* alt_score, AltExchange* x = nullptr) {
+                    int32_t* alt_node, float* alt_score, AltExchange* x = nullptr, const uint64_t* admit = nullptr,
+                    int64_t n_admit = 0) {
   const bool committed = form & kPlaceCommitted, lw = form & kPlaceLw, ranked = form & kPlaceRanked;
   const bool shard = form & kPlaceShard;
   if (rounds) *rounds = 0;
@@ -4727,7 +4802,8 @@ int32_t place_entry(int form, rbgtopo_ctx* c, const int32_t* gb, int64_t words, 
   const RankReq* rkp = ranked ? &rk : nullptr;
   if (!lw && !committed) return place_groups_impl(c, gb, words, assign, status, domain, rkp);
   int32_t r = 0;
-  const int rc = lw ? place_groups_lw(c, gb, words, rp, rp_words, assign, status, domain, rkp, committed ? &r : nullptr)
+  const int rc = lw ? place_groups_lw(c, gb, words, rp, rp_words, assign, status, domain, rkp, committed ? &r : nullptr,
+                                     admit, n_admit)
                     : place_groups_committed(c, gb, words, assign, status, domain, &r, rkp);
   if (rounds) *rounds = r;
   return rc;
@@ -4785,6 +4861,48 @@ int32_t rbgtopo_place_groups_lw_committed_ranked(rbgtopo_ctx* c, const int32_t* 
                                                  float* score, int32_t* alt_node, float* alt_score) {
   return place_entry(kPlaceLw | kPlaceCommitted | kPlaceRanked, c, gb, words, role_pods, role_pods_words, n_alt, assign,
                      status, domain, rounds, score, alt_node, alt_score);
+}
+
+// ---- node eligibility (DESIGN.md §3.19) -------------------------------------------------------------------------------
+namespace {
+// The eligible forms: the leader-worker loop with class masks.  role_pods == NULL stands for (S, C) = (1, -1) for every
+// role, which places replicas exactly as rbgtopo_place_groups[_ranked] does.  world > 1 is refused before anything runs.
+int32_t eligible_entry(bool ranked, rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp,
+                       int64_t rp_words, const uint64_t* admit, int64_t n_admit, int32_t n_alt, int32_t* assign,
+                       int32_t* status, int32_t* domain, float* score, int32_t* alt_node, float* alt_score) {
+  if (!c || !gb || !assign || !admit) return fail(RBGTOPO_EINVAL, "null argument");
+  if (c->cfg.world > 1)
+    return fail(RBGTOPO_ELIMIT, "eligible placement needs world == 1: a rank holds only its slab of every dense row");
+  std::vector<int32_t> own_rp;
+  if (!rp) {
+    if (const int hrc = check_groups_blob(gb, words)) return hrc;
+    own_rp.reserve(2);  // non-null data() for a blob without groups
+    for (int g = 0; g < gb[2]; ++g)  // a q outside [1, MAXQ] fails validation before the table is read
+      for (int i = 0, q = std::clamp(group_rec(gb, g)[3], 0, MAXQ); i < q; ++i) {
+        own_rp.push_back(1);
+        own_rp.push_back(-1);
+      }
+    rp = own_rp.data();
+    rp_words = (int64_t)own_rp.size();
+  }
+  return place_entry(kPlaceLw | (ranked ? kPlaceRanked : 0), c, gb, words, rp, rp_words, n_alt, assign, status, domain,
+                     nullptr, score, alt_node, alt_score, nullptr, admit, n_admit);
+}
+}  // namespace
+
+int32_t rbgtopo_place_groups_eligible(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* role_pods,
+                                      int64_t role_pods_words, const uint64_t* role_admit, int64_t n_role_admit,
+                                      int32_t* assign, int32_t* status, int32_t* domain) {
+  return eligible_entry(false, c, gb, words, role_pods, role_pods_words, role_admit, n_role_admit, 0, assign, status,
+                        domain, nullptr, nullptr, nullptr);
+}
+
+int32_t rbgtopo_place_groups_eligible_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* role_pods,
+                                             int64_t role_pods_words, const uint64_t* role_admit, int64_t n_role_admit,
+                                             int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain,
+                                             float* score, int32_t* alt_node, float* alt_score) {
+  return eligible_entry(true, c, gb, words, role_pods, role_pods_words, role_admit, n_role_admit, n_alt, assign, status,
+                        domain, score, alt_node, alt_score);
 }
 
 // ---- ranked alternates on node-axis shards (DESIGN.md §3.17) ---------------------------------------------------------

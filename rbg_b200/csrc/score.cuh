@@ -49,10 +49,16 @@ constexpr int EMIT_MAX_BLOCK = 16;  // upper bound of b.bsteps
 // LV (k_score_emit_claims_lv, a batch with a group at an exclusive level >= 1, DESIGN.md §3.16): no records.  The
 // background pass of an exclusive step reads each node's owner as commit_owner<true> gives it to group
 // step_grp[step] at the step's level (owner_L ⊕ K ⊕ P, the claim lists `cm0` the host built from the previous round).
-template <bool CLAIMS, bool LV = false>
+// ELIG (k_score_emit_elig, rbgtopo_place_groups_eligible[_ranked], DESIGN.md §3.19): node classes.  cls[n] = the class
+// of node n (u8, padded past the last node like free_); admit[step * MAXP + p] = the classes role row p of the step may
+// use.  A node whose class bit is clear counts as having no room (-1) for that row, so its background entry is -inf and
+// the sparse pass, which only adds onto entries or sets them to -inf, keeps it there.
+template <bool CLAIMS, bool LV = false, bool ELIG = false>
 __device__ __forceinline__ void score_emit(TopoDev t, BatchDev b, int items, const int* __restrict__ claim_off,
                                            const int2* __restrict__ claim_rec, bool occ,
-                                           const int* __restrict__ step_grp = nullptr, const CommitDev* cm0 = nullptr) {
+                                           const int* __restrict__ step_grp = nullptr, const CommitDev* cm0 = nullptr,
+                                           const unsigned char* __restrict__ cls = nullptr,
+                                           const unsigned long long* __restrict__ admit = nullptr) {
   const int T = b.chunk, lc = b.lc;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int groups = T >> 2;
@@ -78,9 +84,12 @@ __device__ __forceinline__ void score_emit(TopoDev t, BatchDev b, int items, con
     sDrow[tid] = step_drow(b, step0 + tid, __ldg(hdr + 13));
   }
   __syncthreads();
+  __shared__ unsigned long long sAdmit[ELIG ? EMIT_MAX_BLOCK : 1][ELIG ? MAXP : 1];
   if (tid < nst * MAXP) {
     const int s = tid / MAXP, p = tid - s * MAXP;
     if (p < sH0[s].w) sRoles[s][p] = __ldg(reinterpret_cast<const int4*>(blob + sRoleOff[s]) + p);
+    if constexpr (ELIG)
+      if (p < sH0[s].w) sAdmit[s][p] = __ldg(admit + (size_t)(step0 + s) * MAXP + p);
   }
   __syncthreads();
   {
@@ -139,10 +148,21 @@ __device__ __forceinline__ void score_emit(TopoDev t, BatchDev b, int items, con
           if (!(ow.w == -1 || ow.w == gid)) avx.w = -1;
         }
         float* rowp = mrow0 + (g << 2);
+        // ELIG: the classes of the group's four nodes, one per byte (n % 4 == 0, padded: safe).  Loaded per step
+        // (L1-hot after the first) rather than held across the step loop, which would cost two more live registers.
+        unsigned cls4 = 0;
+        if constexpr (ELIG) cls4 = __ldg(reinterpret_cast<const unsigned*>(cls + n0 + (g << 2)));
         for (int p = 0; p < P; ++p) {
           const int4 role = roles[p];  // count demand need flags
           const float need = (float)role.z;
-          const int4 a = (role.w & RBGTOPO_ROLE_EXCLUSIVE) ? avx : av[j];
+          int4 a = (role.w & RBGTOPO_ROLE_EXCLUSIVE) ? avx : av[j];
+          if constexpr (ELIG) {
+            const unsigned long long m = sAdmit[si][p];
+            if (!((m >> (cls4 & 0xFF)) & 1)) a.x = -1;
+            if (!((m >> ((cls4 >> 8) & 0xFF)) & 1)) a.y = -1;
+            if (!((m >> ((cls4 >> 16) & 0xFF)) & 1)) a.z = -1;
+            if (!((m >> (cls4 >> 24)) & 1)) a.w = -1;
+          }
           float4 o4;
           o4.x = a.x >= role.y ? need * base4[j].x : -INFINITY;
           o4.y = a.y >= role.y ? need * base4[j].y : -INFINITY;
@@ -242,6 +262,14 @@ k_score_emit_claims(TopoDev t, BatchDev b, int items, const int* __restrict__ cl
 __global__ void __launch_bounds__(SCORE_THREADS, 6)
 k_score_emit_claims_lv(TopoDev t, BatchDev b, int items, const int* __restrict__ step_grp, CommitDev cm) {
   score_emit<true, true>(t, b, items, nullptr, nullptr, true, step_grp, &cm);
+}
+
+// rbgtopo_place_groups_eligible[_ranked] (DESIGN.md §3.19): the waves of the leader-worker loop with node classes;
+// admit = the mask section of the wave's side table, MAXP entries per step.
+__global__ void __launch_bounds__(SCORE_THREADS, 6)
+k_score_emit_elig(TopoDev t, BatchDev b, int items, const unsigned char* __restrict__ cls,
+                  const unsigned long long* __restrict__ admit) {
+  score_emit<false, false, true>(t, b, items, nullptr, nullptr, false, nullptr, nullptr, cls, admit);
 }
 
 }  // namespace rbgtopo

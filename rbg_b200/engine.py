@@ -85,6 +85,8 @@ class TopoPlacer:
         self.places_lw_committed_ranked = True  # place_groups_lw_committed_ranked: alternates of committed LW batches (§3.15)
         # place_groups[_committed]_ranked_sharded: ranked alternates on node-axis shards, any world (§3.17)
         self.places_sharded_ranked = True
+        # set_node_classes + place_groups_eligible[_ranked]: node eligibility per role (§3.19), world = 1 only
+        self.places_eligible = world == 1
         h = C.c_void_p()
         self._h = None
         # blob totals of every live staged handle (fetch sizes its outputs from them); created here, not on the first
@@ -152,6 +154,15 @@ class TopoPlacer:
         self._check(self.lib.rbgtopo_set_exclusive_levels(self._h, n_levels, _p(lv), _p(nd), len(occ), _p(occ),
                                                           generation))
         self._n_levels = n_levels
+
+    def set_node_classes(self, node_class, n_classes: int = None, generation: int = 0) -> None:
+        """Node classes (DESIGN.md §3.19): node_class[n] in [0, n_classes) for every node (n_classes defaults to the
+        largest class + 1).  Read only by place_groups_eligible[_ranked]; set_topology drops them."""
+        cls = _i32(node_class)
+        if self.n_nodes and len(cls) != self.n_nodes:   # no topology yet: the library answers RBGTOPO_ENOTOPO
+            raise ValueError(f"node_class has {len(cls)} entries for {self.n_nodes} nodes")
+        k = int(n_classes) if n_classes is not None else (int(cls.max()) + 1 if len(cls) else 0)
+        self._check(self.lib.rbgtopo_set_node_classes(self._h, k, _p(cls), generation))
 
     # -- hot path, host buffers in/out
     def score_assign(self, blob: np.ndarray) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
@@ -311,6 +322,42 @@ class TopoPlacer:
         self._check(self.lib.rbgtopo_place_groups_lw_ranked(
             self._h, _p(gb), len(gb), _p(rp), len(rp), int(n_alt), _p(assign), _p(status), _p(domain),
             _p(score, _lib.f32p), _p(alt_node) if n_alt > 0 else None, _p(alt_score, _lib.f32p) if n_alt > 0 else None))
+        return assign[:pods], status[:ng], domain[:ng], score[:pods], alt_node[:pods], alt_score[:pods]
+
+    def _eligible_args(self, groups_blob, role_pods, role_admit):
+        gb = _i32(groups_blob)
+        rp = None if role_pods is None else _i32(np.asarray(role_pods, dtype=np.int64).reshape(-1))
+        admit = np.ascontiguousarray(np.asarray(role_admit, dtype=np.uint64).reshape(-1))
+        pods = int(gb[4]) if rp is None else self._lw_pods(gb, rp)
+        return gb, rp, admit, int(gb[2]), pods
+
+    def place_groups_eligible(self, groups_blob: np.ndarray, role_pods, role_admit):
+        """place_groups_lw with node eligibility (DESIGN.md §3.19): role_admit holds one uint64 class mask per role of
+        every group in blob order; a role places pods only on nodes whose class bit is set.  role_pods None: one pod
+        per replica, no co-location (assign in place_groups order).  Returns (assign, status, domain)."""
+        gb, rp, admit, ng, pods = self._eligible_args(groups_blob, role_pods, role_admit)
+        assign = np.empty(max(pods, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        self._check(self.lib.rbgtopo_place_groups_eligible(
+            self._h, _p(gb), len(gb), _p(rp), 0 if rp is None else len(rp), _p(admit, _lib.u64p), len(admit),
+            _p(assign), _p(status), _p(domain)))
+        return assign[:pods], status[:ng], domain[:ng]
+
+    def place_groups_eligible_ranked(self, groups_blob: np.ndarray, role_pods, role_admit, n_alt: int):
+        """place_groups_eligible plus ranked alternates per pod (§3.19, as place_groups_lw_ranked): returns (assign,
+        status, domain, score, alt_node, alt_score); no alternate lies on a node the pod's role does not admit."""
+        gb, rp, admit, ng, pods = self._eligible_args(groups_blob, role_pods, role_admit)
+        assign = np.empty(max(pods, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        score = np.empty(max(pods, 1), dtype=np.float32)
+        alt_node = np.empty((max(pods, 1), max(n_alt, 0)), dtype=np.int32)
+        alt_score = np.empty((max(pods, 1), max(n_alt, 0)), dtype=np.float32)
+        self._check(self.lib.rbgtopo_place_groups_eligible_ranked(
+            self._h, _p(gb), len(gb), _p(rp), 0 if rp is None else len(rp), _p(admit, _lib.u64p), len(admit),
+            int(n_alt), _p(assign), _p(status), _p(domain), _p(score, _lib.f32p),
+            _p(alt_node) if n_alt > 0 else None, _p(alt_score, _lib.f32p) if n_alt > 0 else None))
         return assign[:pods], status[:ng], domain[:ng], score[:pods], alt_node[:pods], alt_score[:pods]
 
     # -- staged (device-resident) batches

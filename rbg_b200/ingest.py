@@ -15,6 +15,7 @@ duplicate-free CSR with sorted rows — what rbgtopo_set_topology validates.
 """
 from __future__ import annotations
 
+import re
 from dataclasses import dataclass, field
 from typing import Dict, List, Mapping, Optional, Sequence, Tuple
 
@@ -43,6 +44,7 @@ class NodeInfo:
     allocatable: Mapping[str, int] = field(default_factory=dict)   # resource -> count
     requested: Mapping[str, int] = field(default_factory=dict)     # summed over the node's pods
     unschedulable: bool = False                                    # spec.unschedulable / not Ready
+    taints: Sequence[Mapping[str, str]] = ()                       # spec.taints: {key, value, effect}
 
 
 @dataclass
@@ -197,3 +199,129 @@ def exclusive_occupancy(levels: ExclusiveLevels, index: NodeIndex,
         out.append((pos[node], int(gid), levels.keys.index(key)))
     out.sort()
     return np.asarray(out, dtype=np.int32).reshape(-1, 3)
+
+
+# ---- node classes (DESIGN.md §3.19) ----------------------------------------------------------------------------------
+# Only these taint effects keep a pod off a node; PreferNoSchedule is a preference and is ignored.
+HARD_TAINT_EFFECTS = ("NoSchedule", "NoExecute")
+MAX_NODE_CLASSES = 64   # RBGTOPO_MAX_NODE_CLASSES
+
+
+@dataclass
+class NodeClasses:
+    """Classes for rbgtopo_set_node_classes: node_class[n] (node ids of `index`), and per class the values of the
+    configured label keys (a missing label is absent) and its NoSchedule / NoExecute taints as (key, value, effect)."""
+    keys: Tuple[str, ...]
+    node_class: np.ndarray                       # [n] int32
+    labels: List[Dict[str, str]]
+    taints: List[Tuple[Tuple[str, str, str], ...]]
+
+    @property
+    def n_classes(self) -> int:
+        return len(self.labels)
+
+
+class NotDecidable(ValueError):
+    """A selector the classes cannot decide (a label key outside the configured keys, or matchFields): the group
+    gets no hint."""
+
+
+def build_node_classes(nodes: Sequence[NodeInfo], index: NodeIndex, keys: Sequence[str]) -> NodeClasses:
+    """Nodes with the same values of `keys` and the same hard taints share a class.  Classes are numbered by first
+    appearance over the name-sorted nodes of `index`, so the result does not depend on informer order.  More than
+    RBGTOPO_MAX_NODE_CLASSES (64) classes is an error."""
+    by_name = {nd.name: nd for nd in nodes}
+    if set(by_name) != set(index.names):
+        raise ValueError("node set changed: rebuild the topology")
+    ids: Dict[tuple, int] = {}
+    cls = np.zeros(len(index.names), dtype=np.int32)
+    for n, nm in enumerate(index.names):
+        nd = by_name[nm]
+        lab = tuple((k, nd.labels[k]) for k in keys if k in nd.labels)
+        tnt = tuple(sorted({(t.get("key", ""), t.get("value", ""), t.get("effect", "")) for t in nd.taints
+                            if t.get("effect", "") in HARD_TAINT_EFFECTS}))
+        cls[n] = ids.setdefault((lab, tnt), len(ids))
+    if len(ids) > MAX_NODE_CLASSES:
+        raise ValueError(f"{len(ids)} node classes exceed {MAX_NODE_CLASSES}: configure fewer label keys")
+    return NodeClasses(tuple(keys), cls, [dict(lab) for lab, _ in ids], [tnt for _, tnt in ids])
+
+
+
+def tolerates(tol: Mapping[str, str], taint: Tuple[str, str, str]) -> bool:
+    """corev1 Toleration.ToleratesTaint: an empty effect matches every effect, an empty key every key; operator
+    Exists matches any value, Equal (or empty) the same value."""
+    key, value, effect = taint
+    if tol.get("effect", "") and tol.get("effect") != effect:
+        return False
+    if tol.get("key", "") and tol.get("key") != key:
+        return False
+    op = tol.get("operator", "") or "Equal"
+    if op == "Exists":
+        return True
+    return op == "Equal" and tol.get("value", "") == value
+
+
+_INT64 = re.compile(r"[+-]?[0-9]+")
+
+
+def _int(s) -> Optional[int]:
+    """Go's strconv.ParseInt(s, 10, 64): an optional sign and decimal digits only (no spaces, no underscores), within
+    int64; None otherwise."""
+    s = str(s)
+    if not _INT64.fullmatch(s):
+        return None
+    v = int(s)
+    return v if -(1 << 63) <= v < (1 << 63) else None
+
+
+def _expr_matches(expr: Mapping, labels: Mapping[str, str]) -> bool:
+    key, op, values = expr["key"], expr["operator"], list(expr.get("values", ()))
+    has = key in labels
+    if op == "In":
+        return has and labels[key] in values
+    if op == "NotIn":
+        return not has or labels[key] not in values
+    if op == "Exists":
+        return has
+    if op == "DoesNotExist":
+        return not has
+    if op in ("Gt", "Lt"):
+        if not has or len(values) != 1:
+            return False
+        a, b = _int(labels[key]), _int(values[0])
+        if a is None or b is None:
+            return False
+        return a > b if op == "Gt" else a < b
+    raise ValueError(f"node selector operator {op!r}")
+
+
+def role_admit(classes: NodeClasses, node_selector: Mapping[str, str] = None, node_affinity: Sequence[Mapping] = (),
+               tolerations: Sequence[Mapping[str, str]] = ()) -> int:
+    """The class mask of a pod template (bit c: class c admits it), as kube-scheduler's NodeAffinity and
+    TaintToleration filters decide: every nodeSelector pair matches, one of the required node-affinity terms
+    (node_affinity: the nodeSelectorTerms, ORed; empty = no requirement) has all its matchExpressions match, and every
+    NoSchedule / NoExecute taint of the class is tolerated.  Raises NotDecidable for a key outside classes.keys or a
+    term with matchFields."""
+    node_selector = node_selector or {}
+    keys = set(classes.keys)
+    for k in node_selector:
+        if k not in keys:
+            raise NotDecidable(f"nodeSelector key {k!r} is not a configured class key")
+    for term in node_affinity:
+        if term.get("matchFields"):
+            raise NotDecidable("node affinity matchFields cannot be decided per class")
+        for e in term.get("matchExpressions", ()):
+            if e["key"] not in keys:
+                raise NotDecidable(f"node affinity key {e['key']!r} is not a configured class key")
+    mask = 0
+    for c in range(classes.n_classes):
+        lab = classes.labels[c]
+        if any(lab.get(k) != v for k, v in node_selector.items()):
+            continue
+        if node_affinity and not any(term.get("matchExpressions") and
+                                     all(_expr_matches(e, lab) for e in term["matchExpressions"])
+                                     for term in node_affinity):
+            continue
+        if all(any(tolerates(t, taint) for t in tolerations) for taint in classes.taints[c]):
+            mask |= 1 << c
+    return mask

@@ -27,7 +27,7 @@ import ctypes as C
 import json
 import logging
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Dict, List, Mapping, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -35,6 +35,7 @@ from . import _lib
 from .blob import (MAX_STEP_REPLICAS, MAX_STEP_ROLES, NEED_CAP, ROLE_EXCLUSIVE, STEP_EXCLUSIVE, STEP_GANG,
                    BlobBuilder, Group, GroupsBuilder, Step)
 from .engine import TopoPlacer
+from .ingest import NodeClasses, NotDecidable, role_admit
 
 RBG_PREFIX = "rbg.workloads.x-k8s.io/"                       # api/workloads/constants
 EXCLUSIVE_TOPOLOGY_KEY = RBG_PREFIX + "group-exclusive-topology"   # annotation.go:25
@@ -58,6 +59,11 @@ class RoleSpec:
     demand: int = 1                      # accelerator slots per replica (new input)
     lws_size: int = 0                    # LeaderWorkerPattern.Size, 0 = not LWS
     annotations: Dict[str, str] = field(default_factory=dict)
+    # the pod template's node eligibility (DESIGN.md §3.19): spec.nodeSelector, the nodeSelectorTerms of
+    # affinity.nodeAffinity.requiredDuringSchedulingIgnoredDuringExecution (empty: none), spec.tolerations
+    node_selector: Dict[str, str] = field(default_factory=dict)
+    node_affinity: Sequence[Mapping] = ()
+    tolerations: Sequence[Mapping[str, str]] = ()
 
 
 @dataclass
@@ -297,7 +303,7 @@ class B200TopoPodGroupManager:
 
     def __init__(self, placer: TopoPlacer, inner: Optional[str] = "scheduler-plugins",
                  exclusive_keys: Optional[Sequence[str]] = None, alternates: int = 0, leader_worker: bool = False,
-                 all_gather=None):
+                 all_gather=None, node_classes: Optional[NodeClasses] = None):
         """inner: the gang plugin this manager wraps for the PodGroup CR and the pod-group label —
         "scheduler-plugins" (kube), "volcano" or None (the Go manager takes the implementation object).
         exclusive_keys: the topology keys exclusive groups may name (DESIGN.md §3.9), keys[0] = the level-0 label.
@@ -340,7 +346,15 @@ class B200TopoPodGroupManager:
         alternates, such a group is placed through rbgtopo_place_groups_lw_ranked (§3.12) when the placer has
         `places_lw_ranked`, and its alternates are keyed by pod name and stay inside each replica's co-location
         domain; a placer without it gives no hint for such a group.
-        False (default): those groups are placed as before, one pod per replica."""
+        False (default): those groups are placed as before, one pod per replica.
+        node_classes: the classes installed on the placer (ingest.build_node_classes, then
+        placer.set_node_classes(node_classes.node_class, node_classes.n_classes)); DESIGN.md §3.19.  A group with a role
+        whose pod template excludes an installed class (ingest.role_admit over its nodeSelector, required node
+        affinity and tolerations) is placed through rbgtopo_place_groups_eligible (_ranked with alternates), a
+        leader-worker group with its (S, C) table and pod-keyed hints, so no hint or alternate lands on a node the role
+        cannot run on.  Such a group gets no hint and a logged reason in a committed batch, on a placer with world > 1
+        or without `places_eligible`, and so does a group whose selector the classes cannot decide.  Every other group
+        is placed exactly as without node_classes.  None (default): eligibility is not looked at."""
         if not 0 <= alternates <= 8:
             raise ValueError(f"alternates must be in [0, 8], got {alternates}")
         self.alternates = int(alternates)
@@ -352,6 +366,7 @@ class B200TopoPodGroupManager:
         self.all_gather = all_gather
         self.no_hint: Dict[Tuple[str, str], str] = {}
         self._hints: Dict[Tuple[str, str], Placement] = {}
+        self.node_classes = node_classes
 
     def exclusive_level(self, rbg: RoleBasedGroup, committed: bool = False) -> Tuple[int, str]:
         """(level of the group's exclusive key, reason for no hint or "")."""
@@ -378,13 +393,52 @@ class B200TopoPodGroupManager:
                 and (getattr(self.placer, "places_lw_committed_levels", False)
                      or not any(self.exclusive_level(r, True)[0] > 0 for r in rbgs)))
 
-    def _split_no_hint(self, rbgs: Sequence[RoleBasedGroup], committed: bool = False):
+    def role_masks(self, rbg: RoleBasedGroup) -> Tuple[List[int], str]:
+        """(class mask per role in spec order, reason for no hint or "") under node_classes (DESIGN.md §3.19)."""
+        try:
+            return [role_admit(self.node_classes, r.node_selector, r.node_affinity, r.tolerations)
+                    for r in rbg.roles], ""
+        except NotDecidable as e:
+            return [], f"node eligibility: {e}"
+
+    def is_restricted(self, rbg: RoleBasedGroup) -> bool:
+        """A role's pod template excludes an installed node class (or cannot be decided per class): the group is
+        placed by rbgtopo_place_groups_eligible, or gets no hint."""
+        if self.node_classes is None:
+            return False
+        masks, reason = self.role_masks(rbg)
+        full = (1 << self.node_classes.n_classes) - 1
+        return bool(reason) or any(m & full != full for m in masks)
+
+    def _eligibility_reason(self, rbg: RoleBasedGroup, committed: bool, waves: bool) -> str:
+        """Why a restricted group gets no hint, or ""."""
+        if not self.is_restricted(rbg):
+            return ""
+        reason = self.role_masks(rbg)[1]
+        if reason:
+            return reason
+        if committed:
+            return "node eligibility: committed batches place no node classes"
+        if waves:
+            return "node eligibility: the step-batch path places no node classes"
+        if getattr(self.placer, "world", 1) > 1:
+            return "node eligibility: placers with world > 1 place no node classes"
+        if not getattr(self.placer, "places_eligible", False):
+            return "node eligibility: the placer has no rbgtopo_place_groups_eligible"
+        return ""
+
+    def _split_no_hint(self, rbgs: Sequence[RoleBasedGroup], committed: bool = False, waves: bool = False):
         """The groups that get a hint, and a no-hint Placement per group that does not (logged, hint dropped)."""
         keep, skipped = [], {}
         lw_commit = self.lw_committed(rbgs, committed)
         for i, r in enumerate(rbgs):
             _, reason = self.exclusive_level(r, committed)
-            if not reason and self.is_leader_worker(r):
+            if not reason:
+                reason = self._eligibility_reason(r, committed, waves)
+            if not reason and self.is_restricted(r):   # placed by the eligible call, which ranks for every group
+                if self.is_leader_worker(r):
+                    reason = self.role_pods(r)[1]
+            elif not reason and self.is_leader_worker(r):
                 if committed and not lw_commit:
                     reason = "leader-worker replicas: committed batches place one pod per replica"
                 elif self.alternates and not getattr(self.placer, "places_lw_ranked", False):
@@ -481,9 +535,27 @@ class B200TopoPodGroupManager:
             else:
                 assign, status, domain, _ = self.placer.place_groups_lw_committed(blob, role_pods)
             return self._merge(all_rbgs, self._placements(runs, assign, status, domain, alt_node, pods), skipped)
-        lw = [i for i, r in enumerate(rbgs) if self.is_leader_worker(r)]
-        plain = [i for i, r in enumerate(rbgs) if not self.is_leader_worker(r)]
+        elig = [i for i, r in enumerate(rbgs) if self.is_restricted(r)]
+        lw = [i for i, r in enumerate(rbgs) if self.is_leader_worker(r) and i not in elig]
+        plain = [i for i, r in enumerate(rbgs) if not self.is_leader_worker(r) and i not in elig]
         done: List[Optional[Placement]] = [None] * len(rbgs)   # by position in rbgs
+        if elig:   # DESIGN.md §3.19: masks in blob order, (S, C) when a leader-worker group is among them
+            blob, runs = self.groups_blob([rbgs[i] for i in elig])
+            masks = [self.role_masks(g.rbg)[0] for g in runs]
+            role_admit_ = [masks[k][ri] for k, g in enumerate(runs) for ri in g.order]
+            pods = None
+            if any(self.is_leader_worker(g.rbg) for g in runs):
+                pods = [self.role_pods(g.rbg)[0] if self.is_leader_worker(g.rbg) else [(1, -1)] * len(g.rbg.roles)
+                        for g in runs]
+            role_pods = None if pods is None else [pods[k][ri] for k, g in enumerate(runs) for ri in g.order]
+            alt_node = None
+            if self.alternates > 0:
+                assign, status, domain, _, alt_node, _ = self.placer.place_groups_eligible_ranked(
+                    blob, role_pods, role_admit_, self.alternates)
+            else:
+                assign, status, domain = self.placer.place_groups_eligible(blob, role_pods, role_admit_)
+            for i, p in zip(elig, self._placements(runs, assign, status, domain, alt_node, pods)):
+                done[i] = p
         if plain:
             blob, runs = self.groups_blob([rbgs[i] for i in plain])
             alt_node = None
@@ -550,7 +622,7 @@ class B200TopoPodGroupManager:
     #    kept as the readable mirror of the C++ loop and for cross-checks.
     def reconcile_pod_groups_by_waves(self, rbgs: Sequence[RoleBasedGroup]) -> List[Placement]:
         all_rbgs = rbgs
-        rbgs, skipped = self._split_no_hint(rbgs)
+        rbgs, skipped = self._split_no_hint(rbgs, waves=True)
         runs = [_GroupRun(r, self.arith, excl_level=self.exclusive_level(r)[0]) for r in rbgs]
         n_nodes = self.placer.n_nodes
         w = 0
