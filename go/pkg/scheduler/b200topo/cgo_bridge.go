@@ -152,6 +152,29 @@ static int32_t rbgtopo_go_place_groups_eligible_ranked(rbgtopo_ctx* ctx, const i
   rbgtopo_go_err(ctx, rc, err);
   return rc;
 }
+static int32_t rbgtopo_go_place_groups_eligible_committed(rbgtopo_ctx* ctx, const int32_t* groups, int64_t words,
+                                                          const int32_t* role_pods, int64_t role_pods_words,
+                                                          const uint64_t* role_admit, int64_t n_role_admit,
+                                                          int32_t* assign, int32_t* status, int32_t* domain,
+                                                          int32_t* rounds, char* err) {
+  int32_t rc = rbgtopo_place_groups_eligible_committed(ctx, groups, words, role_pods, role_pods_words, role_admit,
+                                                       n_role_admit, assign, status, domain, rounds);
+  rbgtopo_go_err(ctx, rc, err);
+  return rc;
+}
+static int32_t rbgtopo_go_place_groups_eligible_committed_ranked(rbgtopo_ctx* ctx, const int32_t* groups,
+                                                                 int64_t words, const int32_t* role_pods,
+                                                                 int64_t role_pods_words, const uint64_t* role_admit,
+                                                                 int64_t n_role_admit, int32_t n_alt, int32_t* assign,
+                                                                 int32_t* status, int32_t* domain, int32_t* rounds,
+                                                                 float* score, int32_t* alt_node, float* alt_score,
+                                                                 char* err) {
+  int32_t rc = rbgtopo_place_groups_eligible_committed_ranked(ctx, groups, words, role_pods, role_pods_words,
+                                                              role_admit, n_role_admit, n_alt, assign, status, domain,
+                                                              rounds, score, alt_node, alt_score);
+  rbgtopo_go_err(ctx, rc, err);
+  return rc;
+}
 */
 import "C"
 
@@ -381,6 +404,48 @@ func (p *placer) placeGroupsLWCommitted(blob, rolePods []int32, nPods int) (assi
 		return nil, nil, nil, 0, err
 	}
 	return assign[:nPods], status[:nGroups], domain[:nGroups], int32(r), nil
+}
+
+// placeGroupsEligibleCommitted: placeGroupsEligible as a committed batch (DESIGN.md §3.20): the groups in blob order,
+// each seeing the pods and exclusive domains the groups before it took, every role on the nodes its class mask
+// admits.  rolePods nil: one pod per replica, no co-location.  rounds = wave-loop rounds the library ran.
+func (p *placer) placeGroupsEligibleCommitted(blob, rolePods []int32, roleAdmit []uint64, nPods int) (assign, status, domain []int32, rounds int32, err error) {
+	nGroups := int(blob[2])
+	assign = make([]int32, max(nPods, 1))
+	status = make([]int32, max(nGroups, 1))
+	domain = make([]int32, max(nGroups, 1))
+	var r C.int32_t
+	var buf [C.RBGTOPO_GO_ERRLEN]C.char
+	rc := C.rbgtopo_go_place_groups_eligible_committed(p.ctx, p32(blob), C.int64_t(len(blob)), p32(rolePods),
+		C.int64_t(len(rolePods)), pu64(roleAdmit), C.int64_t(len(roleAdmit)), p32(assign), p32(status), p32(domain),
+		&r, &buf[0])
+	if err = mkErr(rc, &buf); err != nil {
+		return nil, nil, nil, 0, err
+	}
+	return assign[:nPods], status[:nGroups], domain[:nGroups], int32(r), nil
+}
+
+// placeGroupsEligibleCommittedRanked: placeGroupsEligibleCommitted plus, per pod, up to nAlt next-best nodes as
+// placeGroupsLWCommittedRanked ranks them, read from the masked rows: no alternate lies on a node the pod's role does
+// not admit.
+func (p *placer) placeGroupsEligibleCommittedRanked(blob, rolePods []int32, roleAdmit []uint64, nPods, nAlt int) (assign, status, domain, altNode []int32, rounds int32, err error) {
+	nGroups := int(blob[2])
+	assign = make([]int32, max(nPods, 1))
+	status = make([]int32, max(nGroups, 1))
+	domain = make([]int32, max(nGroups, 1))
+	score := make([]float32, max(nPods, 1))
+	altNode = make([]int32, max(nPods*nAlt, 1))
+	altScore := make([]float32, max(nPods*nAlt, 1))
+	var r C.int32_t
+	var buf [C.RBGTOPO_GO_ERRLEN]C.char
+	rc := C.rbgtopo_go_place_groups_eligible_committed_ranked(p.ctx, p32(blob), C.int64_t(len(blob)), p32(rolePods),
+		C.int64_t(len(rolePods)), pu64(roleAdmit), C.int64_t(len(roleAdmit)), C.int32_t(nAlt), p32(assign),
+		p32(status), p32(domain), &r, (*C.float)(unsafe.Pointer(&score[0])), p32(altNode),
+		(*C.float)(unsafe.Pointer(&altScore[0])), &buf[0])
+	if err = mkErr(rc, &buf); err != nil {
+		return nil, nil, nil, nil, 0, err
+	}
+	return assign[:nPods], status[:nGroups], domain[:nGroups], altNode[:nPods*nAlt], int32(r), nil
 }
 
 // placeGroupsLWRanked: placeGroupsLW plus, per pod, up to nAlt next-best nodes that still have room once its group is

@@ -574,6 +574,36 @@ int32_t rbgtopo_place_groups_lw_committed_ranked(rbgtopo_ctx* ctx, const int32_t
                                                  int32_t* assign, int32_t* status, int32_t* domain, int32_t* rounds,
                                                  float* score, int32_t* alt_node, float* alt_score);
 
+/* Node eligibility in a committed batch (DESIGN.md §3.20).  The groups are placed in blob order; group g is placed
+ * exactly as a one-group rbgtopo_place_groups_eligible call would place it, except that earlier groups' pods consume
+ * capacity and their reported exclusive domains are claimed, as in rbgtopo_place_groups_lw_committed (map or
+ * occupancy mode; at levels >= 1, on a ctx with RBGTOPO_CFG_LW_COMMIT_LEVELS, the K / P rule of §3.16).  Every row of
+ * every round carries §3.19's class term: role rho may not use node n when bit node_class[n] of admit_rho is clear.
+ * The term does not depend on claims, so rounds, the exactness bound and the limits are those of
+ * rbgtopo_place_groups_lw_committed.  role_admit / role_pods as rbgtopo_place_groups_eligible (role_pods NULL: (S, C)
+ * = (1, -1) for every role).  Errors: rbgtopo_place_groups_eligible's (RBGTOPO_EINVAL for role_admit NULL or of the
+ * wrong length, or no classes installed; RBGTOPO_ELIMIT at world > 1) and rbgtopo_place_groups_lw_committed's, every
+ * one before anything is placed, with *rounds = 0.  With every mask admitting every installed class the outputs are
+ * bit-identical to rbgtopo_place_groups_lw_committed's, *rounds included (role_pods given), or, with role_pods NULL,
+ * assign / status / domain are rbgtopo_place_groups_committed's. */
+int32_t rbgtopo_place_groups_eligible_committed(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                                const int32_t* role_pods, int64_t role_pods_words,
+                                                const uint64_t* role_admit, int64_t n_role_admit, int32_t* assign,
+                                                int32_t* status, int32_t* domain, int32_t* rounds);
+
+/* Ranked alternates of an eligible committed batch (DESIGN.md §3.20): rbgtopo_place_groups_eligible_committed's
+ * inputs, checks and outputs, plus score / alt_node / alt_score as by rbgtopo_place_groups_lw_committed_ranked, read
+ * from the masked rows of every group's final run, so no alternate lies on a node the pod's role does not admit.  With
+ * every mask admitting every installed class, all outputs are bit-identical to
+ * rbgtopo_place_groups_lw_committed_ranked's (role_pods given), or every output but *rounds to
+ * rbgtopo_place_groups_committed_ranked's (role_pods NULL). */
+int32_t rbgtopo_place_groups_eligible_committed_ranked(rbgtopo_ctx* ctx, const int32_t* groups, int64_t groups_words,
+                                                       const int32_t* role_pods, int64_t role_pods_words,
+                                                       const uint64_t* role_admit, int64_t n_role_admit, int32_t n_alt,
+                                                       int32_t* assign, int32_t* status, int32_t* domain,
+                                                       int32_t* rounds, float* score, int32_t* alt_node,
+                                                       float* alt_score);
+
 /* rbgtopo_place_groups pipeline, staged: the groups are compiled into a
  * device-resident multi-wave plan (one step blob, wave-major, expanded on the
  * device), so rbgtopo_run_staged runs ONE score launch for the dense rows of every

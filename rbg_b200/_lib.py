@@ -64,6 +64,11 @@ SIGNATURES = {
                                                   i32p, i32p]),
     "rbgtopo_place_groups_eligible_ranked": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, C.c_int64, u64p, C.c_int64,
                                                          C.c_int32, i32p, i32p, i32p, f32p, i32p, f32p]),
+    "rbgtopo_place_groups_eligible_committed": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, C.c_int64, u64p,
+                                                            C.c_int64, i32p, i32p, i32p, i32p]),
+    "rbgtopo_place_groups_eligible_committed_ranked": (C.c_int32, [C.c_void_p, i32p, C.c_int64, i32p, C.c_int64, u64p,
+                                                                   C.c_int64, C.c_int32, i32p, i32p, i32p, i32p, f32p,
+                                                                   i32p, f32p]),
     "rbgtopo_shard_place_groups_ranked": (C.c_int32, [C.c_void_p, i32p, C.c_int64, C.c_int32, i32p, i32p, i32p, i32p,
                                                       C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]),
     "rbgtopo_shard_place_groups_committed_ranked": (C.c_int32, [C.c_void_p, i32p, C.c_int64, C.c_int32, i32p, i32p,

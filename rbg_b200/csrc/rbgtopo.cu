@@ -919,7 +919,9 @@ int launch_emit_plan(rbgtopo_ctx* c, Batch* b, cudaStream_t s, long long n_rows,
 // claim_off != nullptr (step batches of rbgtopo_place_groups_lw_committed only): k_score_emit_claims with the owner
 // claims of earlier groups per step (score.cuh).  cm != nullptr (the same call at levels, §3.16):
 // k_score_emit_claims_lv with the group index of every step.  admit != nullptr (step batches of
-// rbgtopo_place_groups_eligible[_ranked], §3.19): k_score_emit_elig with MAXP class masks per step.
+// rbgtopo_place_groups_eligible[_ranked], §3.19): k_score_emit_elig with MAXP class masks per step; with claim_off or
+// cm as well (rbgtopo_place_groups_eligible_committed[_ranked], §3.20): k_score_emit_claims[_lv]_elig.  The claims are
+// tested first: masks alone must never stand in for a committed wave's owner claims.
 int launch_score(rbgtopo_ctx* c, Batch* b, cudaStream_t s, const int* claim_off = nullptr,
                  const int2* claim_rec = nullptr, const int* step_grp = nullptr, const CommitDev* cm = nullptr,
                  const unsigned long long* admit = nullptr) {
@@ -928,12 +930,19 @@ int launch_score(rbgtopo_ctx* c, Batch* b, cudaStream_t s, const int* claim_off 
   if (!b->wave_begin.empty()) return launch_emit_plan(c, b, s, m.total_p);  // multi-wave plan: background rows from the row table
   const int items = (int)emit_items(m.n_steps, c->lc);
   const int grid = items / kEmitBlockSteps;  // one CTA per (block of steps, chunk of nodes)
-  if (admit)
-    k_score_emit_elig<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items, c->topo.cls.p, admit);
+  const unsigned char* cls = c->topo.cls.p;
+  if (cm && admit)
+    k_score_emit_claims_lv_elig<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items, step_grp, *cm, cls,
+                                                               admit);
   else if (cm)
     k_score_emit_claims_lv<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items, step_grp, *cm);
+  else if (claim_off && admit)
+    k_score_emit_claims_elig<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items, claim_off, claim_rec,
+                                                            c->topo.occ, cls, admit);
   else if (claim_off)
     k_score_emit_claims<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items, claim_off, claim_rec, c->topo.occ);
+  else if (admit)
+    k_score_emit_elig<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items, cls, admit);
   else
     k_score_emit<<<grid, SCORE_THREADS, 0, s>>>(topo_dev(c), batch_dev(c, b), items);  // step batch: rows + sparse corrections
   return RBGTOPO_OK;
@@ -3946,10 +3955,15 @@ int exact_one_pod(rbgtopo_ctx* c, const int32_t* gb, int64_t words) {
 // in `cm`.  A batch whose rows exceed kReplayBytes is scored and ranked in chunks of steps.  status / domain not null.
 // rp != nullptr: a committed leader-worker batch (§3.15): the (S, C) table of place_groups_lw, pod waves (next_wave),
 // role counts, `need`, anchors and rows in pods; hc: its owner claims (HostClaims).
+// admit != nullptr: the eligible committed form (§3.20), one class mask per role in blob order.  Every replayed step
+// carries the masks of its role rows (MAXP per step, in staging order, uploaded per chunk into b->lw, which the rounds
+// no longer need) and is scored by k_score_emit_elig: the class -inf does not depend on claims, so the replayed rows
+// equal the masked rows of the final run at every entry the ranking reads.  b->h_lw is rewritten only once the
+// previous chunk's copy has completed (run_alternates ends in a stream synchronise; a later chunk checks it again).
 constexpr long long kReplayBytes = 1LL << 30;
 int rank_committed(rbgtopo_ctx* c, Batch* b, const int32_t* gb, const int32_t* rp, const int32_t* assign,
                    const int32_t* status, const int32_t* domain, const CommitDev& cm, bool lv, const RankReq& rk,
-                   int* launches, const HostClaims* hc = nullptr) {
+                   int* launches, const HostClaims* hc = nullptr, const uint64_t* admit = nullptr) {
   const int ng = gb[2];
   const GroupOffsets off(gb, rp);
   alt_clear(rk, 0, off.pod0[ng]);
@@ -3958,16 +3972,27 @@ int rank_committed(rbgtopo_ctx* c, Batch* b, const int32_t* gb, const int32_t* r
   const int max_rows = (int)std::max<long long>(RBGTOPO_MAX_STEP_ROLES, kReplayBytes / 4 / c->slab_stride);
   StepBlob sb;
   std::vector<AltRow> list;
-  int rc = RBGTOPO_OK;
+  std::vector<uint64_t> masks;  // admit: MAXP per staged step
+  int rc = RBGTOPO_OK, chunks = 0;
   auto flush = [&]() -> int {
     if (sb.ns == 0) return RBGTOPO_OK;
     const std::vector<int32_t>& blob = sb.build();
     int r2 = stage_into(c, b, blob.data(), (int64_t)blob.size());
-    if (!r2) r2 = launch_score(c, b, s);
+    if (!r2 && admit) {
+      if (chunks++ > 0) CK(cudaStreamSynchronize(s));  // already drained by run_alternates: never waits in practice
+      const size_t w = masks.size() * 2;
+      CK(b->lw.reserve(w));
+      CK(b->h_lw.reserve(w));
+      memcpy(b->h_lw.p, masks.data(), w * 4);
+      CK(cudaMemcpyAsync(b->lw.p, b->h_lw.p, w * 4, cudaMemcpyHostToDevice, s));
+    }
+    if (!r2) r2 = launch_score(c, b, s, nullptr, nullptr, nullptr, nullptr,
+                               admit ? reinterpret_cast<const unsigned long long*>(b->lw.p) : nullptr);
     if (!r2) r2 = run_alternates(c, b, b->matrix.p, list, gb, rp, assign, status, domain, rk, &cm, lv, hc);
     *launches += 2;
     sb.clear();
     list.clear();
+    masks.clear();
     return r2;
   };
   for (int g = 0; g < ng && !rc; ++g) {
@@ -3990,6 +4015,10 @@ int rank_committed(rbgtopo_ctx* c, Batch* b, const int32_t* gb, const int32_t* r
           if (placed) list.push_back(AltRow{sb.rowacc + p, g, w.role[p], (int)first(p), pods});
         }
         sb.add(r, w, 0, -1, 0, false, nullptr, 0);
+        if (admit) {
+          masks.resize(masks.size() + MAXP, 0);
+          for (int p = 0; p < w.n; ++p) masks[masks.size() - MAXP + p] = admit[off.r0[g] + w.role[p]];
+        }
       }
       for (int p = 0; p < w.n; ++p)  // the wave's placements: anchors of the later waves
         for (int k = 0; k < w.count[p] * r.S(w.role[p]); ++k) {
@@ -4553,10 +4582,11 @@ struct LwRounds {
     rec_at = side.size();
     for (int i : active) side.insert(side.end(), runs[i].owner_claims.begin(), runs[i].owner_claims.end());
   }
-  // The wave's dense rows, with the owner claims of the earlier groups (lw: the side table on the device).
-  int score(rbgtopo_ctx* c, Batch* b, cudaStream_t s, const int* lw) const {
-    return at_lv ? launch_score(c, b, s, nullptr, nullptr, lw + sec_at, &cm)
-                 : launch_score(c, b, s, lw + sec_at, reinterpret_cast<const int2*>(lw + rec_at));
+  // The wave's dense rows, with the owner claims of the earlier groups (lw: the side table on the device; admit: its
+  // mask section in the eligible form, §3.20).
+  int score(rbgtopo_ctx* c, Batch* b, cudaStream_t s, const int* lw, const unsigned long long* admit) const {
+    return at_lv ? launch_score(c, b, s, nullptr, nullptr, lw + sec_at, &cm, admit)
+                 : launch_score(c, b, s, lw + sec_at, reinterpret_cast<const int2*>(lw + rec_at), nullptr, nullptr, admit);
   }
   // The end of a round: the new claims of the groups it ran.  c = the lowest group whose claims changed; groups <= c
   // saw their final input.  Returns whether another round is needed; it starts at c + 1.
@@ -4596,8 +4626,9 @@ struct LwRounds {
   // group's final claims, the lists of commit_owner<true> at levels, and at level 0 the owner lists of
   // commit_owner<false> (HostClaims), which are LwLists' dhead / dclaim.  What the claim lists took (k_set_heads
   // launches, uploaded words) counts toward a call that succeeds.
+  // admit: the class masks of the eligible form (§3.20), which the replay applies to its rows.
   int finish(rbgtopo_ctx* c, Batch* b, int rc, const int32_t* rp, const int32_t* assign, const int32_t* status,
-             const int32_t* domain, const RankReq* rk, rbgtopo_timing& total) {
+             const int32_t* domain, const RankReq* rk, rbgtopo_timing& total, const uint64_t* admit) {
     int rank_launches = 0;
     if (!rc && rk) {
       HostClaims hc;
@@ -4612,7 +4643,8 @@ struct LwRounds {
       }
       cm.g = ng;
       if (!rc)
-        rc = rank_committed(c, b, gb, rp, assign, status, domain, cm, at_lv, *rk, &rank_launches, at_lv ? nullptr : &hc);
+        rc = rank_committed(c, b, gb, rp, assign, status, domain, cm, at_lv, *rk, &rank_launches, at_lv ? nullptr : &hc,
+                            admit);
     }
     std::lock_guard<std::mutex> g(c->stat_mu);
     total.launches += rank_launches;
@@ -4690,9 +4722,12 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
       }
     }
     if (cr) cr->add_side(runs, active, side);
-    const size_t admit_at = side.size();  // admit: MAXP masks per step, 8-byte aligned (MAXP is even)
+    // admit: MAXP masks per step, read as u64.  The (S, C) section is even (MAXP is); the claim section at levels is
+    // one int per step, so an odd step count is padded to an even word here.
+    static_assert(MAXP % 2 == 0, "the (S, C) section ends 8-byte aligned");
+    if (admit && (side.size() & 1)) side.push_back(0);
+    const size_t admit_at = side.size();
     if (admit) {
-      static_assert(MAXP % 2 == 0, "the mask section starts 8-byte aligned");
       side.resize(admit_at + (size_t)ns * MAXP * 2, 0);
       for (int i = 0; i < ns; ++i) {
         const HostRun& r = runs[active[i]];
@@ -4716,11 +4751,10 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
     CK(cudaMemcpyAsync(b->lw.p, b->h_lw.p, side.size() * 4, cudaMemcpyHostToDevice, s));
     CK(cudaStreamWaitEvent(s, c->base_ready, 0));  // a pending snapshot refresh
     CK(cudaStreamWaitEvent(s, c->topo_ready, 0));
+    const auto* adm = admit ? reinterpret_cast<const unsigned long long*>(b->lw.p + admit_at) : nullptr;
     if (emit)
-      if (const int r2 = cr    ? cr->score(c, b, s, b->lw.p)
-                         : admit ? launch_score(c, b, s, nullptr, nullptr, nullptr, nullptr,
-                                                reinterpret_cast<const unsigned long long*>(b->lw.p + admit_at))
-                                 : launch_score(c, b, s))
+      if (const int r2 = cr ? cr->score(c, b, s, b->lw.p, adm)
+                            : launch_score(c, b, s, nullptr, nullptr, nullptr, nullptr, adm))
         return r2;
     if (!repl) {
       k_lw_assign<<<(unsigned)grid, LW_THREADS, smem, s>>>(topo_dev(c), batch_dev(c, b), b->lw.p, b->lw_best.p,
@@ -4754,7 +4788,7 @@ int place_groups_lw(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int3
   }
   if (cr) {
     *rounds = cr->n_rounds;
-    rc = cr->finish(c, b, rc, rp, assign, status, domain, rk, total);
+    rc = cr->finish(c, b, rc, rp, assign, status, domain, rk, total, admit);
   }
   if (!rc) harvest_base_ms(c);
   // The waves record no pass events, so their pass times are 0, unless the pooled batch still holds those of a staged
@@ -4867,9 +4901,12 @@ int32_t rbgtopo_place_groups_lw_committed_ranked(rbgtopo_ctx* c, const int32_t* 
 namespace {
 // The eligible forms: the leader-worker loop with class masks.  role_pods == NULL stands for (S, C) = (1, -1) for every
 // role, which places replicas exactly as rbgtopo_place_groups[_ranked] does.  world > 1 is refused before anything runs.
-int32_t eligible_entry(bool ranked, rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp,
+// committed (§3.20): the committed leader-worker rounds with the same masks; rounds as rbgtopo_place_groups_lw_committed.
+int32_t eligible_entry(bool committed, bool ranked, rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* rp,
                        int64_t rp_words, const uint64_t* admit, int64_t n_admit, int32_t n_alt, int32_t* assign,
-                       int32_t* status, int32_t* domain, float* score, int32_t* alt_node, float* alt_score) {
+                       int32_t* status, int32_t* domain, int32_t* rounds, float* score, int32_t* alt_node,
+                       float* alt_score) {
+  if (rounds) *rounds = 0;
   if (!c || !gb || !assign || !admit) return fail(RBGTOPO_EINVAL, "null argument");
   if (c->cfg.world > 1)
     return fail(RBGTOPO_ELIMIT, "eligible placement needs world == 1: a rank holds only its slab of every dense row");
@@ -4885,24 +4922,43 @@ int32_t eligible_entry(bool ranked, rbgtopo_ctx* c, const int32_t* gb, int64_t w
     rp = own_rp.data();
     rp_words = (int64_t)own_rp.size();
   }
-  return place_entry(kPlaceLw | (ranked ? kPlaceRanked : 0), c, gb, words, rp, rp_words, n_alt, assign, status, domain,
-                     nullptr, score, alt_node, alt_score, nullptr, admit, n_admit);
+  return place_entry(kPlaceLw | (committed ? kPlaceCommitted : 0) | (ranked ? kPlaceRanked : 0), c, gb, words, rp,
+                     rp_words, n_alt, assign, status, domain, rounds, score, alt_node, alt_score, nullptr, admit,
+                     n_admit);
 }
 }  // namespace
 
 int32_t rbgtopo_place_groups_eligible(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* role_pods,
                                       int64_t role_pods_words, const uint64_t* role_admit, int64_t n_role_admit,
                                       int32_t* assign, int32_t* status, int32_t* domain) {
-  return eligible_entry(false, c, gb, words, role_pods, role_pods_words, role_admit, n_role_admit, 0, assign, status,
-                        domain, nullptr, nullptr, nullptr);
+  return eligible_entry(false, false, c, gb, words, role_pods, role_pods_words, role_admit, n_role_admit, 0, assign,
+                        status, domain, nullptr, nullptr, nullptr, nullptr);
 }
 
 int32_t rbgtopo_place_groups_eligible_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words, const int32_t* role_pods,
                                              int64_t role_pods_words, const uint64_t* role_admit, int64_t n_role_admit,
                                              int32_t n_alt, int32_t* assign, int32_t* status, int32_t* domain,
                                              float* score, int32_t* alt_node, float* alt_score) {
-  return eligible_entry(true, c, gb, words, role_pods, role_pods_words, role_admit, n_role_admit, n_alt, assign, status,
-                        domain, score, alt_node, alt_score);
+  return eligible_entry(false, true, c, gb, words, role_pods, role_pods_words, role_admit, n_role_admit, n_alt, assign,
+                        status, domain, nullptr, score, alt_node, alt_score);
+}
+
+int32_t rbgtopo_place_groups_eligible_committed(rbgtopo_ctx* c, const int32_t* gb, int64_t words,
+                                                const int32_t* role_pods, int64_t role_pods_words,
+                                                const uint64_t* role_admit, int64_t n_role_admit, int32_t* assign,
+                                                int32_t* status, int32_t* domain, int32_t* rounds) {
+  return eligible_entry(true, false, c, gb, words, role_pods, role_pods_words, role_admit, n_role_admit, 0, assign,
+                        status, domain, rounds, nullptr, nullptr, nullptr);
+}
+
+int32_t rbgtopo_place_groups_eligible_committed_ranked(rbgtopo_ctx* c, const int32_t* gb, int64_t words,
+                                                       const int32_t* role_pods, int64_t role_pods_words,
+                                                       const uint64_t* role_admit, int64_t n_role_admit, int32_t n_alt,
+                                                       int32_t* assign, int32_t* status, int32_t* domain,
+                                                       int32_t* rounds, float* score, int32_t* alt_node,
+                                                       float* alt_score) {
+  return eligible_entry(true, true, c, gb, words, role_pods, role_pods_words, role_admit, n_role_admit, n_alt, assign,
+                        status, domain, rounds, score, alt_node, alt_score);
 }
 
 // ---- ranked alternates on node-axis shards (DESIGN.md §3.17) ---------------------------------------------------------

@@ -52,7 +52,9 @@ constexpr int EMIT_MAX_BLOCK = 16;  // upper bound of b.bsteps
 // ELIG (k_score_emit_elig, rbgtopo_place_groups_eligible[_ranked], DESIGN.md §3.19): node classes.  cls[n] = the class
 // of node n (u8, padded past the last node like free_); admit[step * MAXP + p] = the classes role row p of the step may
 // use.  A node whose class bit is clear counts as having no room (-1) for that row, so its background entry is -inf and
-// the sparse pass, which only adds onto entries or sets them to -inf, keeps it there.
+// the sparse pass, which only adds onto entries or sets them to -inf, keeps it there.  With CLAIMS as well
+// (k_score_emit_claims[_lv]_elig, rbgtopo_place_groups_eligible_committed[_ranked], DESIGN.md §3.20): LV masks after
+// commit_owner like any other owner; the level-0 rewrite of claimed nodes tests the class bit too.
 template <bool CLAIMS, bool LV = false, bool ELIG = false>
 __device__ __forceinline__ void score_emit(TopoDev t, BatchDev b, int items, const int* __restrict__ claim_off,
                                            const int2* __restrict__ claim_rec, bool occ,
@@ -184,9 +186,17 @@ __device__ __forceinline__ void score_emit(TopoDev t, BatchDev b, int items, con
             const int ow = occ ? owner_merge(__ldg(t.node_owner + m), cl.y) : cl.y;
             const int a = (ow == -1 || ow == gid) ? __ldg(t.free_ + m) : -1;
             const float bm = __ldg(t.base + m);
-            for (int p = 0; p < P; ++p)
-              if (roles[p].w & RBGTOPO_ROLE_EXCLUSIVE)
-                mrow0[(size_t)p * stride + (m - n0)] = a >= roles[p].y ? (float)roles[p].z * bm : -INFINITY;
+            if constexpr (ELIG) {  // the rewrite must not turn a class-excluded node back into a finite entry
+              const unsigned k = __ldg(cls + m);
+              for (int p = 0; p < P; ++p)
+                if (roles[p].w & RBGTOPO_ROLE_EXCLUSIVE)
+                  mrow0[(size_t)p * stride + (m - n0)] =
+                      a >= roles[p].y && ((sAdmit[si][p] >> k) & 1) ? (float)roles[p].z * bm : -INFINITY;
+            } else {
+              for (int p = 0; p < P; ++p)
+                if (roles[p].w & RBGTOPO_ROLE_EXCLUSIVE)
+                  mrow0[(size_t)p * stride + (m - n0)] = a >= roles[p].y ? (float)roles[p].z * bm : -INFINITY;
+            }
           }
           __syncthreads();  // ... and the consumed and anchor passes follow it
         }
@@ -270,6 +280,22 @@ __global__ void __launch_bounds__(SCORE_THREADS, 6)
 k_score_emit_elig(TopoDev t, BatchDev b, int items, const unsigned char* __restrict__ cls,
                   const unsigned long long* __restrict__ admit) {
   score_emit<false, false, true>(t, b, items, nullptr, nullptr, false, nullptr, nullptr, cls, admit);
+}
+
+// rbgtopo_place_groups_eligible_committed[_ranked] (DESIGN.md §3.20): k_score_emit_claims with node classes (a batch at
+// level 0) ...
+__global__ void __launch_bounds__(SCORE_THREADS, 6)
+k_score_emit_claims_elig(TopoDev t, BatchDev b, int items, const int* __restrict__ claim_off,
+                         const int2* __restrict__ claim_rec, bool occ, const unsigned char* __restrict__ cls,
+                         const unsigned long long* __restrict__ admit) {
+  score_emit<true, false, true>(t, b, items, claim_off, claim_rec, occ, nullptr, nullptr, cls, admit);
+}
+
+// ... and k_score_emit_claims_lv with node classes (a batch with a group at a level >= 1).
+__global__ void __launch_bounds__(SCORE_THREADS, 6)
+k_score_emit_claims_lv_elig(TopoDev t, BatchDev b, int items, const int* __restrict__ step_grp, CommitDev cm,
+                            const unsigned char* __restrict__ cls, const unsigned long long* __restrict__ admit) {
+  score_emit<true, true, true>(t, b, items, nullptr, nullptr, true, step_grp, &cm, cls, admit);
 }
 
 }  // namespace rbgtopo

@@ -87,6 +87,8 @@ class TopoPlacer:
         self.places_sharded_ranked = True
         # set_node_classes + place_groups_eligible[_ranked]: node eligibility per role (§3.19), world = 1 only
         self.places_eligible = world == 1
+        # place_groups_eligible_committed[_ranked]: node eligibility in committed batches (§3.20), world = 1 only
+        self.places_eligible_committed = world == 1
         h = C.c_void_p()
         self._h = None
         # blob totals of every live staged handle (fetch sizes its outputs from them); created here, not on the first
@@ -359,6 +361,39 @@ class TopoPlacer:
             int(n_alt), _p(assign), _p(status), _p(domain), _p(score, _lib.f32p),
             _p(alt_node) if n_alt > 0 else None, _p(alt_score, _lib.f32p) if n_alt > 0 else None))
         return assign[:pods], status[:ng], domain[:ng], score[:pods], alt_node[:pods], alt_score[:pods]
+
+    def place_groups_eligible_committed(self, groups_blob: np.ndarray, role_pods, role_admit):
+        """place_groups_eligible as a committed batch (DESIGN.md §3.20): in blob order, each group sees the pods and
+        the exclusive domains the groups before it took, and every role stays on the nodes its mask admits.  Returns
+        (assign, status, domain, wave-loop rounds run)."""
+        gb, rp, admit, ng, pods = self._eligible_args(groups_blob, role_pods, role_admit)
+        assign = np.empty(max(pods, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        rounds = C.c_int32()
+        self._check(self.lib.rbgtopo_place_groups_eligible_committed(
+            self._h, _p(gb), len(gb), _p(rp), 0 if rp is None else len(rp), _p(admit, _lib.u64p), len(admit),
+            _p(assign), _p(status), _p(domain), C.byref(rounds)))
+        return assign[:pods], status[:ng], domain[:ng], rounds.value
+
+    def place_groups_eligible_committed_ranked(self, groups_blob: np.ndarray, role_pods, role_admit, n_alt: int):
+        """place_groups_eligible_committed plus ranked alternates per pod (§3.20, as place_groups_lw_committed_ranked):
+        returns (assign, status, domain, rounds, score, alt_node, alt_score); no alternate lies on a node the pod's
+        role does not admit."""
+        gb, rp, admit, ng, pods = self._eligible_args(groups_blob, role_pods, role_admit)
+        assign = np.empty(max(pods, 1), dtype=np.int32)
+        status = np.empty(max(ng, 1), dtype=np.int32)
+        domain = np.empty(max(ng, 1), dtype=np.int32)
+        rounds = C.c_int32()
+        score = np.empty(max(pods, 1), dtype=np.float32)
+        alt_node = np.empty((max(pods, 1), max(n_alt, 0)), dtype=np.int32)
+        alt_score = np.empty((max(pods, 1), max(n_alt, 0)), dtype=np.float32)
+        self._check(self.lib.rbgtopo_place_groups_eligible_committed_ranked(
+            self._h, _p(gb), len(gb), _p(rp), 0 if rp is None else len(rp), _p(admit, _lib.u64p), len(admit),
+            int(n_alt), _p(assign), _p(status), _p(domain), C.byref(rounds), _p(score, _lib.f32p),
+            _p(alt_node) if n_alt > 0 else None, _p(alt_score, _lib.f32p) if n_alt > 0 else None))
+        return (assign[:pods], status[:ng], domain[:ng], rounds.value, score[:pods], alt_node[:pods],
+                alt_score[:pods])
 
     # -- staged (device-resident) batches
     def stage(self, blob: np.ndarray) -> int:

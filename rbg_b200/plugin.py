@@ -107,6 +107,7 @@ class RoleBasedGroup:
 
 
 RBGTOPO_NO_HINT = -1   # Placement.status of a group the manager gives no hint (B200TopoPodGroupManager.no_hint)
+ALL_CLASSES = (1 << 64) - 1   # the class mask of a role that admits every node class (DESIGN.md §3.19)
 
 
 @dataclass
@@ -352,9 +353,12 @@ class B200TopoPodGroupManager:
         whose pod template excludes an installed class (ingest.role_admit over its nodeSelector, required node
         affinity and tolerations) is placed through rbgtopo_place_groups_eligible (_ranked with alternates), a
         leader-worker group with its (S, C) table and pod-keyed hints, so no hint or alternate lands on a node the role
-        cannot run on.  Such a group gets no hint and a logged reason in a committed batch, on a placer with world > 1
-        or without `places_eligible`, and so does a group whose selector the classes cannot decide.  Every other group
-        is placed exactly as without node_classes.  None (default): eligibility is not looked at."""
+        cannot run on.  A committed batch holding such a group goes through rbgtopo_place_groups_eligible_committed
+        (§3.20) on a placer with `places_eligible_committed` (see reconcile_pod_groups).  Such a group gets no hint and
+        a logged reason in a committed batch on a placer without that call or whose levels it cannot place, on a
+        placer with world > 1 or without `places_eligible`, on the step-batch path, and so does a group whose
+        selector the classes cannot decide.  Every other group is placed exactly as without node_classes.  None
+        (default): eligibility is not looked at."""
         if not 0 <= alternates <= 8:
             raise ValueError(f"alternates must be in [0, 8], got {alternates}")
         self.alternates = int(alternates)
@@ -393,6 +397,18 @@ class B200TopoPodGroupManager:
                 and (getattr(self.placer, "places_lw_committed_levels", False)
                      or not any(self.exclusive_level(r, True)[0] > 0 for r in rbgs)))
 
+    def eligible_committed(self, rbgs: Sequence[RoleBasedGroup], committed: bool) -> bool:
+        """A committed batch placed by one rbgtopo_place_groups_eligible_committed call (DESIGN.md §3.20): it holds a
+        restricted group that gets a hint (its selectors decided, its exclusive key placeable), the placer places
+        such batches (`places_eligible_committed`, world == 1), and it has no group at an exclusive level >= 1 unless
+        the placer places those in committed leader-worker batches (`places_lw_committed_levels`), as lw_committed."""
+        return (committed and getattr(self.placer, "places_eligible_committed", False)
+                and getattr(self.placer, "world", 1) == 1
+                and any(self.is_restricted(r) and not self.role_masks(r)[1] and not self.exclusive_level(r, True)[1]
+                        for r in rbgs)
+                and (getattr(self.placer, "places_lw_committed_levels", False)
+                     or not any(self.exclusive_level(r, True)[0] > 0 for r in rbgs)))
+
     def role_masks(self, rbg: RoleBasedGroup) -> Tuple[List[int], str]:
         """(class mask per role in spec order, reason for no hint or "") under node_classes (DESIGN.md §3.19)."""
         try:
@@ -410,14 +426,15 @@ class B200TopoPodGroupManager:
         full = (1 << self.node_classes.n_classes) - 1
         return bool(reason) or any(m & full != full for m in masks)
 
-    def _eligibility_reason(self, rbg: RoleBasedGroup, committed: bool, waves: bool) -> str:
-        """Why a restricted group gets no hint, or ""."""
+    def _eligibility_reason(self, rbg: RoleBasedGroup, committed: bool, waves: bool, elig_commit: bool = False) -> str:
+        """Why a restricted group gets no hint, or "".  elig_commit: the committed batch goes through
+        rbgtopo_place_groups_eligible_committed (eligible_committed)."""
         if not self.is_restricted(rbg):
             return ""
         reason = self.role_masks(rbg)[1]
         if reason:
             return reason
-        if committed:
+        if committed and not elig_commit:
             return "node eligibility: committed batches place no node classes"
         if waves:
             return "node eligibility: the step-batch path places no node classes"
@@ -430,12 +447,13 @@ class B200TopoPodGroupManager:
     def _split_no_hint(self, rbgs: Sequence[RoleBasedGroup], committed: bool = False, waves: bool = False):
         """The groups that get a hint, and a no-hint Placement per group that does not (logged, hint dropped)."""
         keep, skipped = [], {}
-        lw_commit = self.lw_committed(rbgs, committed)
+        elig_commit = not waves and self.eligible_committed(rbgs, committed)
+        lw_commit = elig_commit or self.lw_committed(rbgs, committed)
         for i, r in enumerate(rbgs):
             _, reason = self.exclusive_level(r, committed)
             if not reason:
-                reason = self._eligibility_reason(r, committed, waves)
-            if not reason and self.is_restricted(r):   # placed by the eligible call, which ranks for every group
+                reason = self._eligibility_reason(r, committed, waves, elig_commit)
+            if not reason and (self.is_restricted(r) or elig_commit):   # the eligible calls rank for every group
                 if self.is_leader_worker(r):
                     reason = self.role_pods(r)[1]
             elif not reason and self.is_leader_worker(r):
@@ -514,12 +532,35 @@ class B200TopoPodGroupManager:
         passes the groups ordered by namespaced name).  With alternates, a committed batch of one-pod replicas gets
         them from place_groups_committed_ranked (§3.14) when the placer has `places_committed_ranked`: room and
         exclusive claims counted after the whole batch.  A committed batch with leader-worker groups gets them from
-        place_groups_lw_committed_ranked (§3.15) when the placer has `places_lw_committed_ranked`."""
+        place_groups_lw_committed_ranked (§3.15) when the placer has `places_lw_committed_ranked`.  A committed batch
+        that holds a group restricted by node_classes goes through ONE place_groups_eligible_committed call (_ranked
+        with alternates, §3.20) when the placer has `places_eligible_committed` and every group's level is placeable
+        (as for lw_committed): every role carries its class mask (all ones for unrestricted groups), role_pods is
+        given only when a leader-worker group is in the batch, and the hints of leader-worker groups are keyed by pod
+        name.  The restricted groups' claims then count for the groups after them too."""
         all_rbgs = rbgs
+        elig_commit = self.eligible_committed(rbgs, committed)
         lw_commit = self.lw_committed(rbgs, committed)
         rbgs, skipped = self._split_no_hint(rbgs, committed)
         if not rbgs:
             return self._merge(all_rbgs, [], skipped)
+        if elig_commit:   # one call in the given order, with node eligibility for every role
+            blob, runs = self.groups_blob(rbgs)
+            masks = [self.role_masks(g.rbg)[0] if self.is_restricted(g.rbg) else [ALL_CLASSES] * len(g.rbg.roles)
+                     for g in runs]
+            role_admit_ = [masks[k][ri] for k, g in enumerate(runs) for ri in g.order]
+            pods = None
+            if any(self.is_leader_worker(g.rbg) for g in runs):
+                pods = [self.role_pods(g.rbg)[0] if self.is_leader_worker(g.rbg) else [(1, -1)] * len(g.rbg.roles)
+                        for g in runs]
+            role_pods = None if pods is None else [pods[k][ri] for k, g in enumerate(runs) for ri in g.order]
+            alt_node = None
+            if self.alternates > 0:
+                assign, status, domain, _, _, alt_node, _ = self.placer.place_groups_eligible_committed_ranked(
+                    blob, role_pods, role_admit_, self.alternates)
+            else:
+                assign, status, domain, _ = self.placer.place_groups_eligible_committed(blob, role_pods, role_admit_)
+            return self._merge(all_rbgs, self._placements(runs, assign, status, domain, alt_node, pods), skipped)
         if lw_commit:   # one call in the given order: every group sees what the groups before it took
             blob, runs = self.groups_blob(rbgs)
             pods = [self.role_pods(g.rbg)[0] if self.is_leader_worker(g.rbg) else [(1, -1)] * len(g.rbg.roles)
